@@ -1338,6 +1338,12 @@ __global__ void __launch_bounds__(256) k_input_conv(InConvArgs a) {
     }
 }
 
+// dynamic shared memory of k_input_conv: weights [3*k*k][C] + bias [C] + the u8 normalisation table [3][256]
+constexpr int INCONV_SMEM_MAX = 226 * 1024;
+inline size_t input_conv_smem_bytes(int kernel, int c8) {
+    return sizeof(float) * ((size_t)3 * kernel * kernel * c8 * 8 + (size_t)c8 * 8 + 3 * 256);
+}
+
 __global__ void k_f32_to_bf16(const float* in, __nv_bfloat16* out, long long n) {
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
         out[i] = __float2bfloat16_rn(in[i]);
@@ -1708,6 +1714,15 @@ int pifpaf_net_create(pifpaf_net_t** out, int32_t device, int32_t max_batch) {
     PIFPAF_CUDA_TRY(cudaFuncSetAttribute(k_dw_gemm<1, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024));
     PIFPAF_CUDA_TRY(cudaFuncSetAttribute(k_dw_gemm<1, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024));
     PIFPAF_CUDA_TRY(cudaFuncSetAttribute(k_dw_gemm<1, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024));
+    // the stem stages its weights in shared memory: 7x7 with more than 72 channels is past the default 48 KB
+    PIFPAF_CUDA_TRY(cudaFuncSetAttribute(k_input_conv<1, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, INCONV_SMEM_MAX));
+    PIFPAF_CUDA_TRY(cudaFuncSetAttribute(k_input_conv<3, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, INCONV_SMEM_MAX));
+    PIFPAF_CUDA_TRY(cudaFuncSetAttribute(k_input_conv<5, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, INCONV_SMEM_MAX));
+    PIFPAF_CUDA_TRY(cudaFuncSetAttribute(k_input_conv<7, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, INCONV_SMEM_MAX));
+    PIFPAF_CUDA_TRY(cudaFuncSetAttribute(k_input_conv<1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, INCONV_SMEM_MAX));
+    PIFPAF_CUDA_TRY(cudaFuncSetAttribute(k_input_conv<3, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, INCONV_SMEM_MAX));
+    PIFPAF_CUDA_TRY(cudaFuncSetAttribute(k_input_conv<5, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, INCONV_SMEM_MAX));
+    PIFPAF_CUDA_TRY(cudaFuncSetAttribute(k_input_conv<7, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, INCONV_SMEM_MAX));
     *out = net;
     return PIFPAF_OK;
 }
@@ -1741,6 +1756,8 @@ int pifpaf_net_input_conv(pifpaf_net_t* net, int32_t in_h, int32_t in_w, int32_t
     const int ho = (in_h + 2 * pad - kernel) / stride + 1, wo = (in_w + 2 * pad - kernel) / stride + 1;
     PIFPAF_CHECK_ARG(to.h == ho && to.w == wo && to.c >= pad8(c_out), "output tensor shape mismatch");
     PIFPAF_CHECK_ARG(kernel == 1 || kernel == 3 || kernel == 5 || kernel == 7, "input conv kernel must be 1, 3, 5 or 7");
+    PIFPAF_CHECK_ARG(c_out >= 1 && input_conv_smem_bytes(kernel, pad8(c_out) / 8) <= (size_t)INCONV_SMEM_MAX,
+                     "input conv: the weights of a kxk conv with this many output channels do not fit in shared memory");
     PIFPAF_CUDA_TRY(cudaSetDevice(net->device));
     const int C = pad8(c_out);
     std::vector<float> w((size_t)3 * kernel * kernel * C, 0.f), b(C, 0.f);
@@ -2176,7 +2193,7 @@ static int net_forward_impl(pifpaf_net_t* net, const float* images_dev, int32_t 
             a.in = images_dev; a.B = batch;
             const long long total = (long long)batch * a.Hout * a.Wout;
             const int grid = (int)std::min<long long>((total + 255) / 256, (long long)n_sm * 16);
-            const size_t smem = sizeof(float) * ((size_t)3 * a.kernel * a.kernel * a.C8 * 8 + a.C8 * 8 + 3 * 256);
+            const size_t smem = input_conv_smem_bytes(a.kernel, a.C8);
             if (u8 != nullptr) {
                 a.in_u8 = u8->images;
                 for (int c = 0; c < 3; c++) { a.mean[c] = u8->mean[c]; a.stdev[c] = u8->stdev[c]; }

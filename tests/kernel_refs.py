@@ -1,0 +1,200 @@
+"""Float64 references of the network ops of libpifpaf_b200 (include/pifpaf_b200.h), with the error bound a correct
+kernel must meet.  Pure numpy; tests/test_kernel_refs.py checks them against torch in float64, tests/test_kernels_gpu.py
+compares every kernel with them.
+
+Bound of one bf16 output (f32 accumulation of K products, then round to nearest even):
+    |got - ref| <= 2^-8 |ref| + (K + 2) 2^-23 (sum |a w| + |b| + |res|)
+the first term is the output rounding (half a bf16 ulp), the second the f32 accumulation (tensor-core adds may
+truncate: a full f32 ulp per add).  Outputs kept in f32 (the heads) have no rounding term."""
+import numpy as np
+
+U_BF16 = 2.0 ** -8          # unit roundoff of bf16 (8-bit significand)
+U_F32 = 2.0 ** -23          # one f32 ulp (relative)
+SENTINEL = -12288.0         # exact in bf16 (-1.5 * 2^13); no op of the tests produces it
+OP_RAW, OP_SIGMOID, OP_ADD_X, OP_ADD_Y, OP_SOFTPLUS = 0, 1, 2, 3, 4
+
+
+def bf16_round(a):
+    """float -> nearest bf16 value (ties to even), as float32."""
+    a = np.ascontiguousarray(a, dtype=np.float32)
+    u = a.view(np.uint32).astype(np.uint64)
+    u = ((u + 0x7fff + ((u >> 16) & 1)) >> 16) << 16
+    return u.astype(np.uint32).view(np.float32)
+
+
+def bf16_truncate(a):
+    """float -> bf16 by dropping the low 16 bits (rounding toward zero); only to show what the bound rejects."""
+    a = np.ascontiguousarray(a, dtype=np.float32)
+    return (a.view(np.uint32) & np.uint32(0xffff0000)).view(np.float32)
+
+
+def random_bf16(rng, shape, scale=1.0):
+    return bf16_round(rng.standard_normal(shape) * scale)
+
+
+def out_hw(h, w, kernel, stride, pad):
+    return (h + 2 * pad - kernel) // stride + 1, (w + 2 * pad - kernel) // stride + 1
+
+
+def conv_ref(x, w, b, stride, pad, groups=1):
+    """x [B, H, W, C] (NHWC), w [N, C / groups, k, k] (torch layout), b [N] or None
+    -> (y, mag): y = conv + b in float64 [B, Ho, Wo, N], mag = sum |x w| + |b| (the scale of the accumulation error)."""
+    x = np.asarray(x, dtype=np.float64)
+    w = np.asarray(w, dtype=np.float64)
+    B, H, W, C = x.shape
+    N, cg, k, _ = w.shape
+    assert C == cg * groups and N % groups == 0
+    ng = N // groups
+    Ho, Wo = out_hw(H, W, k, stride, pad)
+    xp = np.zeros((B, H + 2 * pad, W + 2 * pad, C))
+    xp[:, pad:pad + H, pad:pad + W] = x
+    y = np.zeros((B, Ho, Wo, N))
+    mag = np.zeros((B, Ho, Wo, N))
+    for ky in range(k):
+        for kx in range(k):
+            xs = xp[:, ky:ky + stride * (Ho - 1) + 1:stride, kx:kx + stride * (Wo - 1) + 1:stride]
+            if groups == C and ng == 1:                  # depthwise: elementwise per channel
+                y += xs * w[:, 0, ky, kx]
+                mag += np.abs(xs) * np.abs(w[:, 0, ky, kx])
+                continue
+            for g in range(groups):
+                xg = xs[..., g * cg:(g + 1) * cg]
+                wg = w[g * ng:(g + 1) * ng, :, ky, kx]
+                y[..., g * ng:(g + 1) * ng] += xg @ wg.T
+                mag[..., g * ng:(g + 1) * ng] += np.abs(xg) @ np.abs(wg).T
+    if b is not None:
+        b = np.asarray(b, dtype=np.float64)
+        y += b
+        mag += np.abs(b)
+    return y, mag
+
+
+def bf16_bound(ref, mag, k_terms):
+    """error bound of a bf16 output: ref and mag from conv_ref (mag including |b| and |res|)"""
+    return U_BF16 * np.abs(ref) + (k_terms + 2) * U_F32 * mag
+
+
+def epilogue(y, mag, relu, res=None):
+    """+ residual, then ReLU (the order of the torchvision block tail); ReLU is 1-Lipschitz, the bound carries over"""
+    if res is not None:
+        res = np.asarray(res, dtype=np.float64)
+        y = y + res
+        mag = mag + np.abs(res)
+    if relu:
+        y = np.maximum(y, 0.0)
+    return y, mag
+
+
+def dw_gemm_ref(x, dw_w, dw_b, dw_relu, w, b, relu):
+    """fused depthwise 5x5 (stride 1, pad 2, f32 weights) -> 1x1 (bf16 weights) with a bf16 intermediate.
+    x [B, H, W, C], dw_w [C, 5, 5], w [N, C] -> (ref, bound) of the bf16 output.
+    The kernel rounds its f32 depthwise result d_gpu to bf16; |bf16(d_gpu) - d| <= 2^-8 |d| + (1 + 2^-8) e_dw, so the
+    1x1 sees an operand error of at most that per k, weighted by |w_nk|."""
+    C = x.shape[-1]
+    d, dmag = conv_ref(x, np.asarray(dw_w).reshape(C, 1, 5, 5), dw_b, 1, 2, groups=C)
+    d, dmag = epilogue(d, dmag, dw_relu)
+    e_dw = 27 * U_F32 * dmag
+    d_err = U_BF16 * np.abs(d) + (1 + U_BF16) * e_dw
+    w = np.asarray(w, dtype=np.float64)
+    y = d @ w.T + np.asarray(b, dtype=np.float64)
+    mag = np.abs(d) @ np.abs(w).T + np.abs(b)
+    op_err = d_err @ np.abs(w).T
+    y, mag = epilogue(y, mag, relu)
+    return y, bf16_bound(y, mag, C) + op_err
+
+
+def normalise_u8(images_hwc, mean, std):
+    """torchvision ToTensor + Normalize in float32 with IEEE order: ((u / 255) - mean[c]) / std[c]; -> NHWC f32"""
+    x = images_hwc.astype(np.float32) / np.float32(255.0)
+    return (x - np.asarray(mean, dtype=np.float32)) / np.asarray(std, dtype=np.float32)
+
+
+def heads_ref(a, w, b, n_fields, n_comp, comp_ops):
+    """CompositeField4 eval epilogue (upsample 1) on a [B, h, w, K] feature map with weights w [N, K]:
+    -> per head (ref, bound) arrays [B, F, comp, h, w] in float64.  The bound pushes the accumulation error through
+    the activation (sigmoid: Lipschitz 1/4, softplus: 1) and adds a few f32 ulp for expf / log1pf / the index add."""
+    a = np.asarray(a, dtype=np.float64)
+    w = np.asarray(w, dtype=np.float64)
+    B, h, wd, K = a.shape
+    y = a @ w.T + b
+    acc = (K + 2) * U_F32 * (np.abs(a) @ np.abs(w).T + np.abs(b))
+    xs = np.arange(wd, dtype=np.float64).reshape(1, 1, wd)
+    ys = np.arange(h, dtype=np.float64).reshape(1, h, 1)
+    out, col, op_off = [], 0, 0
+    for nf, nc in zip(n_fields, n_comp):
+        v = y[..., col:col + nf * nc].reshape(B, h, wd, nf, nc).transpose(0, 3, 4, 1, 2).copy()
+        e = acc[..., col:col + nf * nc].reshape(B, h, wd, nf, nc).transpose(0, 3, 4, 1, 2).copy()
+        for c in range(nc):
+            op = comp_ops[op_off + c]
+            if op == OP_SIGMOID:
+                v[:, :, c] = 1.0 / (1.0 + np.exp(-v[:, :, c]))
+                e[:, :, c] = 0.25 * e[:, :, c] + 8 * 2.0 ** -24
+            elif op == OP_ADD_X:
+                v[:, :, c] += xs
+                e[:, :, c] += 2.0 ** -24 * np.abs(v[:, :, c])
+            elif op == OP_ADD_Y:
+                v[:, :, c] += ys
+                e[:, :, c] += 2.0 ** -24 * np.abs(v[:, :, c])
+            elif op == OP_SOFTPLUS:
+                v[:, :, c] = np.logaddexp(0.0, v[:, :, c])
+                e[:, :, c] += 8 * 2.0 ** -24 * (np.abs(v[:, :, c]) + 1.0)
+            else:
+                e[:, :, c] += 2.0 ** -24 * np.abs(v[:, :, c])
+        out.append((v, e))
+        col += nf * nc
+        op_off += nc
+    return out
+
+
+def worst_ratio(got, ref, bound):
+    """max |got - ref| / bound (> 1: the kernel is outside its error bound); NaN / inf in got count as infinite"""
+    got = np.asarray(got, dtype=np.float64)
+    err = np.abs(got - ref)
+    err[~np.isfinite(got)] = np.inf
+    return float((err / np.maximum(bound, 1e-300)).max()) if err.size else 0.0
+
+
+def fused_rings(channels, n_out):
+    """(window ring, B ring) depths that pifpaf_net_dw_conv1x1_scatter picks for a fused depthwise -> 1x1 op.
+    Mirrors fused_smem_bytes, the candidate list {3,2},{2,2},{2,1},{1,1} and GEMM_SMEM_BUDGET of
+    openpifpaf_b200/csrc/net.cu; test_kernel_refs.py::test_fused_ring_plan_mirror_matches_net_cu fails when those
+    change, so the cases of test_kernels_gpu.py keep reaching every ring depth."""
+    def pad8(v):
+        return (v + 7) // 8 * 8
+
+    def pad16(v):
+        return (v + 15) // 16 * 16
+    C = pad8(channels)
+    nb = (n_out + 191) // 192                    # FD_MAX_BLOCK_N = 3 x 64 columns per CTA
+    bn = pad16((n_out + nb - 1) // nb)
+    window = 12 * 20 * 64 * 2                    # DwTile<1, 8, 16, 4, 1>::BYTES: (8+4) x (16+4) pixels x 64 channels
+    stg = 8 * 16 * 33 * 4                        # STG_BYTES
+    for ws, bs in ((3, 2), (2, 2), (2, 1), (1, 1)):
+        size = (1024 + 128 * 64 * 2 + bs * bn * 64 * 2 + ws * window + bn * nb * 5 + C * 26 * 4 + stg
+                + 2 * (ws + bs) * 8 + 64)
+        if size <= 222 * 1024:
+            return ws, bs
+    return None
+
+
+def written_columns(op, tensors):
+    """(tensor, first column, end column) windows one op of network.build_ops writes ('heads' writes none of the
+    activation tensors).  Plain outputs cover pad8(n) columns: the kernels store whole 8-channel vectors."""
+    def pad8(v):
+        return (v + 7) // 8 * 8
+    kind = op['kind']
+    if kind == 'input_conv':
+        return [(op['out'], 0, pad8(op['c_out']))]
+    if kind in ('conv1x1', 'dw_conv1x1') and 'pieces' in op:
+        return [(t, col, col + cnt) for (_, cnt, t, col) in op['pieces']]
+    if kind == 'conv1x1':
+        if op['shuffle_src'] >= 0:
+            return [(op['out'], 0, 2 * op['n_out'])]
+        return [(op['out'], op['out_off'], op['out_off'] + pad8(op['n_out']))]
+    if kind == 'conv':
+        return [(op['out'], op['out_off'], op['out_off'] + pad8(op['n_out']))]
+    if kind == 'dwconv':
+        return [(op['out'], op['out_off'], op['out_off'] + pad8(op['channels']))]
+    if kind == 'heads':
+        return []
+    raise ValueError(kind)

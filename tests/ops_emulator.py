@@ -9,13 +9,11 @@ import torch
 import torch.nn.functional as F
 
 
-def run_ops(tensors, ops, images, bf16=False, dw_bf16_weights=None):
+def run_ops(tensors, ops, images, bf16=False):
     """images [B,3,H,W] float32 -> list of head outputs [B,F,comp,h,w].
 
-    dw_bf16_weights: the stand-alone 5x5 depthwise ops run on the tensor cores (k_dwconv5_tc), which takes the folded
-    depthwise weights as bf16 like every 1x1 weight (bias and accumulation f32); default: same as ``bf16``."""
-    if dw_bf16_weights is None:
-        dw_bf16_weights = bf16
+    With ``bf16`` activations and the weights of the GEMM-like ops (1x1, implicit-GEMM conv, heads) are rounded to bf16;
+    depthwise and stem weights stay f32, as the kernels read them."""
     B = images.shape[0]
     acts = [torch.zeros((B, h, w, c), dtype=torch.float32) for (h, w, c) in tensors]
 
@@ -75,8 +73,6 @@ def run_ops(tensors, ops, images, bf16=False, dw_bf16_weights=None):
             c = o['channels']
             a = acts[o['in']][..., o['in_off']:o['in_off'] + c].permute(0, 3, 1, 2)
             w = torch.from_numpy(o['w']).reshape(c, 1, o['kernel'], o['kernel'])
-            if dw_bf16_weights and o['kernel'] == 5 and o['pad'] == 2 and o['stride'] in (1, 2):
-                w = w.to(torch.bfloat16).to(torch.float32)
             y = F.conv2d(a, w, torch.from_numpy(o['b']), o['stride'], o['pad'], groups=c)
             if o['relu']:
                 y = F.relu(y)

@@ -1,0 +1,200 @@
+"""CPU: the float64 references of tests/kernel_refs.py against torch in float64, the bound they come with, and the
+write-once property of the op lists that the teacher-forced checks of tests/test_kernels_gpu.py rely on."""
+import numpy as np
+import pytest
+import torch
+import torch.nn.functional as F
+
+import kernel_refs as kr
+from openpifpaf_b200 import network
+from oracle import net_oracle
+
+
+def torch_conv(x_nhwc, w, b, stride, pad, groups=1):
+    x = torch.from_numpy(np.asarray(x_nhwc, dtype=np.float64)).permute(0, 3, 1, 2)
+    y = F.conv2d(x, torch.from_numpy(np.asarray(w, dtype=np.float64)),
+                 None if b is None else torch.from_numpy(np.asarray(b, dtype=np.float64)), stride, pad, groups=groups)
+    return y.permute(0, 2, 3, 1).numpy()
+
+
+@pytest.mark.parametrize('k,stride,pad,c_in,n_out,groups', [
+    (1, 1, 0, 24, 40, 1),       # pointwise
+    (1, 2, 0, 16, 8, 1),        # strided 1x1 (ResNet downsample)
+    (3, 1, 1, 7, 5, 1),         # dense
+    (3, 2, 0, 6, 4, 1),         # strided, no padding
+    (7, 2, 3, 3, 16, 1),        # stem
+    (5, 1, 2, 12, 12, 12),      # depthwise
+    (5, 2, 1, 9, 9, 9),         # depthwise, stride 2
+    (3, 1, 1, 8, 12, 4),        # grouped
+])
+def test_conv_ref_matches_torch_float64(k, stride, pad, c_in, n_out, groups):
+    rng = np.random.default_rng(k * 100 + c_in)
+    x = rng.standard_normal((2, 11, 9, c_in))
+    w = rng.standard_normal((n_out, c_in // groups, k, k))
+    b = rng.standard_normal(n_out)
+    y, mag = kr.conv_ref(x, w, b, stride, pad, groups=groups)
+    want = torch_conv(x, w, b, stride, pad, groups)
+    assert y.shape == want.shape
+    np.testing.assert_allclose(y, want, rtol=1e-12, atol=1e-12)
+    # mag is the same conv on absolute values
+    np.testing.assert_allclose(mag, torch_conv(np.abs(x), np.abs(w), np.abs(b), stride, pad, groups), rtol=1e-12)
+
+
+def test_residual_epilogue_adds_before_relu():
+    rng = np.random.default_rng(1)
+    x = rng.standard_normal((1, 6, 5, 8))
+    w = rng.standard_normal((8, 8, 3, 3))
+    b = rng.standard_normal(8)
+    res = rng.standard_normal((1, 6, 5, 8))
+    y, mag = kr.conv_ref(x, w, b, 1, 1)
+    y, mag = kr.epilogue(y, mag, True, res)
+    want = np.maximum(torch_conv(x, w, b, 1, 1) + res, 0.0)
+    np.testing.assert_allclose(y, want, rtol=1e-12, atol=1e-12)
+    assert (mag >= np.abs(res)).all()
+
+
+def test_dw_gemm_ref_is_depthwise_then_pointwise():
+    rng = np.random.default_rng(2)
+    C, N = 10, 6
+    x = rng.standard_normal((2, 7, 9, C))
+    dw_w = rng.standard_normal((C, 5, 5))
+    dw_b = rng.standard_normal(C)
+    w = rng.standard_normal((N, C))
+    b = rng.standard_normal(N)
+    y, bound = kr.dw_gemm_ref(x, dw_w, dw_b, 1, w, b, 1)
+    d = np.maximum(torch_conv(x, dw_w.reshape(C, 1, 5, 5), dw_b, 1, 2, groups=C), 0.0)
+    want = np.maximum(torch_conv(d, w.reshape(N, C, 1, 1), b, 1, 0), 0.0)
+    np.testing.assert_allclose(y, want, rtol=1e-12, atol=1e-12)
+    # the bf16 intermediate term dominates the bound: at least 2^-8 sum_k |w_nk| |d_k|
+    assert (bound >= kr.U_BF16 * (np.abs(d) @ np.abs(w).T) - 1e-12).all()
+
+
+def test_heads_ref_matches_torch_ops():
+    rng = np.random.default_rng(3)
+    B, h, w, K = 2, 5, 7, 24
+    n_fields, n_comp = [3, 2], [5, 9]
+    comp_ops = [1, 2, 3, 4, 0] + [1, 2, 3, 0, 0, 4, 4, 1, 0]
+    N = sum(f * c for f, c in zip(n_fields, n_comp))
+    a = rng.standard_normal((B, h, w, K))
+    wt = rng.standard_normal((N, K)) * 3
+    bias = rng.standard_normal(N)
+    got = kr.heads_ref(a, wt, bias, n_fields, n_comp, comp_ops)
+    y = torch.from_numpy(a) @ torch.from_numpy(wt).T + torch.from_numpy(bias)
+    col, off = 0, 0
+    for (v, e), nf, nc in zip(got, n_fields, n_comp):
+        t = y[..., col:col + nf * nc].reshape(B, h, w, nf, nc).permute(0, 3, 4, 1, 2).clone()
+        for c in range(nc):
+            op = comp_ops[off + c]
+            if op == 1:
+                t[:, :, c] = torch.sigmoid(t[:, :, c])
+            elif op == 2:
+                t[:, :, c] += torch.arange(w, dtype=torch.float64).view(1, 1, w)
+            elif op == 3:
+                t[:, :, c] += torch.arange(h, dtype=torch.float64).view(1, h, 1)
+            elif op == 4:
+                t[:, :, c] = F.softplus(t[:, :, c])
+        # torch's softplus returns x above 20 (threshold): log1p(exp(-20)) = 2e-9 from the exact value
+        np.testing.assert_allclose(v, t.numpy(), rtol=1e-12, atol=3e-9)
+        assert (e > 0).all()
+        col += nf * nc
+        off += nc
+
+
+def test_bf16_round_is_torch_round_to_nearest_even():
+    rng = np.random.default_rng(4)
+    a = np.concatenate([rng.standard_normal(100000).astype(np.float32) * 1e3,
+                        np.array([1 + 2 ** -8, 1 + 3 * 2 ** -8, -(1 + 2 ** -8), 2 ** -130], dtype=np.float32)])
+    want = torch.from_numpy(a).to(torch.bfloat16).to(torch.float32).numpy()
+    np.testing.assert_array_equal(kr.bf16_round(a), want)
+    assert kr.bf16_round(np.float32(kr.SENTINEL)) == np.float32(kr.SENTINEL)
+
+
+def test_bound_accepts_round_to_nearest_and_rejects_truncation():
+    """the bf16 bound is tight enough to see half an ulp: f32 results rounded to nearest pass, truncated ones fail"""
+    rng = np.random.default_rng(5)
+    x = kr.random_bf16(rng, (2, 9, 9, 64))
+    w = kr.random_bf16(rng, (48, 64, 1, 1), 1 / 8)
+    ref, mag = kr.conv_ref(x, w, None, 1, 0)
+    f32 = ref.astype(np.float32)
+    bound = kr.bf16_bound(ref, mag, 64)
+    assert kr.worst_ratio(kr.bf16_round(f32), ref, bound) <= 1.0
+    assert kr.worst_ratio(kr.bf16_truncate(f32), ref, bound) > 1.0
+    assert kr.worst_ratio(np.where(ref > 0, np.nan, f32), ref, bound) == np.inf
+
+
+def test_normalise_u8_is_torchvision_order():
+    rng = np.random.default_rng(6)
+    u = rng.integers(0, 256, (2, 5, 7, 3), dtype=np.uint8)
+    mean, std = network.CompiledNet.IMAGE_MEAN, network.CompiledNet.IMAGE_STD
+    t = torch.from_numpy(u).to(torch.float32) / 255.0
+    want = (t - torch.tensor(mean, dtype=torch.float32)) / torch.tensor(std, dtype=torch.float32)
+    np.testing.assert_array_equal(kr.normalise_u8(u, mean, std), want.numpy())
+
+
+def _write_once(tensors, ops):
+    owner = [np.full(c, -1) for (_, _, c) in tensors]
+    for i, o in enumerate(ops):
+        for t, c0, c1 in kr.written_columns(o, tensors):
+            assert 0 <= c0 < c1 <= tensors[t][2], (i, o['kind'], t, c0, c1)
+            clash = owner[t][c0:c1]
+            assert (clash < 0).all(), f'op {i} ({o["kind"]}) writes tensor {t} columns owned by op {clash.max()}'
+            owner[t][c0:c1] = i
+    return owner
+
+
+@pytest.mark.parametrize('base,layout,fuse', [
+    ('shufflenetv2k16', 'bins', True), ('shufflenetv2k16', 'bins', False), ('shufflenetv2k16', 'shuffle', False),
+    ('shufflenetv2k30', 'bins', False), ('resnet18', None, None), ('resnet50', None, None)])
+def test_every_tensor_column_is_written_by_one_op(base, layout, fuse):
+    """each (tensor, column) is written by at most one op of a forward: a tap after the forward shows every op's
+    output as that op left it, and every op's inputs as it read them"""
+    if base.startswith('resnet'):
+        plan = network.plan_from_shell(net_oracle.make_shell(base, seed=0))
+        tensors, ops, _ = network.build_ops(plan, 97, 129)
+    else:
+        plan = network.random_plan(base, seed=0)
+        tensors, ops, _ = network.build_ops(plan, 97, 129, layout=layout, fuse_dw=fuse)
+    owner = _write_once(tensors, ops)
+    # and every column an op reads was produced before it (or is never written: zero padding)
+    for i, o in enumerate(ops):
+        if o['kind'] == 'input_conv':
+            continue
+        width = o.get('k_cols', o.get('channels', o.get('c_in')))
+        reads = [(o['in'], o.get('in_off', 0), width)]
+        if o.get('shuffle_src', -1) >= 0:
+            reads.append((o['shuffle_src'], o['shuffle_off'], o['n_out']))
+        if o.get('residual', -1) >= 0:
+            reads.append((o['residual'], o['residual_off'], o['n_out']))
+        for t, c0, n in reads:
+            assert (owner[t][c0:c0 + n] < i).all(), (i, o['kind'], t)
+
+
+def test_fused_ring_plan_mirror_matches_net_cu():
+    """kernel_refs.fused_rings copies the shared-memory plan of the fused depthwise -> 1x1 op; the lines it copies
+    are still those of net.cu (change both together)"""
+    import os
+    import re
+    src = open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))),
+                            'openpifpaf_b200', 'csrc', 'net.cu')).read()
+    flat = re.sub(r'\s+', ' ', src)
+    for line in [
+        'size_t fused_smem_bytes(int ws, int bs, int block_n, int n_pad, int c_dw) { return 1024 + (size_t)BM * BK * 2 + '
+        '(size_t)bs * block_n * BK * 2 + (size_t)ws * DwTile<1, PH, PW, 4, 1>::BYTES + (size_t)n_pad * 5 + '
+        '(size_t)c_dw * 26 * 4 + STG_BYTES + (size_t)(2 * (ws + bs)) * 8 + 64; }',
+        'const int cand[][2] = {{3, 2}, {2, 2}, {2, 1}, {1, 1}};',
+        'if (fused_smem_bytes(c[0], c[1], block_n, n_pad, C) <= GEMM_SMEM_BUDGET)',
+        'const int n_blocks = (n_out + FD_MAX_BLOCK_N - 1) / FD_MAX_BLOCK_N;',
+        'const int block_n = pad16((n_out + n_blocks - 1) / n_blocks);',
+        'constexpr int FD_MAX_BLOCK_N = 3 * NGROUP;',
+        'constexpr size_t GEMM_SMEM_BUDGET = 222 * 1024;',
+        'constexpr int PH = 8, PW = 16;',
+        'static constexpr int IH = (TH - 1) * S + 5, IW = (TW - 1) * S + 5;',
+        'static constexpr int BYTES = IH * IW * 64 * 2;',
+        'constexpr int STG_LD = 33;',
+        'constexpr int STG_BYTES = CONSUMER_WARPS * 16 * STG_LD * 4;',
+        'constexpr int CONSUMER_WARPS = 8;',
+        'constexpr int BM = 128;',
+        'constexpr int BK = 64;',
+    ]:
+        assert line in flat, line
+    assert kr.fused_rings(176, 176) == (3, 2) and kr.fused_rings(1024, 192) == (1, 1)
