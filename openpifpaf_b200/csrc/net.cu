@@ -78,6 +78,20 @@ __device__ __forceinline__ void tma_load_4d(void* smem_dst, const CUtensorMap* m
           "r"(c0), "r"(c1), "r"(c2), "r"(c3)
         : "memory");
 }
+// shared -> global tensor store (bulk async-group completion, tracked per issuing thread)
+__device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, const void* smem_src, int c0, int c1) {
+    asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
+                 ::"l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(smem_src)), "r"(c0), "r"(c1)
+                 : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// all but the newest PENDING bulk groups of this thread have finished reading shared memory
+template <int PENDING>
+__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(PENDING) : "memory"); }
+// all bulk groups of this thread have completed (their global writes are done)
+__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+// orders generic-proxy shared-memory writes before the async proxy (TMA, wgmma) reads them
+__device__ __forceinline__ void fence_proxy_async_shared() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 // ---- warpgroup MMA (wgmma): D[registers] (+)= A[smem] * B[smem]^T, bf16 inputs, f32 accumulate, issued by the four
 // warps of a warpgroup together.  m64nNk16: thread t of the warpgroup holds, for every group of 8 columns,
 // d[4j], d[4j+1] = row 16 * (warp % 4) + lane / 4, columns 8j + 2 * (lane % 4) + {0, 1}; d[4j+2], d[4j+3] = 8 rows below.
@@ -132,11 +146,14 @@ __device__ __forceinline__ void wgmma_n64(float* d, uint64_t adesc, uint64_t bde
         : "l"(adesc), "l"(bdesc), "r"(accumulate)
         : "memory");
 }
-// one 64-column group (or the narrower last group: n = 16, 32, 48) of a k16 step
-__device__ __forceinline__ void wgmma_group(int n, float* d, uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
-    if (n >= 64) wgmma_n64(d, adesc, bdesc, accumulate);
-    else if (n == 48) wgmma_n48(d, adesc, bdesc, accumulate);
-    else if (n == 32) wgmma_n32(d, adesc, bdesc, accumulate);
+// one 64-column group (or the narrower last group: N = 16, 32, 48) of a k16 step.  N is a compile-time constant:
+// a wgmma behind a runtime branch makes ptxas fence every one of them (warpgroup.arrive, C7519)
+template <int N>
+__device__ __forceinline__ void wgmma_group(float* d, uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+    static_assert(N == 16 || N == 32 || N == 48 || N == 64, "wgmma group width");
+    if constexpr (N == 64) wgmma_n64(d, adesc, bdesc, accumulate);
+    else if constexpr (N == 48) wgmma_n48(d, adesc, bdesc, accumulate);
+    else if constexpr (N == 32) wgmma_n32(d, adesc, bdesc, accumulate);
     else wgmma_n16(d, adesc, bdesc, accumulate);
 }
 
@@ -178,8 +195,19 @@ enum { MODE_PLAIN = 0, MODE_SHUFFLE = 1, MODE_HEADS = 2, MODE_SCATTER = 3 };
 
 // MODE_SCATTER: destination of one chunk of 16 GEMM columns (32 bytes per row, one 256-bit store per lane): base
 // already points at the chunk's first column inside its tensor (a multiple of 16 channels)
-struct DestGroup { __nv_bfloat16* base; int ld; int pad; };
+// store: the same destination for the TMA-store epilogue, (store map index << 16) | first column inside that map
+struct DestGroup { __nv_bfloat16* base; int ld; int store; };
 static_assert(sizeof(DestGroup) == 16, "DestGroup is copied to shared memory as 16-byte entries");
+
+// TMA-store epilogue (MODE_PLAIN without residual, MODE_SCATTER): output tensor maps, rows bounded at the forward's
+// batch * h * w.  Plain: map 0 = the output window.  Scatter: one map per destination tensor.
+constexpr int MAX_STORE_MAPS = 8;
+struct StoreMaps { CUtensorMap m[MAX_STORE_MAPS]; };
+constexpr int OUT_BOX_COLS = 16, OUT_BOX_ROWS = 16;      // one box: a warp's 16 rows x 16 columns, 32-byte swizzle
+constexpr int OUT_BOX_BYTES = OUT_BOX_ROWS * OUT_BOX_COLS * 2;
+constexpr int OUT_CHUNK_BYTES = 2 * OUT_BOX_BYTES;       // 32 columns: half of a wgmma column group
+constexpr int OUT_WARP_BYTES = 2 * OUT_CHUNK_BYTES;      // double buffered
+static_assert(CONSUMER_WARPS * OUT_WARP_BYTES <= STG_BYTES, "the output chunks live in the f32 staging region");
 
 // per GEMM output column (heads mode): plane = field * n_comp + comp; sub = (dy << 8) | dx is the PixelShuffle
 // position of this conv channel inside the up x up block of its cell (heads.py:333-343), 0 without upsampling
@@ -196,6 +224,7 @@ struct GemmArgs {
     const __nv_bfloat16* src0; int ld0; int src0_col_off; int half; int gap;
     int src_tma;                 // pass-through tile arrives by TMA in shared memory (else read from global)
     int b_resident;              // all K blocks of this CTA's weight tile stay in shared memory (loaded once)
+    int tma_store;               // epilogue through shared memory + TMA stores (StoreMaps), else per-lane global stores
     // scatter: chunks of 16 columns go to different tensors (the 'bins' layout: every channel is written once,
     // into the buffer of the block that consumes it)
     const DestGroup* dest;       // [n_blocks * block_n / 16]
@@ -384,19 +413,19 @@ __device__ __forceinline__ void epilogue_chunk(const GemmArgs& g, int m, int n0,
 }
 
 // ------------------------------------------------------------------ consumer side shared by the wgmma kernels
-// D (+)= A-tile rows [64 * wg, +64) x B-tile^T over one 64-wide K block: 4 k16 steps x NG column groups
-template <int NG>
-__device__ __forceinline__ void mma_k_block(float (&acc)[NG][32], uint32_t sa, uint32_t sb, int block_n, bool first) {
+// D (+)= A-tile rows [64 * wg, +64) x B-tile^T over one 64-wide K block: 4 k16 steps x NG column groups, the last
+// LASTW (16, 32, 48 or 64) columns wide -- the tile is (NG - 1) * 64 + LASTW columns
+template <int NG, int LASTW>
+__device__ __forceinline__ void mma_k_block(float (&acc)[NG][32], uint32_t sa, uint32_t sb, bool first) {
 #pragma unroll
     for (int k = 0; k < BK / MMA_K; k++) {
         const uint64_t adesc = make_smem_desc(sa + k * MMA_K * 2);
+        const uint32_t accumulate = (first && k == 0) ? 0u : 1u;
 #pragma unroll
-        for (int gi = 0; gi < NG; gi++) {
-            const int n = block_n - gi * NGROUP;
-            if (n > 0)
-                wgmma_group(n, acc[gi], adesc, make_smem_desc(sb + gi * NGROUP * BK * 2 + k * MMA_K * 2),
-                            (first && k == 0) ? 0u : 1u);
-        }
+        for (int gi = 0; gi < NG - 1; gi++)
+            wgmma_group<NGROUP>(acc[gi], adesc, make_smem_desc(sb + gi * NGROUP * BK * 2 + k * MMA_K * 2), accumulate);
+        wgmma_group<LASTW>(acc[NG - 1], adesc, make_smem_desc(sb + (NG - 1) * NGROUP * BK * 2 + k * MMA_K * 2),
+                           accumulate);
     }
 }
 
@@ -441,14 +470,77 @@ __device__ __forceinline__ void warp_epilogue(const GemmArgs& g, float (&acc)[NG
     }
 }
 
+// TMA-store epilogue of one consumer warp (MODE_PLAIN without residual, MODE_SCATTER): its 16 rows x BN accumulators
+// go, with bias and ReLU, as bf16 straight from the wgmma fragments into 16 x 16 boxes in shared memory (32-byte
+// swizzle: a row's two 16-byte halves swap on rows 4-7 of every 8, which makes the fragment-order writes
+// conflict-free), and one lane stores every box with a TMA tensor store.  The warp does not wait for the stores: it
+// goes on to the next tile's MMAs, and reclaims a 32-column chunk buffer (two boxes) only when the bulk group that
+// read it two chunks ago has finished reading.  The tensor maps clip rows at M and, in plain mode, columns at the
+// window's pad8(N), so rows past the batch and columns past the window are never written.
+// obuf: this warp's two chunk buffers; ob: which of them is next (carried across tiles)
+template <int NG, int LASTW>
+__device__ __forceinline__ void warp_epilogue_tma(const GemmArgs& g, const StoreMaps& maps, float (&acc)[NG][32],
+                                                  unsigned char* obuf, int& ob, int m_blk, int n_blk, int row0,
+                                                  const float* bias_s, const DestGroup* dest_s) {
+    constexpr int BN = (NG - 1) * NGROUP + LASTW;
+    const int lane = threadIdx.x & 31;
+    const int r = lane >> 2, q = lane & 3;
+    const int sw = (r >> 2) & 1;                       // rows r and r + 8 share it
+    const int m0 = m_blk * BM + row0;
+    const float* bias_t = bias_s + n_blk * BN;
+    const int n_lim = g.mode == MODE_SCATTER ? g.N : ((g.N + 7) & ~7);
+#pragma unroll
+    for (int gi = 0; gi < NG; gi++) {
+#pragma unroll
+        for (int h = 0; h < 2; h++) {
+            const int p = gi * NGROUP + h * 32;        // first tile column of this chunk
+            if (p >= BN) continue;
+            const int boxes = (BN - p) >= 32 ? 2 : 1;  // compile-time after unrolling
+            unsigned char* buf = obuf + ob * OUT_CHUNK_BYTES;
+            if (lane == 0) bulk_wait_read<1>();
+            __syncwarp();
+#pragma unroll
+            for (int t = 0; t < 4; t++) {
+                if (t >= 2 * boxes) continue;
+                const int j = h * 4 + t;               // 8-column fragment group inside the wgmma group
+                const float2 b = *reinterpret_cast<const float2*>(bias_t + p + 8 * t + 2 * q);
+                float v0 = acc[gi][4 * j] + b.x, v1 = acc[gi][4 * j + 1] + b.y;
+                float v2 = acc[gi][4 * j + 2] + b.x, v3 = acc[gi][4 * j + 3] + b.y;
+                if (g.relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); v2 = fmaxf(v2, 0.f); v3 = fmaxf(v3, 0.f); }
+                unsigned char* bx = buf + (t >> 1) * OUT_BOX_BYTES + (((t & 1) ^ sw) << 4) + q * 4;
+                *reinterpret_cast<uint32_t*>(bx + r * 32) = pack_bf16(v0, v1);
+                *reinterpret_cast<uint32_t*>(bx + (r + 8) * 32) = pack_bf16(v2, v3);
+            }
+            fence_proxy_async_shared();
+            __syncwarp();
+            if (lane == 0) {
+                for (int x = 0; x < boxes; x++) {
+                    const int n0 = n_blk * BN + p + x * OUT_BOX_COLS;
+                    if (n0 >= n_lim) break;
+                    if (g.mode == MODE_SCATTER) {
+                        const int st = dest_s[n0 >> 4].store;
+                        tma_store_2d(&maps.m[st >> 16], buf + x * OUT_BOX_BYTES, st & 0xffff, m0);
+                    } else {
+                        tma_store_2d(&maps.m[0], buf + x * OUT_BOX_BYTES, n0, m0);
+                    }
+                }
+                bulk_commit();
+            }
+            ob ^= 1;
+        }
+    }
+}
+
 // ------------------------------------------------------------------ wgmma GEMM
-// NG = ceil(block_n / 64) column groups: 32 * NG accumulator registers per consumer thread
-template <int NG>
+// NG = ceil(block_n / 64) column groups: 32 * NG accumulator registers per consumer thread; the last group is LASTW
+// columns wide (block_n == (NG - 1) * 64 + LASTW)
+template <int NG, int LASTW>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 k_gemm_wg(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
-          const __grid_constant__ CUtensorMap tmap_src, GemmArgs g) {
+          const __grid_constant__ CUtensorMap tmap_src, const __grid_constant__ StoreMaps smaps, GemmArgs g) {
     extern __shared__ __align__(1024) unsigned char smem_raw[];
-    // carve: [stages][A 16 KB | B block_n*128 B] then resident weights, pass-through tiles, tables, staging, barriers
+    // carve: [stages][A 16 KB | B block_n*128 B] then resident weights, pass-through tiles, staging / output chunks
+    // (1024-byte aligned: everything before is a multiple of 2 KB), tables, barriers
     unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     const int a_bytes = BM * BK * 2;
     const int b_bytes = g.block_n * BK * 2;
@@ -460,10 +552,11 @@ k_gemm_wg(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CU
     // pass-through tiles of the fused shuffle: [2][BM rows][block_n] bf16, filled by TMA
     const int src_bytes = g.src_tma ? BM * g.block_n * 2 : 0;
     unsigned char* src_tiles = b_res + b_res_bytes;
-    float* bias_s = reinterpret_cast<float*>(src_tiles + 2 * (size_t)src_bytes);   // [n_blocks * block_n]
+    // f32 staging tiles of warp_epilogue, or the bf16 output chunks of warp_epilogue_tma (same region)
+    float* stg_s = reinterpret_cast<float*>(src_tiles + 2 * (size_t)src_bytes);
+    float* bias_s = reinterpret_cast<float*>(reinterpret_cast<unsigned char*>(stg_s) + STG_BYTES);   // [n_blocks * block_n]
     DestGroup* dest_s = reinterpret_cast<DestGroup*>(bias_s + g.n_blocks * g.block_n);   // [n_blocks * block_n / 16]
-    float* stg_s = reinterpret_cast<float*>(dest_s + g.n_blocks * g.block_n / CHUNK);
-    uint64_t* full_bar = reinterpret_cast<uint64_t*>(reinterpret_cast<unsigned char*>(stg_s) + STG_BYTES);   // [stages]
+    uint64_t* full_bar = reinterpret_cast<uint64_t*>(dest_s + g.n_blocks * g.block_n / CHUNK);   // [stages]
     uint64_t* empty_bar = full_bar + g.stages;                          // [stages]
     uint64_t* src_full = empty_bar + g.stages;                          // [2]
     uint64_t* src_empty = src_full + 2;                                 // [2]
@@ -561,6 +654,8 @@ k_gemm_wg(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CU
 #pragma unroll
             for (int i = 0; i < 32; i++) acc[gi][i] = 0.f;
         float* stg = stg_s + cw * 16 * STG_LD;
+        unsigned char* obuf = reinterpret_cast<unsigned char*>(stg_s) + cw * OUT_WARP_BYTES;
+        int ob = 0;
         int stage = 0; uint32_t phase = 0;
         int sbuf = 0; uint32_t sbuf_phase = 0;
         if (g.b_resident) mbar_wait(b_full, 0);
@@ -573,7 +668,7 @@ k_gemm_wg(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CU
 #pragma unroll
                 for (int gi = 0; gi < NG; gi++) fence_acc(acc[gi]);
                 wgmma_fence();
-                mma_k_block<NG>(acc, sa + wg * WG_ROWS * BK * 2, sb, g.block_n, kb == 0);
+                mma_k_block<NG, LASTW>(acc, sa + wg * WG_ROWS * BK * 2, sb, kb == 0);
                 wgmma_commit();
                 // the MMAs of the previous K block have retired: its slot goes back to the producer
                 if (kb > 0) {
@@ -587,6 +682,11 @@ k_gemm_wg(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CU
 #pragma unroll
             for (int gi = 0; gi < NG; gi++) fence_acc(acc[gi]);
             if (lane == 0) mbar_arrive(&empty_bar[prev]);
+            if (g.tma_store) {
+                warp_epilogue_tma<NG, LASTW>(g, smaps, acc, obuf, ob, m_blk, n_blk, wg * WG_ROWS + (cw & 3) * 16,
+                                             bias_s, dest_s);
+                continue;
+            }
             if (g.src_tma) mbar_wait(&src_full[sbuf], sbuf_phase);
             warp_epilogue<NG>(g, acc, stg, m_blk, n_blk, wg * WG_ROWS + (cw & 3) * 16, bias_s,
                               g.src_tma ? reinterpret_cast<const __nv_bfloat16*>(src_tiles + (size_t)sbuf * src_bytes) : nullptr,
@@ -597,6 +697,9 @@ k_gemm_wg(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CU
                 if (++sbuf == 2) { sbuf = 0; sbuf_phase ^= 1; }
             }
         }
+        // the dependent kernel's grid-dependency wait covers completed writes only: the tensor stores must be done
+        // before this CTA exits
+        if (g.tma_store && lane == 0) bulk_wait_all();
     }
 }
 
@@ -1047,9 +1150,7 @@ struct FusedArgs {
     int ws, bs;                  // ring depths: windows, B stages
 };
 
-__device__ __forceinline__ void fence_proxy_async_shared() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-
-template <int S, int NG>
+template <int S, int NG, int LASTW>
 __global__ void __launch_bounds__(FD_THREADS, 1)
 k_dw_gemm(const __grid_constant__ CUtensorMap tmap_win, const __grid_constant__ CUtensorMap tmap_b, GemmArgs g, FusedArgs f) {
     using T = DwTile<S, PH, PW, 4, 1>;
@@ -1215,8 +1316,8 @@ k_dw_gemm(const __grid_constant__ CUtensorMap tmap_win, const __grid_constant__ 
 #pragma unroll
             for (int gi = 0; gi < NG; gi++) fence_acc(acc_mma[gi]);
             wgmma_fence();
-            mma_k_block<NG>(acc_mma, smem_u32(a_st) + wg * WG_ROWS * BK * 2, smem_u32(b_st + (size_t)bi * b_bytes),
-                            g.block_n, kb == 0);
+            mma_k_block<NG, LASTW>(acc_mma, smem_u32(a_st) + wg * WG_ROWS * BK * 2, smem_u32(b_st + (size_t)bi * b_bytes),
+                                   kb == 0);
             wgmma_commit();
             b_prev = bi;
             if (++bi == f.bs) { bi = 0; bph ^= 1; }
@@ -1233,6 +1334,23 @@ size_t fused_smem_bytes(int ws, int bs, int block_n, int n_pad, int c_dw) {
     return 1024 + (size_t)BM * BK * 2 + (size_t)bs * block_n * BK * 2 + (size_t)ws * DwTile<1, PH, PW, 4, 1>::BYTES +
            (size_t)n_pad * 5 + (size_t)c_dw * 26 * 4 + STG_BYTES + (size_t)(2 * (ws + bs)) * 8 + 64;
 }
+
+// every (column groups, last group width) instantiation, indexed [NG - 1][LASTW / 16 - 1]: any block_n that is a
+// multiple of 16 up to 256 (192 for the fused op)
+using GemmKernel = decltype(&k_gemm_wg<1, 16>);
+const GemmKernel GEMM_KERNELS[4][4] = {
+    {k_gemm_wg<1, 16>, k_gemm_wg<1, 32>, k_gemm_wg<1, 48>, k_gemm_wg<1, 64>},
+    {k_gemm_wg<2, 16>, k_gemm_wg<2, 32>, k_gemm_wg<2, 48>, k_gemm_wg<2, 64>},
+    {k_gemm_wg<3, 16>, k_gemm_wg<3, 32>, k_gemm_wg<3, 48>, k_gemm_wg<3, 64>},
+    {k_gemm_wg<4, 16>, k_gemm_wg<4, 32>, k_gemm_wg<4, 48>, k_gemm_wg<4, 64>}};
+using DwGemmKernel = decltype(&k_dw_gemm<1, 1, 16>);
+const DwGemmKernel DW_GEMM_KERNELS[3][4] = {
+    {k_dw_gemm<1, 1, 16>, k_dw_gemm<1, 1, 32>, k_dw_gemm<1, 1, 48>, k_dw_gemm<1, 1, 64>},
+    {k_dw_gemm<1, 2, 16>, k_dw_gemm<1, 2, 32>, k_dw_gemm<1, 2, 48>, k_dw_gemm<1, 2, 64>},
+    {k_dw_gemm<1, 3, 16>, k_dw_gemm<1, 3, 32>, k_dw_gemm<1, 3, 48>, k_dw_gemm<1, 3, 64>}};
+// block_n (a multiple of 16) -> {NG - 1, LASTW / 16 - 1}
+inline int tile_groups(int block_n) { return (block_n + NGROUP - 1) / NGROUP - 1; }
+inline int tile_last(int block_n) { return (block_n - tile_groups(block_n) * NGROUP) / 16 - 1; }
 
 // ------------------------------------------------------------------ input conv: f32 NCHW [B,3,H,W] -> bf16 NHWC
 struct InConvArgs {
@@ -1411,6 +1529,25 @@ int make_tmap_plain(CUtensorMap* map, const void* base, uint64_t rows, uint64_t 
     return PIFPAF_OK;
 }
 
+// 2-D bf16 output view for the TMA-store epilogue: box = 16 rows x 16 columns (32 bytes), 32-byte swizzle
+int make_tmap_store(CUtensorMap* map, const void* base, uint64_t rows, uint64_t cols, uint64_t ld) {
+    PFN_encodeTiled fn = get_encode_fn();
+    if (!fn) { pifpaf::set_error("cuTensorMapEncodeTiled entry point not available"); return PIFPAF_E_CUDA; }
+    const cuuint64_t dims[2] = {cols, rows};
+    const cuuint64_t strides[1] = {ld * 2};
+    const cuuint32_t box[2] = {OUT_BOX_COLS, OUT_BOX_ROWS};
+    const cuuint32_t estr[2] = {1, 1};
+    CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), dims, strides, box, estr,
+                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_32B, CU_TENSOR_MAP_L2_PROMOTION_NONE,
+                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) {
+        pifpaf::set_error("cuTensorMapEncodeTiled (store) failed (%d): rows=%llu cols=%llu ld=%llu base=%p", (int)r,
+                          (unsigned long long)rows, (unsigned long long)cols, (unsigned long long)ld, base);
+        return PIFPAF_E_CUDA;
+    }
+    return PIFPAF_OK;
+}
+
 // 4-D bf16 NHWC activation view {C, W, H, B} for implicit-GEMM convolutions: box = 64 channels x the
 // input window of a PH x PW output patch, traversed with the conv stride
 int make_tmap_conv(CUtensorMap* map, const void* base, uint64_t c, uint64_t w, uint64_t h, uint64_t b, uint64_t ld,
@@ -1484,6 +1621,12 @@ struct Op {
     CUtensorMap tmap_a{}, tmap_b{}, tmap_src{};
     int a_tensor = -1; int rows_per_image = 0; int tiles_per_image = 0;
     size_t smem = 0;
+    // TMA-store epilogue (g.tma_store): the output views {base, columns, row pitch}, one per store map; the maps
+    // bound rows at batch * rows_per_image and are re-encoded when the batch changes (store_rows: the M they hold)
+    struct StoreView { const __nv_bfloat16* base; int cols; int ld; };
+    std::vector<StoreView> store_views;
+    StoreMaps smaps{};
+    int store_rows = -1;
     // dw
     DwArgs dw{};
     CUtensorMap tmap_dw{}; bool dw_tma = false;
@@ -1517,6 +1660,7 @@ struct pifpaf_net {
     bool pdl = true;                     // programmatic dependent launch between the ops of a forward (PIFPAF_PDL=0: off)
     int gemm_res_stages = 0;             // weights-resident GEMMs: split N further until this many A stages fit (PIFPAF_GEMM_RES_STAGES)
     bool dw_cbf = false;                 // stride-2 depthwise: channel-block-fastest item order (PIFPAF_DW_CBF=1)
+    bool gemm_tma_store = true;          // plain / scatter 1x1 GEMMs store through TMA (PIFPAF_GEMM_TMA_STORE=0: per-lane stores)
     int head_fields[4] = {0, 0, 0, 0}, head_comp[4] = {0, 0, 0, 0}, head_h = 0, head_w = 0;
     int in_h = 0, in_w = 0;
 };
@@ -1573,6 +1717,8 @@ void choose_block_n(int n_out, int* block_n, int* n_blocks) {
 
 constexpr size_t GEMM_SMEM_BUDGET = 222 * 1024;
 
+// STG_BYTES: the f32 staging tiles of the per-lane epilogue, or the bf16 output chunks of the TMA-store epilogue, which
+// fit in the same bytes -- both epilogues get the same ring depth and weight residency
 size_t gemm_smem_bytes(int block_n, int n_blocks, int stages, bool shuffle, bool b_resident = false, int num_k_blocks = 0) {
     const size_t b_stage = b_resident ? 0 : (size_t)block_n * BK * 2;
     const size_t b_res = b_resident ? (size_t)num_k_blocks * block_n * BK * 2 : 0;
@@ -1678,6 +1824,13 @@ int emit_gemm(pifpaf_net* net, Op& op, int in_tensor, int in_col_off, int k_cols
     return rc;
 }
 
+// plain 1x1 GEMM without residual: the TMA-store epilogue writes the window [out_col_off, + pad8(N)) of `to`
+void plan_tma_store_plain(const pifpaf_net* net, Op& op, const Tensor& to) {
+    if (!net->gemm_tma_store) return;
+    op.g.tma_store = 1;
+    op.store_views = {Op::StoreView{to.data + op.g.out_col_off, pad8(op.g.N), to.c}};
+}
+
 }  // namespace
 
 extern "C" {
@@ -1701,19 +1854,17 @@ int pifpaf_net_create(pifpaf_net_t** out, int32_t device, int32_t max_batch) {
     if (const char* e = std::getenv("PIFPAF_DW_CBF")) net->dw_cbf = std::atoi(e) != 0;
     if (const char* e = std::getenv("PIFPAF_PDL")) net->pdl = std::atoi(e) != 0;
     if (const char* e = std::getenv("PIFPAF_GEMM_RES_STAGES")) net->gemm_res_stages = std::atoi(e);
-    PIFPAF_CUDA_TRY(cudaFuncSetAttribute(k_gemm_wg<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024));
-    PIFPAF_CUDA_TRY(cudaFuncSetAttribute(k_gemm_wg<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024));
-    PIFPAF_CUDA_TRY(cudaFuncSetAttribute(k_gemm_wg<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024));
-    PIFPAF_CUDA_TRY(cudaFuncSetAttribute(k_gemm_wg<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024));
+    if (const char* e = std::getenv("PIFPAF_GEMM_TMA_STORE")) net->gemm_tma_store = std::atoi(e) != 0;
+    for (auto& row : GEMM_KERNELS)
+        for (auto* k : row) PIFPAF_CUDA_TRY(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024));
+    for (auto& row : DW_GEMM_KERNELS)
+        for (auto* k : row) PIFPAF_CUDA_TRY(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024));
     PIFPAF_CUDA_TRY(cudaFuncSetAttribute(k_dwconv5_tma<1, DW1_TH, DW1_TW, 4, 3>,
                                          cudaFuncAttributeMaxDynamicSharedMemorySize, DwS1::SMEM));
     PIFPAF_CUDA_TRY(cudaFuncSetAttribute(k_dwconv5_tma<2, DW2_TH, DW2_TW, 4, 2>,
                                          cudaFuncAttributeMaxDynamicSharedMemorySize, DwS2::SMEM));
     PIFPAF_CUDA_TRY(cudaFuncSetAttribute(k_dwconv5_tma<2, DW2_TH, DW2_TW, 4, 2, true>,
                                          cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024));
-    PIFPAF_CUDA_TRY(cudaFuncSetAttribute(k_dw_gemm<1, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024));
-    PIFPAF_CUDA_TRY(cudaFuncSetAttribute(k_dw_gemm<1, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024));
-    PIFPAF_CUDA_TRY(cudaFuncSetAttribute(k_dw_gemm<1, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024));
     // the stem stages its weights in shared memory: 7x7 with more than 72 channels is past the default 48 KB
     PIFPAF_CUDA_TRY(cudaFuncSetAttribute(k_input_conv<1, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, INCONV_SMEM_MAX));
     PIFPAF_CUDA_TRY(cudaFuncSetAttribute(k_input_conv<3, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, INCONV_SMEM_MAX));
@@ -1807,6 +1958,7 @@ int pifpaf_net_conv1x1(pifpaf_net_t* net, int32_t in_tensor, int32_t in_col_off,
     if (shuffle_src_tensor < 0) {
         g.mode = MODE_PLAIN;
         PIFPAF_CHECK_ARG(out_col_off + pad8(n_out) <= to.c, "output window outside the tensor");
+        plan_tma_store_plain(net, op, to);
     } else {
         PIFPAF_CHECK_ARG(shuffle_src_tensor < nt, "bad shuffle source tensor");
         const Tensor& ts = net->tensors[shuffle_src_tensor];
@@ -1847,6 +1999,8 @@ int pifpaf_net_conv1x1_scatter(pifpaf_net_t* net, int32_t in_tensor, int32_t in_
     GemmArgs& g = op.g;
     g.mode = MODE_SCATTER; g.relu = relu;
     std::vector<DestGroup> groups((size_t)g.n_blocks * g.block_n / 16, DestGroup{nullptr, 0, 0});
+    // TMA-store epilogue: one store map per destination tensor (a chunk's box covers exactly its 16 columns)
+    std::vector<int> map_tensor;
     int expect = 0;
     for (int i = 0; i < n_pieces; i++) {
         PIFPAF_CHECK_ARG(piece_col0[i] == expect && piece_count[i] >= 16 && piece_count[i] % 16 == 0,
@@ -1856,11 +2010,23 @@ int pifpaf_net_conv1x1_scatter(pifpaf_net_t* net, int32_t in_tensor, int32_t in_
         PIFPAF_CHECK_ARG(to.h == tin.h && to.w == tin.w, "conv1x1 keeps the spatial shape");
         PIFPAF_CHECK_ARG(piece_tensor_col[i] >= 0 && piece_tensor_col[i] % 16 == 0 &&
                          piece_tensor_col[i] + piece_count[i] <= to.c, "piece window outside its tensor");
+        int mi = 0;
+        while (mi < (int)map_tensor.size() && map_tensor[mi] != piece_tensor[i]) mi++;
+        if (mi == (int)map_tensor.size()) map_tensor.push_back(piece_tensor[i]);
         for (int c = 0; c < piece_count[i]; c += 16)
-            groups[(size_t)(expect + c) / 16] = DestGroup{to.data + piece_tensor_col[i] + c, to.c, 0};
+            groups[(size_t)(expect + c) / 16] = DestGroup{to.data + piece_tensor_col[i] + c, to.c,
+                                                          (mi << 16) | (piece_tensor_col[i] + c)};
         expect += piece_count[i];
     }
     PIFPAF_CHECK_ARG(expect == n_out, "pieces must cover all n_out columns");
+    // more destination tensors than store maps: the per-lane store epilogue
+    if (net->gemm_tma_store && (int)map_tensor.size() <= MAX_STORE_MAPS) {
+        g.tma_store = 1;
+        for (int t : map_tensor) {
+            const Tensor& to = net->tensors[t];
+            op.store_views.push_back(Op::StoreView{to.data, to.c, to.c});
+        }
+    }
     DestGroup* d_groups = nullptr;
     rc = net_upload(net, &d_groups, groups);
     if (rc != PIFPAF_OK) return rc;
@@ -1901,6 +2067,8 @@ int pifpaf_net_conv(pifpaf_net_t* net, int32_t in_tensor, int32_t in_col_off, in
             PIFPAF_CHECK_ARG(tr.h == ho && tr.w == wo && residual_col_off % 8 == 0 && residual_col_off + n_out <= tr.c,
                              "residual tensor shape mismatch");
             g.res = tr.data; g.ld_res = tr.c; g.res_col_off = residual_col_off;
+        } else {
+            plan_tma_store_plain(net, op, to);
         }
         plan_gemm_smem(g, &op.smem, false);
         net->ops.push_back(op);
@@ -2212,7 +2380,7 @@ static int net_forward_impl(pifpaf_net_t* net, const float* images_dev, int32_t 
             g.M = batch * op.rows_per_image;
             g.m_blocks = batch * op.tiles_per_image;
             const int grid = std::max(1, std::min(n_sm / g.n_blocks, g.m_blocks)) * g.n_blocks;
-            auto* kern = g.block_n <= NGROUP ? k_dw_gemm<1, 1> : g.block_n <= 2 * NGROUP ? k_dw_gemm<1, 2> : k_dw_gemm<1, 3>;
+            auto* kern = DW_GEMM_KERNELS[tile_groups(g.block_n)][tile_last(g.block_n)];
             PIFPAF_CUDA_TRY(launch_k(pdl, kern, dim3(grid), dim3(FD_THREADS), op.smem, st, op.tmap_dw, op.tmap_b, g, op.fu));
             PIFPAF_LAUNCH_CHECK();
         } else if (op.kind == OP_DW) {
@@ -2266,10 +2434,17 @@ static int net_forward_impl(pifpaf_net_t* net, const float* images_dev, int32_t 
                 const int tiles = g.m_blocks * g.n_blocks;
                 int grid = std::min(tiles, n_sm);
                 if (g.b_resident) grid = std::max(1, std::min(n_sm / g.n_blocks, g.m_blocks)) * g.n_blocks;
-                auto* kern = g.block_n <= NGROUP ? k_gemm_wg<1> : g.block_n <= 2 * NGROUP ? k_gemm_wg<2>
-                             : g.block_n <= 3 * NGROUP ? k_gemm_wg<3> : k_gemm_wg<4>;
+                if (g.tma_store && op.store_rows != g.M) {
+                    for (size_t i = 0; i < op.store_views.size(); i++) {
+                        const Op::StoreView& v = op.store_views[i];
+                        const int rc = make_tmap_store(&op.smaps.m[i], v.base, (uint64_t)g.M, (uint64_t)v.cols, (uint64_t)v.ld);
+                        if (rc != PIFPAF_OK) return rc;
+                    }
+                    op.store_rows = g.M;
+                }
+                auto* kern = GEMM_KERNELS[tile_groups(g.block_n)][tile_last(g.block_n)];
                 PIFPAF_CUDA_TRY(launch_k(pdl, kern, dim3(grid), dim3(GEMM_THREADS), op.smem, st, op.tmap_a, op.tmap_b,
-                                         g.src_tma ? op.tmap_src : op.tmap_a, g));
+                                         g.src_tma ? op.tmap_src : op.tmap_a, op.smaps, g));
             }
             PIFPAF_LAUNCH_CHECK();
         }
