@@ -350,11 +350,14 @@ int pifpaf_net_forward_u8(pifpaf_net_t* net, const uint8_t* images_nhwc_dev, int
 
 /* Same as pifpaf_net_forward but brackets every op with CUDA events on `stream` and, after a final
  * synchronise, writes per-op milliseconds to op_ms[num_ops] (profiling leg of bench.py; never the
- * headline timing).  op_kind[i]: 0 input conv, 1 wgmma GEMM, 2 depthwise conv, 3 fused depthwise -> GEMM; op_flops/op_bytes are
- * the algorithmic FLOPs and bytes (inputs + outputs + weights, each once) of op i for this batch. */
+ * headline timing).  op_kind[i]: 0 input conv, 1 wgmma GEMM, 2 depthwise conv, 3 fused kernels; op_flops/op_bytes are
+ * the algorithmic FLOPs and bytes (inputs + outputs + weights, each once) of op i for this batch.  A 1x1 GEMM fused
+ * into the stride-2 depthwise conv after it (PIFPAF_FUSE_PW_DW, on by default) launches nothing: kind 3, 0 FLOPs,
+ * 0 bytes; the depthwise op then reports the fused launch (kind 3, the FLOPs of both ops). */
 int pifpaf_net_forward_timed(pifpaf_net_t* net, const float* images_dev, int32_t batch, int32_t gemm_impl,
                              void* stream, float* op_ms, int32_t* op_kind, double* op_flops, double* op_bytes);
-/* Debug/parity tap: copy activation tensor `id` (first `batch` images) to host as f32 [B][h][w][c_phys]. */
+/* Debug/parity tap: copy activation tensor `id` (first `batch` images) to host as f32 [B][h][w][c_phys].  A 1x1
+ * output the last forward kept inside the fused 1x1 -> depthwise kernel is computed first (its GEMM runs again). */
 int pifpaf_net_tap_tensor(pifpaf_net_t* net, int32_t id, int32_t batch, float* out, int64_t out_elems);
 /* Debug/parity: fill activation tensor `id` (first `batch` images) from host f32 [B][h][w][c_phys] (rounded to bf16). */
 int pifpaf_net_set_tensor(pifpaf_net_t* net, int32_t id, int32_t batch, const float* data, int64_t n_elems);

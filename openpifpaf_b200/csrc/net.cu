@@ -910,6 +910,82 @@ __device__ __forceinline__ void dw_advance_cf(DwPos& p, const DwPos& d, int cblk
     p.b += d.b + carry;
 }
 
+// One warp's share of a depthwise 5x5 item: the 4 x BW output pixels at (oy0, ox0) of image b, lane = the channel
+// pair c0, c0 + 1; bias initialises the f32 sums, the 25 taps run in (ky, kx) order, a.relu, bf16 stores.
+// win: the item's input window in shared memory, IW pixels per row, 128 bytes (64 channels) per pixel; p0: the
+// window pixel at the block's first tap.  SWZ: the 16-byte units of pixel p sit at unit ^ (p & 7) (k_pw_dw's
+// intermediate window, which its wgmma epilogue writes without bank conflicts that way); the eight possible units
+// are resolved once per block, so the loads need no address arithmetic.
+template <int S, int BW, int IW, bool SWZ>
+__device__ __forceinline__ void dw5_block(const DwArgs& a, const unsigned char* win, int p0, int lane,
+                                          const float (&wgt)[25][2], float bias0, float bias1, int b, int oy0,
+                                          int ox0, int c0) {
+    constexpr int WIN_Y = 3 * S + 5, WIN_X = (BW - 1) * S + 5;
+    const unsigned char* tile = win + p0 * 128 + (SWZ ? (lane & 3) * 4 : lane * 4);
+    const unsigned char* rows[SWZ ? 8 : 1];          // SWZ: the lane's word in a pixel p with p & 7 == c
+#pragma unroll
+    for (int c = 0; c < (SWZ ? 8 : 1); c++) rows[c] = tile + (SWZ ? ((lane >> 2) ^ ((p0 + c) & 7)) << 4 : 0);
+    float acc[4][BW][2];
+#pragma unroll
+    for (int i = 0; i < 4; i++)
+#pragma unroll
+        for (int j = 0; j < BW; j++) { acc[i][j][0] = bias0; acc[i][j][1] = bias1; }
+#pragma unroll
+    for (int ry = 0; ry < WIN_Y; ry++) {
+        float f[WIN_X][2];
+#pragma unroll
+        for (int cx = 0; cx < WIN_X; cx++) {
+            const int p = ry * IW + cx;
+            const uint32_t v = *reinterpret_cast<const uint32_t*>(rows[SWZ ? p & 7 : 0] + p * 128);
+            f[cx][0] = __uint_as_float(v << 16);
+            f[cx][1] = __uint_as_float(v & 0xffff0000u);
+        }
+#pragma unroll
+        for (int i = 0; i < 4; i++) {
+            const int ky = ry - i * S;                    // compile-time after unrolling
+            if (ky < 0 || ky >= 5) continue;
+#pragma unroll
+            for (int kx = 0; kx < 5; kx++) {
+#pragma unroll
+                for (int j = 0; j < BW; j++) {
+                    acc[i][j][0] = fmaf(f[j * S + kx][0], wgt[ky * 5 + kx][0], acc[i][j][0]);
+                    acc[i][j][1] = fmaf(f[j * S + kx][1], wgt[ky * 5 + kx][1], acc[i][j][1]);
+                }
+            }
+        }
+    }
+    if (a.relu) {
+#pragma unroll
+        for (int i = 0; i < 4; i++)
+#pragma unroll
+            for (int j = 0; j < BW; j++) {
+                acc[i][j][0] = fmaxf(acc[i][j][0], 0.f); acc[i][j][1] = fmaxf(acc[i][j][1], 0.f);
+            }
+    }
+    const size_t out_row = (size_t)a.Wout * a.ld_out;           // elements per output image row
+    __nv_bfloat16* orow = a.out + ((size_t)(b * a.Hout + oy0) * a.Wout + ox0) * a.ld_out + a.out_col_off + c0;
+    if (oy0 + 4 <= a.Hout && ox0 + BW <= a.Wout) {          // interior block: no per-pixel predicates
+#pragma unroll
+        for (int i = 0; i < 4; i++) {
+            __nv_bfloat16* op = orow + i * out_row;
+#pragma unroll
+            for (int j = 0; j < BW; j++)
+                *reinterpret_cast<uint32_t*>(op + (size_t)j * a.ld_out) = pack_bf16(acc[i][j][0], acc[i][j][1]);
+        }
+    } else {
+#pragma unroll
+        for (int i = 0; i < 4; i++) {
+            if (oy0 + i >= a.Hout) continue;
+            __nv_bfloat16* op = orow + i * out_row;
+#pragma unroll
+            for (int j = 0; j < BW; j++) {
+                if (ox0 + j >= a.Wout) continue;
+                *reinterpret_cast<uint32_t*>(op + (size_t)j * a.ld_out) = pack_bf16(acc[i][j][0], acc[i][j][1]);
+            }
+        }
+    }
+}
+
 template <int S, int TH, int TW, int BW, int NSTAGE, bool CBF = false>
 __global__ void __launch_bounds__(DwTile<S, TH, TW, BW, NSTAGE>::THREADS, 2)
 k_dwconv5_tma(const __grid_constant__ CUtensorMap tmap_in, DwArgs a) {
@@ -964,7 +1040,6 @@ k_dwconv5_tma(const __grid_constant__ CUtensorMap tmap_in, DwArgs a) {
     const DwPos step = decompose(gridDim.x);
     const DwPos step_ring = decompose(NSTAGE * gridDim.x);
     DwPos pos = decompose(blockIdx.x);
-    const size_t out_row = (size_t)a.Wout * a.ld_out;           // elements per output image row
     int buf = 0; uint32_t phase = 0;
     int w_cblk = -1;
     float wgt[25][2];
@@ -990,67 +1065,9 @@ k_dwconv5_tma(const __grid_constant__ CUtensorMap tmap_in, DwArgs a) {
         // every warp waits (also those whose block lies past the image edge): passing this wait proves that all
         // warps counted out of the slot's previous item, so the per-slot count never mixes two items
         mbar_wait(&full[buf], phase);
-        if (oy0 < a.Hout && ox0 < a.Wout && c0 < C) {
-            const unsigned char* tile = dsm + (size_t)buf * T::BYTES + lane * 4 +
-                                        ((by * 4 * S) * T::IW + bx * BW * S) * 128;
-            float acc[4][BW][2];
-#pragma unroll
-            for (int i = 0; i < 4; i++)
-#pragma unroll
-                for (int j = 0; j < BW; j++) { acc[i][j][0] = bias0; acc[i][j][1] = bias1; }
-#pragma unroll
-            for (int ry = 0; ry < T::WIN_Y; ry++) {
-                float f[T::WIN_X][2];
-#pragma unroll
-                for (int cx = 0; cx < T::WIN_X; cx++) {
-                    const uint32_t v = *reinterpret_cast<const uint32_t*>(tile + (ry * T::IW + cx) * 128);
-                    f[cx][0] = __uint_as_float(v << 16);
-                    f[cx][1] = __uint_as_float(v & 0xffff0000u);
-                }
-#pragma unroll
-                for (int i = 0; i < 4; i++) {
-                    const int ky = ry - i * S;                    // compile-time after unrolling
-                    if (ky < 0 || ky >= 5) continue;
-#pragma unroll
-                    for (int kx = 0; kx < 5; kx++) {
-#pragma unroll
-                        for (int j = 0; j < BW; j++) {
-                            acc[i][j][0] = fmaf(f[j * S + kx][0], wgt[ky * 5 + kx][0], acc[i][j][0]);
-                            acc[i][j][1] = fmaf(f[j * S + kx][1], wgt[ky * 5 + kx][1], acc[i][j][1]);
-                        }
-                    }
-                }
-            }
-            if (a.relu) {
-#pragma unroll
-                for (int i = 0; i < 4; i++)
-#pragma unroll
-                    for (int j = 0; j < BW; j++) {
-                        acc[i][j][0] = fmaxf(acc[i][j][0], 0.f); acc[i][j][1] = fmaxf(acc[i][j][1], 0.f);
-                    }
-            }
-            __nv_bfloat16* orow = a.out + ((size_t)(pos.b * a.Hout + oy0) * a.Wout + ox0) * a.ld_out + a.out_col_off + c0;
-            if (oy0 + 4 <= a.Hout && ox0 + BW <= a.Wout) {          // interior block: no per-pixel predicates
-#pragma unroll
-                for (int i = 0; i < 4; i++) {
-                    __nv_bfloat16* op = orow + i * out_row;
-#pragma unroll
-                    for (int j = 0; j < BW; j++)
-                        *reinterpret_cast<uint32_t*>(op + (size_t)j * a.ld_out) = pack_bf16(acc[i][j][0], acc[i][j][1]);
-                }
-            } else {
-#pragma unroll
-                for (int i = 0; i < 4; i++) {
-                    if (oy0 + i >= a.Hout) continue;
-                    __nv_bfloat16* op = orow + i * out_row;
-#pragma unroll
-                    for (int j = 0; j < BW; j++) {
-                        if (ox0 + j >= a.Wout) continue;
-                        *reinterpret_cast<uint32_t*>(op + (size_t)j * a.ld_out) = pack_bf16(acc[i][j][0], acc[i][j][1]);
-                    }
-                }
-            }
-        }
+        if (oy0 < a.Hout && ox0 < a.Wout && c0 < C)
+            dw5_block<S, BW, T::IW, false>(a, dsm + (size_t)buf * T::BYTES, (by * 4 * S) * T::IW + bx * BW * S, lane,
+                                           wgt, bias0, bias1, pos.b, oy0, ox0, c0);
         // count this warp out of the slot; the last one out re-arms it.  Every shared-memory read of the slot has
         // been consumed by an fma above (results are in registers), the fence orders them before the count.
         __syncwarp();
@@ -1335,6 +1352,195 @@ size_t fused_smem_bytes(int ws, int bs, int block_n, int n_pad, int c_dw) {
            (size_t)n_pad * 5 + (size_t)c_dw * 26 * 4 + STG_BYTES + (size_t)(2 * (ws + bs)) * 8 + 64;
 }
 
+// ------------------------------------------------------------------ fused 1x1 GEMM -> depthwise 5x5
+// InvertedResidualK branch2 head (basenetworks.py:214-218: 1x1, BN, ReLU, dw5x5 stride 2, BN) of the stage-entry
+// block whose 1x1 reads the stem output (at most 32 channels) as ONE kernel: the 1x1 output -- the largest activation
+// of the network -- never visits HBM.  The 1x1 is recomputed on each item's input window instead: the halo of a
+// stride-2 5x5 window re-reads 1.3x the pixels, and 32-channel k16 steps cost the tensor core next to nothing.
+// Persistent CTA over (image, tile row, tile column) items of TH x TW output pixels:
+//   last warp  TMA producer: the item's window of the 1x1 input, IH x IW pixels x 32 channels (4-D box, zero fill,
+//              64-byte swizzle: the K-major wgmma layout of 64-byte rows) into a 2-deep ring
+//   the others per 64-channel block of the 1x1 output: the warpgroups multiply 64-pixel row chunks of the window
+//              by the block's resident weights (2 x wgmma.m64n64k16, the k16 steps and f32 epilogue of k_gemm_wg:
+//              bit-identical to the t_c that k_gemm_wg would write), bias + ReLU, bf16 into the intermediate window
+//              (128 bytes per pixel, 16-byte units XOR (pixel & 7)).  Pixels outside the image are written as 0, not
+//              relu(bias): the depthwise conv zero-pads ITS input, the 1x1 output.  Then, after a barrier, the
+//              depthwise FMA loop of k_dwconv5_tma (dw5_block, one 4 x BW output block per warp) on that block; a
+//              second barrier before the next block's epilogue overwrites the intermediate.
+// Resident per CTA, staged before the grid-dependency wait: the 1x1 weights [cblks * 64][32] bf16 (64-byte swizzle)
+// and bias, the depthwise weights [25][C] f32 and bias.
+template <int S, int TH, int TW, int BW>
+struct PwDwTile {
+    static constexpr int IH = (TH - 1) * S + 5, IW = (TW - 1) * S + 5;
+    static constexpr int NPIX = IH * IW;
+    static constexpr int CHUNKS = (NPIX + WG_ROWS - 1) / WG_ROWS;      // 64-row wgmma chunks of the window
+    static constexpr int IN_BYTES = CHUNKS * WG_ROWS * 64;             // 64-byte rows; the tail rows are never stored
+    static constexpr int MID_BYTES = NPIX * 128;
+    static constexpr int NSTAGE = 2;
+    static constexpr int WARPS = (TH / 4) * (TW / BW);               // consumer warps: one 4 x BW depthwise block each
+    static constexpr int WGS = WARPS / 4;                             // ... forming this many wgmma warpgroups
+    static constexpr int THREADS = 32 * (WARPS + 1);
+    static_assert(WARPS % 4 == 0, "whole warpgroups");
+};
+constexpr int PWDW_K = 32;       // 1x1 input channels the window carries (64-byte pixel rows)
+
+struct PwDwArgs {
+    DwArgs dw;                   // the depthwise op (dw.in: the elided 1x1 output, not read)
+    const __nv_bfloat16* w1; int ldw1, n1;   // 1x1 weights [n1][ldw1] bf16 (ldw1 <= PWDW_K), bias [n1] f32
+    const float* b1; int relu1;
+    int Hin, Win;                // the 1x1 input == the depthwise input grid
+    int cblks;                   // 64-channel blocks of the depthwise
+};
+
+// K-major, SWIZZLE_64B shared-memory matrix descriptor of wgmma: 64-byte rows, SBO = 512 B (8 rows), layout 64B (2)
+__device__ __forceinline__ uint64_t make_smem_desc_64b(uint32_t smem_addr) {
+    uint64_t d = 0;
+    d |= static_cast<uint64_t>((smem_addr >> 4) & 0x3fffu);
+    d |= static_cast<uint64_t>(1u) << 16;
+    d |= static_cast<uint64_t>(512u >> 4) << 32;
+    d |= static_cast<uint64_t>(2u) << 62;
+    return d;
+}
+
+size_t pw_dw_smem_bytes(int in_bytes, int mid_bytes, int cblks, int c_dw) {
+    return 1024 + 2 * (size_t)in_bytes + (size_t)mid_bytes + (size_t)cblks * 64 * (PWDW_K * 2 + 4) + (size_t)c_dw * 26 * 4;
+}
+
+template <int S, int TH, int TW, int BW>
+__global__ void __launch_bounds__(PwDwTile<S, TH, TW, BW>::THREADS, 1)
+k_pw_dw(const __grid_constant__ CUtensorMap tmap_in, PwDwArgs f) {
+    using T = PwDwTile<S, TH, TW, BW>;
+    extern __shared__ __align__(1024) unsigned char smem_raw[];
+    // align with pointer arithmetic on the array itself: the compiler keeps the shared address space (LDS / STS
+    // instead of generic loads and stores)
+    unsigned char* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+    __shared__ uint64_t full[T::NSTAGE], empty[T::NSTAGE];
+    const DwArgs& a = f.dw;
+    const int C = a.C8 * 8;
+    const int c_pad = f.cblks * 64;
+    // the wgmma operands (window ring, 1x1 weights) start on multiples of 4 KB, as the swizzle patterns require
+    unsigned char* in_s = smem;                                       // [NSTAGE][IN_BYTES]
+    unsigned char* w1_s = in_s + T::NSTAGE * T::IN_BYTES;             // [c_pad][64 B]
+    unsigned char* mid = w1_s + (size_t)c_pad * PWDW_K * 2;           // [NPIX][128 B]
+    float* b1_s = reinterpret_cast<float*>(mid + T::MID_BYTES);       // [c_pad]
+    float* dww_s = b1_s + c_pad;                                      // [25][C] + bias [C]
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+
+    if (warp == T::WARPS && lane == 0) tma_prefetch_desc(&tmap_in);
+    // 1x1 weights: row n, 16-byte unit u at u ^ ((n >> 1) & 3) (the 64-byte swizzle TMA would have produced)
+    for (int i = threadIdx.x; i < c_pad * (PWDW_K / 8); i += T::THREADS) {
+        const int n = i / (PWDW_K / 8), u = i % (PWDW_K / 8);
+        uint4 v = make_uint4(0u, 0u, 0u, 0u);
+        if (n < f.n1 && u * 8 < f.ldw1) v = *reinterpret_cast<const uint4*>(f.w1 + (size_t)n * f.ldw1 + u * 8);
+        *reinterpret_cast<uint4*>(w1_s + n * 64 + ((u ^ ((n >> 1) & 3)) << 4)) = v;
+    }
+    for (int i = threadIdx.x; i < c_pad; i += T::THREADS) b1_s[i] = i < f.n1 ? f.b1[i] : 0.f;
+    for (int i = threadIdx.x; i < 25 * C; i += T::THREADS) dww_s[i] = a.weight[i];
+    for (int i = threadIdx.x; i < C; i += T::THREADS) dww_s[25 * C + i] = a.bias[i];
+    if (threadIdx.x == 0) {
+        for (int s = 0; s < T::NSTAGE; s++) { mbar_init(&full[s], 1); mbar_init(&empty[s], T::WARPS); }
+        fence_barrier_init();
+    }
+    fence_proxy_async_shared();          // the weight tile is read by wgmma (async proxy)
+    __syncthreads();
+    pdl_launch_dependents();
+    pdl_wait();
+
+    const int tiles_x = (a.Wout + TW - 1) / TW, tiles_y = (a.Hout + TH - 1) / TH;
+    const int per_img = tiles_y * tiles_x;
+    const int total = a.B * per_img;
+
+    if (warp == T::WARPS) {
+        // ===== TMA producer =====
+        if (lane == 0) {
+            int s = 0; uint32_t ph = 0;
+            for (int w = blockIdx.x; w < total; w += gridDim.x) {
+                const int b = w / per_img, t = w - b * per_img;
+                const int ty = t / tiles_x, tx = t - ty * tiles_x;
+                mbar_wait(&empty[s], ph ^ 1);
+                mbar_expect_tx(&full[s], (uint32_t)(T::NPIX * PWDW_K * 2));
+                tma_load_4d(in_s + (size_t)s * T::IN_BYTES, &tmap_in, &full[s], 0, tx * TW * S - a.pad,
+                            ty * TH * S - a.pad, b);
+                if (++s == T::NSTAGE) { s = 0; ph ^= 1; }
+            }
+        }
+        return;
+    }
+    // ===== consumer warps: 1x1 row chunks (per warpgroup), then one 4 x BW depthwise block each =====
+    const int wg = warp >> 2;
+    const int by = warp / (TW / BW), bx = warp % (TW / BW);
+    const int q = lane & 3;
+    float acc[32];
+#pragma unroll
+    for (int i = 0; i < 32; i++) acc[i] = 0.f;
+    int s = 0; uint32_t ph = 0;
+    for (int w = blockIdx.x; w < total; w += gridDim.x) {
+        const int b = w / per_img, t = w - b * per_img;
+        const int ty = t / tiles_x, tx = t - ty * tiles_x;
+        const int iy0 = ty * TH * S - a.pad, ix0 = tx * TW * S - a.pad;
+        const uint32_t a_s = smem_u32(in_s + (size_t)s * T::IN_BYTES);
+        mbar_wait(&full[s], ph);
+        for (int cb = 0; cb < f.cblks; cb++) {
+            const uint32_t b_s = smem_u32(w1_s + (size_t)cb * 64 * PWDW_K * 2);
+            for (int mc = wg; mc < T::CHUNKS; mc += T::WGS) {
+                fence_acc(acc);
+                wgmma_fence();
+#pragma unroll
+                for (int k = 0; k < PWDW_K / MMA_K; k++)
+                    wgmma_n64(acc, make_smem_desc_64b(a_s + mc * WG_ROWS * PWDW_K * 2 + k * MMA_K * 2),
+                              make_smem_desc_64b(b_s + k * MMA_K * 2), k == 0 ? 0u : 1u);
+                wgmma_commit();
+                wgmma_wait<0>();
+                fence_acc(acc);
+                // epilogue (k_gemm_wg's): bias + ReLU in f32, bf16; rows r and r + 8 of this warp's 16
+#pragma unroll
+                for (int h = 0; h < 2; h++) {
+                    const int r = mc * WG_ROWS + (warp & 3) * 16 + (lane >> 2) + 8 * h;
+                    if (r >= T::NPIX) continue;
+                    const int wy = r / T::IW, wx = r - wy * T::IW;
+                    const bool inside = (unsigned)(iy0 + wy) < (unsigned)f.Hin && (unsigned)(ix0 + wx) < (unsigned)f.Win;
+                    unsigned char* row = mid + r * 128 + q * 4;
+#pragma unroll
+                    for (int j = 0; j < 8; j++) {
+                        const float2 bb = *reinterpret_cast<const float2*>(b1_s + cb * 64 + 8 * j + 2 * q);
+                        float v0 = acc[4 * j + 2 * h] + bb.x, v1 = acc[4 * j + 2 * h + 1] + bb.y;
+                        if (f.relu1) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+                        *reinterpret_cast<uint32_t*>(row + ((j ^ (r & 7)) << 4)) = inside ? pack_bf16(v0, v1) : 0u;
+                    }
+                }
+            }
+            // the window slot is free once the last block's MMAs have read it
+            if (cb == f.cblks - 1) {
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&empty[s]);
+            }
+            asm volatile("bar.sync 1, %0;" ::"n"(32 * T::WARPS) : "memory");
+            const int c0 = cb * 64 + lane * 2;
+            const int oy0 = ty * TH + by * 4, ox0 = tx * TW + bx * BW;
+            if (oy0 < a.Hout && ox0 < a.Wout && c0 < C) {
+                float wgt[25][2];
+#pragma unroll
+                for (int tp = 0; tp < 25; tp++) {
+                    const float2 wv = *reinterpret_cast<const float2*>(dww_s + (size_t)tp * C + c0);
+                    wgt[tp][0] = wv.x; wgt[tp][1] = wv.y;
+                }
+                const float2 bv = *reinterpret_cast<const float2*>(dww_s + 25 * (size_t)C + c0);
+                dw5_block<S, BW, T::IW, true>(a, mid, (by * 4 * S) * T::IW + bx * BW * S, lane, wgt, bv.x, bv.y,
+                                              b, oy0, ox0, c0);
+            }
+            // every depthwise read of the intermediate is done before the next block's epilogue overwrites it
+            asm volatile("bar.sync 1, %0;" ::"n"(32 * T::WARPS) : "memory");
+        }
+        if (++s == T::NSTAGE) { s = 0; ph ^= 1; }
+    }
+}
+
+// stride 2, 8 x 16 output tiles (DwS2's shape: the smaller halo): 2 x 45 KB window ring + 85 KB intermediate + the
+// resident weights -> 1 CTA per SM.  4 x 2 depthwise blocks: 16 consumer warps (four warpgroups) instead of the 8
+// of 4 x 4 blocks -- both phases are latency bound at one CTA per SM, twice the warps hide twice the latency
+constexpr int PWDW_TH = 8, PWDW_TW = 16, PWDW_BW = 2;
+using PwDwS2 = PwDwTile<2, PWDW_TH, PWDW_TW, PWDW_BW>;
+
 // every (column groups, last group width) instantiation, indexed [NG - 1][LASTW / 16 - 1]: any block_n that is a
 // multiple of 16 up to 256 (192 for the fused op)
 using GemmKernel = decltype(&k_gemm_wg<1, 16>);
@@ -1574,16 +1780,18 @@ int make_tmap_conv(CUtensorMap* map, const void* base, uint64_t c, uint64_t w, u
 // No L2 promotion: the 128-byte channel block of a pixel is all the kernel wants from that pixel for a long time
 // (the channel block is the slowest work index) and pixel strides of 352 / 704 bytes leave most blocks straddling
 // 128-byte lines: a wider promotion fetches bytes nobody reads.
+// box_c / swz: k_pw_dw's window of a 32-channel 1x1 input is a 64-byte swizzled box of 32 channels (its wgmma layout)
 int make_tmap_dw(CUtensorMap* map, const void* base, uint64_t c, uint64_t w, uint64_t h, uint64_t b, uint64_t ld,
-                 uint32_t box_w, uint32_t box_h) {
+                 uint32_t box_w, uint32_t box_h, uint32_t box_c = 64,
+                 CUtensorMapSwizzle swz = CU_TENSOR_MAP_SWIZZLE_NONE) {
     PFN_encodeTiled fn = get_encode_fn();
     if (!fn) { pifpaf::set_error("cuTensorMapEncodeTiled entry point not available"); return PIFPAF_E_CUDA; }
     const cuuint64_t dims[4] = {c, w, h, b};
     const cuuint64_t strides[3] = {ld * 2, w * ld * 2, h * w * ld * 2};
-    const cuuint32_t box[4] = {64, box_w, box_h, 1};
+    const cuuint32_t box[4] = {box_c, box_w, box_h, 1};
     const cuuint32_t estr[4] = {1, 1, 1, 1};
     CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(base), dims, strides, box, estr,
-                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_NONE,
+                    CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_NONE,
                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) {
         pifpaf::set_error("cuTensorMapEncodeTiled (dw) failed (%d): c=%llu w=%llu h=%llu b=%llu ld=%llu box=%ux%u", (int)r,
@@ -1639,6 +1847,17 @@ struct Op {
     double bytes_per_image = 0;      // algorithmic activation bytes (inputs once + outputs once)
     double weight_bytes = 0;
     int n_real = 0;                  // output channels that are not padding (emit_gemm)
+    double a_bytes_per_image = 0;    // GEMM: the input part of bytes_per_image
+    double dw_out_bytes_per_image = 0;   // depthwise: the output part of bytes_per_image
+    std::vector<int> touches;        // tensor ids the op reads or writes (-1: none)
+    // fused 1x1 -> depthwise (plan_pw_dw): the GEMM op is elided (not launched) and the depthwise op right after it
+    // launches k_pw_dw with pw + tmap_pw instead
+    bool elided = false;
+    bool pw_dw = false;
+    PwDwArgs pw{};
+    CUtensorMap tmap_pw{};
+    size_t pw_smem = 0;
+    double pw_flops_per_image = 0, pw_bytes_per_image = 0, pw_weight_bytes = 0;
 };
 
 }  // namespace
@@ -1661,6 +1880,9 @@ struct pifpaf_net {
     int gemm_res_stages = 0;             // weights-resident GEMMs: split N further until this many A stages fit (PIFPAF_GEMM_RES_STAGES)
     bool dw_cbf = false;                 // stride-2 depthwise: channel-block-fastest item order (PIFPAF_DW_CBF=1)
     bool gemm_tma_store = true;          // plain / scatter 1x1 GEMMs store through TMA (PIFPAF_GEMM_TMA_STORE=0: per-lane stores)
+    bool fuse_pw_dw = true;              // 1x1 -> stride-2 depthwise pairs run as k_pw_dw (PIFPAF_FUSE_PW_DW=0: two kernels)
+    size_t pw_dw_planned = 0;            // ops.size() when plan_pw_dw last ran
+    int elided_batch = 0;                // > 0: the last forward elided GEMMs (at this batch); pifpaf_net_tap_tensor re-runs them
     int head_fields[4] = {0, 0, 0, 0}, head_comp[4] = {0, 0, 0, 0}, head_h = 0, head_w = 0;
     int in_h = 0, in_w = 0;
 };
@@ -1815,6 +2037,7 @@ int emit_gemm(pifpaf_net* net, Op& op, int in_tensor, int in_col_off, int k_cols
     op.n_real = n_real;
     op.flops_per_image = 2.0 * (double)op.rows_per_image * (double)nnz;
     op.bytes_per_image = (double)op.rows_per_image * k_real * 2.0;      // A read once (bf16); outputs added by the caller
+    op.a_bytes_per_image = op.bytes_per_image;
     op.weight_bytes = (double)nnz * 2.0;
     // the map covers the whole tensor; the view's first column is a TMA coordinate (16-byte aligned).
     // Columns past the view multiply zero weight rows (B is zero padded), columns past the tensor are zero filled.
@@ -1829,6 +2052,89 @@ void plan_tma_store_plain(const pifpaf_net* net, Op& op, const Tensor& to) {
     if (!net->gemm_tma_store) return;
     op.g.tma_store = 1;
     op.store_views = {Op::StoreView{to.data + op.g.out_col_off, pad8(op.g.N), to.c}};
+}
+
+// Decides, once all ops are known, which 1x1 GEMM -> depthwise pairs run as one k_pw_dw launch.  The GEMM qualifies
+// when it is plain (no residual, shuffle or implicit conv), reads one K block from column 0 of a tensor of at most
+// PWDW_K channels and writes column 0 of its output tensor; it is fused when the next op is the TMA depthwise 5x5,
+// stride 2, pad 2 reading that tensor from column 0, and no other op touches the tensor.
+int plan_pw_dw(pifpaf_net* net) {
+    net->pw_dw_planned = net->ops.size();
+    for (Op& op : net->ops) { op.elided = false; op.pw_dw = false; }
+    if (!net->fuse_pw_dw) return PIFPAF_OK;
+    for (size_t i = 0; i + 1 < net->ops.size(); i++) {
+        Op& gop = net->ops[i];
+        Op& dop = net->ops[i + 1];
+        if (gop.kind != OP_GEMM || dop.kind != OP_DW || !dop.dw_tma) continue;
+        const GemmArgs& g = gop.g;
+        const DwArgs& d = dop.dw;
+        if (g.mode != MODE_PLAIN || g.conv_k != 0 || g.res != nullptr || g.num_k_blocks != 1 || g.a_col0 != 0 ||
+            g.out_col_off != 0)
+            continue;
+        if (d.kernel != 5 || d.stride != 2 || d.pad != 2 || d.in != g.out || d.in_col_off != 0) continue;
+        const Tensor& tin = net->tensors[gop.a_tensor];
+        if (tin.c > PWDW_K) continue;
+        int t_mid = -1;
+        for (int t = 0; t < (int)net->tensors.size(); t++)
+            if (net->tensors[t].data == g.out) t_mid = t;
+        bool private_mid = t_mid >= 0;
+        for (size_t j = 0; j < net->ops.size() && private_mid; j++)
+            if (j != i && j != i + 1)
+                for (int t : net->ops[j].touches) private_mid = private_mid && t != t_mid;
+        const int cblks = (d.C8 + 7) / 8;
+        const size_t smem = pw_dw_smem_bytes(PwDwS2::IN_BYTES, PwDwS2::MID_BYTES, cblks, d.C8 * 8);
+        if (!private_mid || smem > 226 * 1024) continue;
+        PwDwArgs& p = dop.pw;
+        p.dw = d;
+        p.w1 = g.wgt; p.ldw1 = g.ldw; p.n1 = g.block_n * g.n_blocks; p.b1 = g.bias; p.relu1 = g.relu;
+        p.Hin = tin.h; p.Win = tin.w; p.cblks = cblks;
+        const int rc = make_tmap_dw(&dop.tmap_pw, tin.data, (uint64_t)tin.c, (uint64_t)tin.w, (uint64_t)tin.h,
+                                    (uint64_t)net->max_batch, (uint64_t)tin.c, PwDwS2::IW, PwDwS2::IH, PWDW_K,
+                                    CU_TENSOR_MAP_SWIZZLE_64B);
+        if (rc != PIFPAF_OK) return rc;
+        dop.pw_smem = smem;
+        // both ops' FLOPs; the 1x1 input read once, the depthwise output written once, the 1x1 weights
+        dop.pw_flops_per_image = gop.flops_per_image + dop.flops_per_image;
+        dop.pw_bytes_per_image = gop.a_bytes_per_image + dop.dw_out_bytes_per_image;
+        dop.pw_weight_bytes = gop.weight_bytes + dop.weight_bytes;
+        gop.elided = true;
+        dop.pw_dw = true;
+    }
+    return PIFPAF_OK;
+}
+
+int effective_sms(const pifpaf_net* net) { return net->sm_limit > 0 ? std::min(net->sm_limit, net->n_sm) : net->n_sm; }
+
+// one launch of a GEMM op (k_gemm_wg, or the SIMT debug kernel for gemm_impl == 1) at this batch
+int launch_gemm(pifpaf_net* net, Op& op, int batch, int gemm_impl, bool pdl, cudaStream_t st) {
+    const int n_sm = effective_sms(net);
+    GemmArgs g = op.g;
+    if (g.mode == MODE_HEADS)
+        for (int i = 0; i < net->n_heads; i++) g.head_base[i] = net->head_out[net->head_cur][i];
+    g.M = batch * op.rows_per_image;
+    g.m_blocks = g.conv_k > 0 ? batch * op.tiles_per_image : (g.M + BM - 1) / BM;
+    if (gemm_impl == 1) {
+        const long long jobs = (long long)g.m_blocks * 4 * (g.n_blocks * g.block_n / CHUNK);
+        const int grid = (int)std::min<long long>((jobs + 3) / 4, (long long)n_sm * 16);
+        k_gemm_simt<<<grid, 128, 0, st>>>(g);
+    } else {
+        const int tiles = g.m_blocks * g.n_blocks;
+        int grid = std::min(tiles, n_sm);
+        if (g.b_resident) grid = std::max(1, std::min(n_sm / g.n_blocks, g.m_blocks)) * g.n_blocks;
+        if (g.tma_store && op.store_rows != g.M) {
+            for (size_t i = 0; i < op.store_views.size(); i++) {
+                const Op::StoreView& v = op.store_views[i];
+                const int rc = make_tmap_store(&op.smaps.m[i], v.base, (uint64_t)g.M, (uint64_t)v.cols, (uint64_t)v.ld);
+                if (rc != PIFPAF_OK) return rc;
+            }
+            op.store_rows = g.M;
+        }
+        auto* kern = GEMM_KERNELS[tile_groups(g.block_n)][tile_last(g.block_n)];
+        PIFPAF_CUDA_TRY(launch_k(pdl, kern, dim3(grid), dim3(GEMM_THREADS), op.smem, st, op.tmap_a, op.tmap_b,
+                                 g.src_tma ? op.tmap_src : op.tmap_a, op.smaps, g));
+    }
+    PIFPAF_LAUNCH_CHECK();
+    return PIFPAF_OK;
 }
 
 }  // namespace
@@ -1855,6 +2161,9 @@ int pifpaf_net_create(pifpaf_net_t** out, int32_t device, int32_t max_batch) {
     if (const char* e = std::getenv("PIFPAF_PDL")) net->pdl = std::atoi(e) != 0;
     if (const char* e = std::getenv("PIFPAF_GEMM_RES_STAGES")) net->gemm_res_stages = std::atoi(e);
     if (const char* e = std::getenv("PIFPAF_GEMM_TMA_STORE")) net->gemm_tma_store = std::atoi(e) != 0;
+    if (const char* e = std::getenv("PIFPAF_FUSE_PW_DW")) net->fuse_pw_dw = std::atoi(e) != 0;
+    PIFPAF_CUDA_TRY(cudaFuncSetAttribute(k_pw_dw<2, PWDW_TH, PWDW_TW, PWDW_BW>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         226 * 1024));
     for (auto& row : GEMM_KERNELS)
         for (auto* k : row) PIFPAF_CUDA_TRY(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024));
     for (auto& row : DW_GEMM_KERNELS)
@@ -1930,6 +2239,7 @@ int pifpaf_net_input_conv(pifpaf_net_t* net, int32_t in_h, int32_t in_w, int32_t
     a.kernel = kernel; a.stride = stride; a.pad = pad; a.relu = relu;
     op.flops_per_image = 2.0 * ho * wo * c_out * 3.0 * kernel * kernel;
     op.bytes_per_image = (double)in_h * in_w * 3 * 4.0 + (double)ho * wo * c_out * 2.0;
+    op.touches = {out_tensor};
     net->in_h = in_h; net->in_w = in_w;
     net->ops.push_back(op);
     return PIFPAF_OK;
@@ -1978,6 +2288,7 @@ int pifpaf_net_conv1x1(pifpaf_net_t* net, int32_t in_tensor, int32_t in_col_off,
         if (rc != PIFPAF_OK) return rc;
     }
     plan_gemm_smem(g, &op.smem, g.src_tma != 0);
+    op.touches = {in_tensor, out_tensor, shuffle_src_tensor};
     net->ops.push_back(op);
     return PIFPAF_OK;
 }
@@ -2033,6 +2344,8 @@ int pifpaf_net_conv1x1_scatter(pifpaf_net_t* net, int32_t in_tensor, int32_t in_
     g.dest = d_groups;
     op.bytes_per_image += (double)op.rows_per_image * op.n_real * 2.0;
     plan_gemm_smem(g, &op.smem, false);
+    op.touches.assign(piece_tensor, piece_tensor + n_pieces);
+    op.touches.push_back(in_tensor);
     net->ops.push_back(op);
     return PIFPAF_OK;
 }
@@ -2071,6 +2384,7 @@ int pifpaf_net_conv(pifpaf_net_t* net, int32_t in_tensor, int32_t in_col_off, in
             plan_tma_store_plain(net, op, to);
         }
         plan_gemm_smem(g, &op.smem, false);
+        op.touches = {in_tensor, out_tensor, residual_tensor};
         net->ops.push_back(op);
         return PIFPAF_OK;
     }
@@ -2119,6 +2433,7 @@ int pifpaf_net_conv(pifpaf_net_t* net, int32_t in_tensor, int32_t in_col_off, in
     if (rc != PIFPAF_OK) return rc;
     rc = make_tmap(&op.tmap_b, d_w, (uint64_t)n_pad, (uint64_t)k_total, (uint64_t)k_total, (uint32_t)block_n);
     if (rc != PIFPAF_OK) return rc;
+    op.touches = {in_tensor, out_tensor, residual_tensor};
     net->ops.push_back(op);
     return PIFPAF_OK;
 }
@@ -2162,6 +2477,8 @@ int pifpaf_net_dwconv(pifpaf_net_t* net, int32_t in_tensor, int32_t in_col_off, 
         if (rc != PIFPAF_OK) return rc;
         op.dw_tma = true;
     }
+    op.touches = {in_tensor, out_tensor};
+    op.dw_out_bytes_per_image = (double)ho * wo * channels * 2.0;
     net->ops.push_back(op);
     return PIFPAF_OK;
 }
@@ -2263,6 +2580,8 @@ int pifpaf_net_dw_conv1x1_scatter(pifpaf_net_t* net, int32_t in_tensor, int32_t 
     if (rc != PIFPAF_OK) return rc;
     rc = make_tmap(&op.tmap_b, d_w, (uint64_t)n_pad, (uint64_t)k_pad, (uint64_t)k_pad, (uint32_t)block_n);
     if (rc != PIFPAF_OK) return rc;
+    op.touches.assign(piece_tensor, piece_tensor + n_pieces);
+    op.touches.push_back(in_tensor);
     net->ops.push_back(op);
     return PIFPAF_OK;
 }
@@ -2317,6 +2636,7 @@ int pifpaf_net_heads_upsampled(pifpaf_net_t* net, int32_t in_tensor, int32_t k_c
     g.hw = tin.h * tin.w; g.w = tin.w;
     g.up = up; g.up_low = low; g.out_h = out_h; g.out_w = out_w;
     net->n_heads = n_heads; net->head_h = out_h; net->head_w = out_w;
+    op.touches = {in_tensor};
     net->ops.push_back(op);
     return PIFPAF_OK;
 }
@@ -2347,8 +2667,13 @@ static int net_forward_impl(pifpaf_net_t* net, const float* images_dev, int32_t 
         net->setup_synced = true;
     }
     if (net->head_buffers == 2) net->head_cur ^= 1;
-    const int n_sm = net->sm_limit > 0 ? std::min(net->sm_limit, net->n_sm) : net->n_sm;
+    if (net->pw_dw_planned != net->ops.size()) {
+        const int rc = plan_pw_dw(net);
+        if (rc != PIFPAF_OK) return rc;
+    }
+    const int n_sm = effective_sms(net);
     int op_index = 0;
+    net->elided_batch = 0;
     // PDL between consecutive ops (not in the per-op timing pass: the events would sit between the launches; not for
     // the first op: its predecessor in the stream is a copy or another forward's decode, not one of these kernels)
     const bool pdl_on = net->pdl && events == nullptr && gemm_impl == 0;
@@ -2356,6 +2681,10 @@ static int net_forward_impl(pifpaf_net_t* net, const float* images_dev, int32_t 
         if (events) PIFPAF_CUDA_TRY(cudaEventRecord(events[op_index], st));
         const bool pdl = pdl_on && op_index > 0;
         op_index++;
+        if (op.elided && gemm_impl == 0) {          // computed inside the k_pw_dw launch of the next op
+            net->elided_batch = batch;
+            continue;
+        }
         if (op.kind == OP_INPUT_CONV) {
             InConvArgs a = op.ic;
             a.in = images_dev; a.B = batch;
@@ -2386,7 +2715,14 @@ static int net_forward_impl(pifpaf_net_t* net, const float* images_dev, int32_t 
         } else if (op.kind == OP_DW) {
             DwArgs a = op.dw;
             a.B = batch;
-            if (op.dw_tma && gemm_impl == 0) {
+            if (op.pw_dw && gemm_impl == 0) {
+                PwDwArgs p = op.pw;
+                p.dw.B = batch;
+                const long long total = (long long)batch * ((a.Hout + PWDW_TH - 1) / PWDW_TH) * ((a.Wout + PWDW_TW - 1) / PWDW_TW);
+                const int grid = (int)std::min<long long>(total, (long long)n_sm);     // 1 CTA per SM by shared memory
+                PIFPAF_CUDA_TRY(launch_k(pdl, k_pw_dw<2, PWDW_TH, PWDW_TW, PWDW_BW>, dim3(grid), dim3(PwDwS2::THREADS),
+                                         op.pw_smem, st, op.tmap_pw, p));
+            } else if (op.dw_tma && gemm_impl == 0) {
                 const int cblks = (a.C8 + 7) / 8;
                 // persistent grid == resident CTAs (stride 1: 2 per SM, stride 2: 1 per SM by shared memory)
                 if (a.stride == 1) {
@@ -2421,32 +2757,8 @@ static int net_forward_impl(pifpaf_net_t* net, const float* images_dev, int32_t 
             }
             PIFPAF_LAUNCH_CHECK();
         } else {
-            GemmArgs g = op.g;
-            if (g.mode == MODE_HEADS)
-                for (int i = 0; i < net->n_heads; i++) g.head_base[i] = net->head_out[net->head_cur][i];
-            g.M = batch * op.rows_per_image;
-            g.m_blocks = g.conv_k > 0 ? batch * op.tiles_per_image : (g.M + BM - 1) / BM;
-            if (gemm_impl == 1) {
-                const long long jobs = (long long)g.m_blocks * 4 * (g.n_blocks * g.block_n / CHUNK);
-                const int grid = (int)std::min<long long>((jobs + 3) / 4, (long long)n_sm * 16);
-                k_gemm_simt<<<grid, 128, 0, st>>>(g);
-            } else {
-                const int tiles = g.m_blocks * g.n_blocks;
-                int grid = std::min(tiles, n_sm);
-                if (g.b_resident) grid = std::max(1, std::min(n_sm / g.n_blocks, g.m_blocks)) * g.n_blocks;
-                if (g.tma_store && op.store_rows != g.M) {
-                    for (size_t i = 0; i < op.store_views.size(); i++) {
-                        const Op::StoreView& v = op.store_views[i];
-                        const int rc = make_tmap_store(&op.smaps.m[i], v.base, (uint64_t)g.M, (uint64_t)v.cols, (uint64_t)v.ld);
-                        if (rc != PIFPAF_OK) return rc;
-                    }
-                    op.store_rows = g.M;
-                }
-                auto* kern = GEMM_KERNELS[tile_groups(g.block_n)][tile_last(g.block_n)];
-                PIFPAF_CUDA_TRY(launch_k(pdl, kern, dim3(grid), dim3(GEMM_THREADS), op.smem, st, op.tmap_a, op.tmap_b,
-                                         g.src_tma ? op.tmap_src : op.tmap_a, op.smaps, g));
-            }
-            PIFPAF_LAUNCH_CHECK();
+            const int rc = launch_gemm(net, op, batch, gemm_impl, pdl, st);
+            if (rc != PIFPAF_OK) return rc;
         }
     }
     if (events) PIFPAF_CUDA_TRY(cudaEventRecord(events[op_index], st));
@@ -2486,9 +2798,13 @@ int pifpaf_net_forward_timed(pifpaf_net_t* net, const float* images_dev, int32_t
     for (size_t i = 0; i < n && rc == PIFPAF_OK; i++) {
         cudaEventElapsedTime(&op_ms[i], ev[i], ev[i + 1]);
         const Op& op = net->ops[i];
-        if (op_kind) op_kind[i] = op.kind == OP_INPUT_CONV ? 0 : (op.kind == OP_GEMM ? 1 : (op.kind == OP_DW ? 2 : 3));
-        if (op_flops) op_flops[i] = op.flops_per_image * batch;
-        if (op_bytes) op_bytes[i] = op.bytes_per_image * batch + op.weight_bytes;
+        const bool fused = gemm_impl == 0 && (op.elided || op.pw_dw);
+        if (op_kind) op_kind[i] = fused || op.kind == OP_FUSED ? 3 : (op.kind == OP_INPUT_CONV ? 0 : (op.kind == OP_GEMM ? 1 : 2));
+        // an elided GEMM launches nothing (its events bracket no work) and its work is counted in the fused launch
+        if (op_flops) op_flops[i] = !fused ? op.flops_per_image * batch : op.pw_dw ? op.pw_flops_per_image * batch : 0.0;
+        if (op_bytes)
+            op_bytes[i] = !fused ? op.bytes_per_image * batch + op.weight_bytes
+                                 : op.pw_dw ? op.pw_bytes_per_image * batch + op.pw_weight_bytes : 0.0;
     }
     for (auto& e : ev) cudaEventDestroy(e);
     return rc;
@@ -2500,6 +2816,14 @@ int pifpaf_net_tap_tensor(pifpaf_net_t* net, int32_t id, int32_t batch, float* o
     const long long n = (long long)batch * t.h * t.w * t.c;
     PIFPAF_CHECK_ARG(out != nullptr && out_elems >= n && batch <= net->max_batch, "output buffer too small");
     PIFPAF_CUDA_TRY(cudaSetDevice(net->device));
+    // a tensor the last forward elided (the 1x1 output inside k_pw_dw): its GEMM runs now, at that forward's batch.
+    // Its input (the stem output) is not overwritten within a forward, so this is what the two-kernel schedule wrote.
+    if (net->elided_batch > 0)
+        for (Op& op : net->ops)
+            if (op.elided && op.g.out == t.data) {
+                const int rc = launch_gemm(net, op, net->elided_batch, 0, false, 0);
+                if (rc != PIFPAF_OK) return rc;
+            }
     float* d_tmp = nullptr;
     PIFPAF_CUDA_TRY(cudaMalloc(reinterpret_cast<void**>(&d_tmp), sizeof(float) * n));
     k_bf16_to_f32<<<1024, 256>>>(t.data, d_tmp, n);

@@ -838,7 +838,8 @@ class CompiledNet:
 
     def forward_timed(self, image_batch, *, gemm_impl=0):
         """Profiling pass: per-op (ms, kind, flops, bytes); kind 0 input conv, 1 wgmma GEMM, 2 depthwise,
-        3 fused depthwise -> GEMM."""
+        3 fused kernels (depthwise -> GEMM, or 1x1 GEMM -> stride-2 depthwise: there the GEMM op launches nothing and
+        reports 0 FLOPs and 0 bytes, and the depthwise op reports the fused launch with the FLOPs of both)."""
         b, n = int(image_batch.shape[0]), self.num_ops
         ms = np.zeros((n,), dtype=np.float32)
         kind = np.zeros((n,), dtype=np.int32)
@@ -851,7 +852,9 @@ class CompiledNet:
         return ms, kind, flops, nbytes
 
     def tap(self, tensor_id, batch):
-        """Debug: activation tensor as float32 numpy [B,h,w,c_phys]."""
+        """Debug: activation tensor as float32 numpy [B,h,w,c_phys].  A 1x1 output that the last forward kept
+        inside the fused 1x1 -> depthwise kernel is computed first (its GEMM runs again at that forward's batch), so
+        the tap returns what the two-kernel schedule writes."""
         h, w, c = self.tensor_shapes[tensor_id]
         out = np.empty((batch, h, w, c), dtype=np.float32)
         _lib.check(self.lib.pifpaf_net_tap_tensor(self.handle, tensor_id, batch, _ptr(out), out.size))
