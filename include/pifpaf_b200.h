@@ -291,6 +291,21 @@ int pifpaf_net_conv(pifpaf_net_t* net, int32_t in_tensor, int32_t in_col_off, in
                     const float* bias, int32_t relu, int32_t out_tensor, int32_t out_col_off,
                     int32_t residual_tensor, int32_t residual_col_off);
 
+/* pifpaf_net_conv with dilated taps (torchvision ResNet layer4 under --resnet-block5-dilation,
+ * basenetworks.py:121-135): tap (ky, kx) reads input pixel (x - pad + kx * dilation, y - pad + ky * dilation); the
+ * output is (H + 2 * pad - dilation * (kernel - 1) - 1) / stride + 1 pixels high (likewise wide).  dilation > 1 needs
+ * stride 1.  pifpaf_net_conv is this entry point with dilation 1. */
+int pifpaf_net_conv_dilated(pifpaf_net_t* net, int32_t in_tensor, int32_t in_col_off, int32_t c_in,
+                            int32_t kernel, int32_t stride, int32_t pad, int32_t n_out, const float* weight,
+                            const float* bias, int32_t relu, int32_t out_tensor, int32_t out_col_off,
+                            int32_t residual_tensor, int32_t residual_col_off, int32_t dilation);
+
+/* 3x3 max pool, padding 1, stride 1 or 2 (torchvision ResNet's MaxPool2d(3, 2, 1) kept by --resnet-pool0-stride,
+ * basenetworks.py:85-93) on channels [in_col_off, in_col_off + channels) of in_tensor; taps outside the image are
+ * ignored (torch pads with -inf).  forward_timed reports it as op kind 4. */
+int pifpaf_net_maxpool(pifpaf_net_t* net, int32_t in_tensor, int32_t in_col_off, int32_t channels, int32_t stride,
+                       int32_t out_tensor, int32_t out_col_off);
+
 /* Depthwise kxk conv (basenetworks.py:228-231), weight [channels][k][k], + bias (folded BN) (+ReLU). */
 int pifpaf_net_dwconv(pifpaf_net_t* net, int32_t in_tensor, int32_t in_col_off, int32_t channels,
                       int32_t kernel, int32_t stride, int32_t pad, const float* weight, const float* bias,
@@ -350,7 +365,7 @@ int pifpaf_net_forward_u8(pifpaf_net_t* net, const uint8_t* images_nhwc_dev, int
 
 /* Same as pifpaf_net_forward but brackets every op with CUDA events on `stream` and, after a final
  * synchronise, writes per-op milliseconds to op_ms[num_ops] (profiling leg of bench.py; never the
- * headline timing).  op_kind[i]: 0 input conv, 1 wgmma GEMM, 2 depthwise conv, 3 fused kernels; op_flops/op_bytes are
+ * headline timing).  op_kind[i]: 0 input conv, 1 wgmma GEMM, 2 depthwise conv, 3 fused kernels, 4 max pool; op_flops/op_bytes are
  * the algorithmic FLOPs and bytes (inputs + outputs + weights, each once) of op i for this batch.  A 1x1 GEMM fused
  * into the stride-2 depthwise conv after it (PIFPAF_FUSE_PW_DW, on by default) launches nothing: kind 3, 0 FLOPs,
  * 0 bytes; the depthwise op then reports the fused launch (kind 3, the FLOPs of both ops). */

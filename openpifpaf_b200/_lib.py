@@ -83,6 +83,9 @@ SYMBOLS = {
                                                       c_i32, VP, VP, c_i32, c_i32, VP, VP, VP, VP]),
     'pifpaf_net_conv': (ctypes.c_int, [VP, c_i32, c_i32, c_i32, c_i32, c_i32, c_i32, c_i32, VP, VP, c_i32, c_i32, c_i32,
                                        c_i32, c_i32]),
+    'pifpaf_net_conv_dilated': (ctypes.c_int, [VP, c_i32, c_i32, c_i32, c_i32, c_i32, c_i32, c_i32, VP, VP, c_i32, c_i32,
+                                               c_i32, c_i32, c_i32, c_i32]),
+    'pifpaf_net_maxpool': (ctypes.c_int, [VP, c_i32, c_i32, c_i32, c_i32, c_i32, c_i32]),
     'pifpaf_net_dwconv': (ctypes.c_int, [VP, c_i32, c_i32, c_i32, c_i32, c_i32, c_i32, VP, VP, c_i32, c_i32, c_i32]),
     'pifpaf_net_heads': (ctypes.c_int, [VP, c_i32, c_i32, c_i32, VP, VP, VP, VP, VP]),
     'pifpaf_net_heads_upsampled': (ctypes.c_int, [VP, c_i32, c_i32, c_i32, VP, VP, VP, c_i32, VP, VP]),

@@ -234,8 +234,9 @@ struct GemmArgs {
     int hw, w;                   // pixels per image, field width (of the conv output)
     int up, up_low, out_h, out_w;   // PixelShuffle factor, low crop, head output size (== h, w when up == 1)
     // implicit-GEMM convolution (conv_k > 0): one M tile = a PH x PW patch of output pixels of one image;
-    // K blocks run over taps x 64-channel blocks; A comes from a 4-D tensor map {C, W, H, B}
-    int conv_k, conv_stride, conv_pad, conv_cblocks;
+    // K blocks run over taps x 64-channel blocks; A comes from a 4-D tensor map {C, W, H, B}; tap t reads input
+    // pixel (x * stride - pad + (t % k) * dil, y * stride - pad + (t / k) * dil)
+    int conv_k, conv_stride, conv_pad, conv_dil, conv_cblocks;
     int Hi, Wi, Ho, Wo, tiles_x, tiles_y;
     // residual add before the ReLU (torchvision BasicBlock / Bottleneck): res[m][res_col_off + n]
     const __nv_bfloat16* res; int ld_res; int res_col_off;
@@ -626,7 +627,8 @@ k_gemm_wg(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CU
                     if (g.conv_k > 0) {
                         const int tap = kb / g.conv_cblocks;
                         cb = kb - tap * g.conv_cblocks;
-                        tma_load_4d(sa, &tmap_a, &full_bar[stage], cb * BK, cx + tap % g.conv_k, cy + tap / g.conv_k, cimg);
+                        tma_load_4d(sa, &tmap_a, &full_bar[stage], cb * BK, cx + (tap % g.conv_k) * g.conv_dil,
+                                    cy + (tap / g.conv_k) * g.conv_dil, cimg);
                     } else {
                         tma_load_2d(sa, &tmap_a, &full_bar[stage], g.a_col0 + kb * BK, m_blk * BM);
                     }
@@ -732,8 +734,8 @@ __global__ void __launch_bounds__(128) k_gemm_simt(GemmArgs g) {
             } else {
                 const int ox = m % g.Wo, oy = (m / g.Wo) % g.Ho, b = m / (g.Wo * g.Ho);
                 for (int tap = 0; tap < g.conv_k * g.conv_k; tap++) {
-                    const int iy = oy * g.conv_stride - g.conv_pad + tap / g.conv_k;
-                    const int ix = ox * g.conv_stride - g.conv_pad + tap % g.conv_k;
+                    const int iy = oy * g.conv_stride - g.conv_pad + (tap / g.conv_k) * g.conv_dil;
+                    const int ix = ox * g.conv_stride - g.conv_pad + (tap % g.conv_k) * g.conv_dil;
                     if (iy < 0 || iy >= g.Hi || ix < 0 || ix >= g.Wi) continue;
                     const __nv_bfloat16* ap = g.a + ((size_t)(b * g.Hi + iy) * g.Wi + ix) * g.lda;
                     for (int k = 0; k < g.K; k++) {
@@ -1094,6 +1096,42 @@ k_dwconv5_tma(const __grid_constant__ CUtensorMap tmap_in, DwArgs a) {
 constexpr int DW1_TH = 8, DW1_TW = 16, DW2_TH = 8, DW2_TW = 16;
 using DwS1 = DwTile<1, DW1_TH, DW1_TW, 4, 3>;
 using DwS2 = DwTile<2, DW2_TH, DW2_TW, 4, 2>;
+
+// 3x3 max pool, pad 1, stride a.stride (torchvision's MaxPool2d(3, 2, 1) in the ResNet input block,
+// basenetworks.py:85-93): one output pixel x 8 channels (one 16-byte vector) per thread.  Taps outside the image are
+// skipped, as torch's -inf padding does; the centre tap is always inside.  The weight / bias fields of DwArgs are unused.
+__global__ void __launch_bounds__(256) k_maxpool(DwArgs a) {
+    pdl_launch_dependents();
+    pdl_wait();
+    const long long total = (long long)a.B * a.Hout * a.Wout * a.C8;
+    for (long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x; t < total;
+         t += (long long)gridDim.x * blockDim.x) {
+        const int c8 = (int)(t % a.C8);
+        long long p = t / a.C8;
+        const int ox = (int)(p % a.Wout); p /= a.Wout;
+        const int oy = (int)(p % a.Hout);
+        const int b = (int)(p / a.Hout);
+        const __nv_bfloat162 ninf = __bfloat162bfloat162(__ushort_as_bfloat16((unsigned short)0xff80u));
+        __nv_bfloat162 m[4] = {ninf, ninf, ninf, ninf};
+#pragma unroll
+        for (int ky = 0; ky < 3; ky++) {
+            const int iy = oy * a.stride - 1 + ky;
+            if (iy < 0 || iy >= a.Hin) continue;
+#pragma unroll
+            for (int kx = 0; kx < 3; kx++) {
+                const int ix = ox * a.stride - 1 + kx;
+                if (ix < 0 || ix >= a.Win) continue;
+                const uint4 v = __ldg(reinterpret_cast<const uint4*>(
+                    a.in + ((size_t)(b * a.Hin + iy) * a.Win + ix) * a.ld_in + a.in_col_off + c8 * 8));
+                const __nv_bfloat162* h = reinterpret_cast<const __nv_bfloat162*>(&v);
+#pragma unroll
+                for (int j = 0; j < 4; j++) m[j] = __hmax2(m[j], h[j]);
+            }
+        }
+        *reinterpret_cast<uint4*>(a.out + ((size_t)(b * a.Hout + oy) * a.Wout + ox) * a.ld_out + a.out_col_off + c8 * 8) =
+            *reinterpret_cast<const uint4*>(m);
+    }
+}
 
 // generic depthwise kxk (any kernel/stride): one output pixel x 8 channels per thread
 __global__ void __launch_bounds__(256) k_dwconv(DwArgs a) {
@@ -1820,7 +1858,7 @@ cudaError_t launch_k(bool pdl, void (*kernel)(KArgs...), dim3 grid, dim3 block, 
 
 struct Tensor { int h, w, c; __nv_bfloat16* data; };
 
-enum OpKind { OP_INPUT_CONV, OP_GEMM, OP_DW, OP_FUSED };
+enum OpKind { OP_INPUT_CONV, OP_GEMM, OP_DW, OP_FUSED, OP_MAXPOOL };
 
 struct Op {
     OpKind kind;
@@ -1835,7 +1873,7 @@ struct Op {
     std::vector<StoreView> store_views;
     StoreMaps smaps{};
     int store_rows = -1;
-    // dw
+    // dw, max pool
     DwArgs dw{};
     CUtensorMap tmap_dw{}; bool dw_tma = false;
     // fused depthwise -> GEMM (OP_FUSED): g + tmap_dw (windows) + tmap_b
@@ -2354,15 +2392,28 @@ int pifpaf_net_conv(pifpaf_net_t* net, int32_t in_tensor, int32_t in_col_off, in
                     int32_t kernel, int32_t stride, int32_t pad, int32_t n_out, const float* weight,
                     const float* bias, int32_t relu, int32_t out_tensor, int32_t out_col_off,
                     int32_t residual_tensor, int32_t residual_col_off) {
+    return pifpaf_net_conv_dilated(net, in_tensor, in_col_off, c_in, kernel, stride, pad, n_out, weight, bias, relu,
+                                   out_tensor, out_col_off, residual_tensor, residual_col_off, 1);
+}
+
+int pifpaf_net_conv_dilated(pifpaf_net_t* net, int32_t in_tensor, int32_t in_col_off, int32_t c_in,
+                            int32_t kernel, int32_t stride, int32_t pad, int32_t n_out, const float* weight,
+                            const float* bias, int32_t relu, int32_t out_tensor, int32_t out_col_off,
+                            int32_t residual_tensor, int32_t residual_col_off, int32_t dilation) {
     PIFPAF_CHECK_ARG(net != nullptr && weight != nullptr, "null argument");
     const int nt = (int)net->tensors.size();
     PIFPAF_CHECK_ARG(in_tensor >= 0 && in_tensor < nt && out_tensor >= 0 && out_tensor < nt, "bad tensor id");
     PIFPAF_CHECK_ARG(kernel >= 1 && kernel <= 7 && stride >= 1 && stride <= 2 && pad >= 0, "unsupported conv geometry");
+    PIFPAF_CHECK_ARG(dilation >= 1 && dilation <= 64, "conv dilation must be 1 to 64");
+    // the stride-2 tensor map steps over every other input pixel; dilated taps would need their own traversal
+    PIFPAF_CHECK_ARG(dilation == 1 || stride == 1, "a dilated conv (dilation > 1) must have stride 1");
     PIFPAF_CHECK_ARG(c_in >= 1 && n_out >= 1, "bad conv size");
     PIFPAF_CUDA_TRY(cudaSetDevice(net->device));
     const Tensor& tin = net->tensors[in_tensor];
     const Tensor& to = net->tensors[out_tensor];
-    const int ho = (tin.h + 2 * pad - kernel) / stride + 1, wo = (tin.w + 2 * pad - kernel) / stride + 1;
+    const int span = dilation * (kernel - 1) + 1;
+    PIFPAF_CHECK_ARG(tin.h + 2 * pad >= span && tin.w + 2 * pad >= span, "conv window larger than the padded input");
+    const int ho = (tin.h + 2 * pad - span) / stride + 1, wo = (tin.w + 2 * pad - span) / stride + 1;
     PIFPAF_CHECK_ARG(to.h == ho && to.w == wo, "conv output tensor shape mismatch");
     PIFPAF_CHECK_ARG(in_col_off % 8 == 0 && in_col_off + c_in <= tin.c, "conv input column window");
     PIFPAF_CHECK_ARG(out_col_off % 16 == 0 && out_col_off + pad8(n_out) <= to.c, "conv output column window");
@@ -2412,7 +2463,7 @@ int pifpaf_net_conv(pifpaf_net_t* net, int32_t in_tensor, int32_t in_col_off, in
     g.stages = choose_stages(block_n, n_blocks, g.num_k_blocks, false);
     g.bias = d_b; g.mode = MODE_PLAIN; g.relu = relu;
     g.out = to.data; g.ldo = to.c; g.out_col_off = out_col_off;
-    g.conv_k = kernel; g.conv_stride = stride; g.conv_pad = pad; g.conv_cblocks = cblocks;
+    g.conv_k = kernel; g.conv_stride = stride; g.conv_pad = pad; g.conv_dil = dilation; g.conv_cblocks = cblocks;
     g.Hi = tin.h; g.Wi = tin.w; g.Ho = ho; g.Wo = wo;
     g.tiles_x = (wo + PW - 1) / PW; g.tiles_y = (ho + PH - 1) / PH;
     g.a = tin.data + in_col_off; g.lda = tin.c; g.wgt = d_w; g.ldw = k_total;
@@ -2479,6 +2530,33 @@ int pifpaf_net_dwconv(pifpaf_net_t* net, int32_t in_tensor, int32_t in_col_off, 
     }
     op.touches = {in_tensor, out_tensor};
     op.dw_out_bytes_per_image = (double)ho * wo * channels * 2.0;
+    net->ops.push_back(op);
+    return PIFPAF_OK;
+}
+
+int pifpaf_net_maxpool(pifpaf_net_t* net, int32_t in_tensor, int32_t in_col_off, int32_t channels, int32_t stride,
+                       int32_t out_tensor, int32_t out_col_off) {
+    PIFPAF_CHECK_ARG(net != nullptr, "null argument");
+    const int nt = (int)net->tensors.size();
+    PIFPAF_CHECK_ARG(in_tensor >= 0 && in_tensor < nt && out_tensor >= 0 && out_tensor < nt, "bad tensor id");
+    PIFPAF_CHECK_ARG(stride == 1 || stride == 2, "max pool stride must be 1 or 2");
+    PIFPAF_CHECK_ARG(channels >= 1, "bad channel count");
+    const Tensor& tin = net->tensors[in_tensor];
+    const Tensor& to = net->tensors[out_tensor];
+    const int ho = (tin.h - 1) / stride + 1, wo = (tin.w - 1) / stride + 1;     // (h + 2 * 1 - 3) / s + 1
+    const int C = pad8(channels);
+    PIFPAF_CHECK_ARG(to.h == ho && to.w == wo, "max pool output tensor shape mismatch");
+    PIFPAF_CHECK_ARG(in_col_off % 8 == 0 && out_col_off % 8 == 0 && in_col_off + C <= tin.c && out_col_off + C <= to.c,
+                     "max pool column windows");
+    Op op; op.kind = OP_MAXPOOL;
+    DwArgs& a = op.dw;
+    a.in = tin.data; a.ld_in = tin.c; a.in_col_off = in_col_off;
+    a.out = to.data; a.ld_out = to.c; a.out_col_off = out_col_off;
+    a.Hin = tin.h; a.Win = tin.w; a.Hout = ho; a.Wout = wo; a.C8 = C / 8;
+    a.kernel = 3; a.stride = stride; a.pad = 1; a.relu = 0;
+    op.flops_per_image = 0;
+    op.bytes_per_image = ((double)tin.h * tin.w + (double)ho * wo) * channels * 2.0;
+    op.touches = {in_tensor, out_tensor};
     net->ops.push_back(op);
     return PIFPAF_OK;
 }
@@ -2556,7 +2634,7 @@ int pifpaf_net_dw_conv1x1_scatter(pifpaf_net_t* net, int32_t in_tensor, int32_t 
     g.N = n_out; g.K = C; g.block_n = block_n; g.n_blocks = n_blocks;
     g.num_k_blocks = (C + BK - 1) / BK;
     g.bias = d_b; g.mode = MODE_SCATTER; g.relu = relu; g.dest = d_groups;
-    g.conv_k = kernel; g.conv_stride = stride; g.conv_pad = pad; g.conv_cblocks = g.num_k_blocks;
+    g.conv_k = kernel; g.conv_stride = stride; g.conv_pad = pad; g.conv_dil = 1; g.conv_cblocks = g.num_k_blocks;
     g.Hi = tin.h; g.Wi = tin.w; g.Ho = tin.h; g.Wo = tin.w;
     g.tiles_x = (g.Wo + PW - 1) / PW; g.tiles_y = (g.Ho + PH - 1) / PH;
     op.a_tensor = in_tensor; op.rows_per_image = g.Ho * g.Wo; op.tiles_per_image = g.tiles_x * g.tiles_y;
@@ -2756,6 +2834,13 @@ static int net_forward_impl(pifpaf_net_t* net, const float* images_dev, int32_t 
                 k_dwconv<<<grid, 256, 0, st>>>(a);
             }
             PIFPAF_LAUNCH_CHECK();
+        } else if (op.kind == OP_MAXPOOL) {
+            DwArgs a = op.dw;
+            a.B = batch;
+            const long long total = (long long)batch * a.Hout * a.Wout * a.C8;
+            const int grid = (int)std::min<long long>((total + 255) / 256, (long long)n_sm * 32);
+            PIFPAF_CUDA_TRY(launch_k(pdl, k_maxpool, dim3(grid), dim3(256), 0, st, a));
+            PIFPAF_LAUNCH_CHECK();
         } else {
             const int rc = launch_gemm(net, op, batch, gemm_impl, pdl, st);
             if (rc != PIFPAF_OK) return rc;
@@ -2799,7 +2884,9 @@ int pifpaf_net_forward_timed(pifpaf_net_t* net, const float* images_dev, int32_t
         cudaEventElapsedTime(&op_ms[i], ev[i], ev[i + 1]);
         const Op& op = net->ops[i];
         const bool fused = gemm_impl == 0 && (op.elided || op.pw_dw);
-        if (op_kind) op_kind[i] = fused || op.kind == OP_FUSED ? 3 : (op.kind == OP_INPUT_CONV ? 0 : (op.kind == OP_GEMM ? 1 : 2));
+        if (op_kind)
+            op_kind[i] = op.kind == OP_MAXPOOL ? 4
+                       : fused || op.kind == OP_FUSED ? 3 : (op.kind == OP_INPUT_CONV ? 0 : (op.kind == OP_GEMM ? 1 : 2));
         // an elided GEMM launches nothing (its events bracket no work) and its work is counted in the fused launch
         if (op_flops) op_flops[i] = !fused ? op.flops_per_image * batch : op.pw_dw ? op.pw_flops_per_image * batch : 0.0;
         if (op_bytes)

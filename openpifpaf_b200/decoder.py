@@ -352,6 +352,7 @@ class CifDet(metaclass=_Statics):
         self.device = int(device)
         self._handle = None
         self._caps = None
+        self._pending = None
 
     def __getstate__(self):
         return (self.n_categories, self.device)
@@ -432,6 +433,15 @@ class CifDet(metaclass=_Statics):
                      suppression=0.1, instance_threshold=0.15, stream=None):
         """field_batch [B,F,6,h,w] CUDA float32.  nms=False: per image the raw (categories, scores, boxes) of
         CifDet::call; nms=True: the filtered detections of decoder/cifdet.py:55-64 (scores after suppression)."""
+        self.decode_batch_async(field_batch, stride, nms=nms, iou_threshold=iou_threshold,
+                                nms_by_category=nms_by_category, suppression=suppression,
+                                instance_threshold=instance_threshold, stream=stream)
+        return self.fetch(stream=stream)
+
+    def decode_batch_async(self, field_batch, stride, *, nms=False, iou_threshold=0.5, nms_by_category=True,
+                           suppression=0.1, instance_threshold=0.15, stream=None):
+        """Enqueue the decode of decode_batch on `stream` (default: the current stream of the fields' device) without
+        waiting for it; fetch() returns its results."""
         if not field_batch.is_cuda or field_batch.dtype != torch.float32:
             raise RuntimeError('decode_batch expects a CUDA float32 tensor (use call() for host fields)')
         field_batch = field_batch.contiguous()
@@ -446,12 +456,21 @@ class CifDet(metaclass=_Statics):
         st = stream if stream is not None else torch.cuda.current_stream(field_batch.device)
         _lib.check(_lib.lib().pifpaf_cifdet_decode_device(handle, field_batch.data_ptr(), B, h, w, int(stride),
                                                           ctypes.byref(p), ctypes.c_void_p(st.cuda_stream)))
-        cap = int(p.max_detections_before_nms)
+        self._pending = (B, int(p.max_detections_before_nms), bool(nms))
+
+    def fetch(self, *, stream=None):
+        """Results of the last decode_batch_async, copied back on `stream` (default: the current stream of the
+        decoder's device; give the stream the decode was enqueued on): per image (categories, scores, boxes)."""
+        pending, self._pending = getattr(self, '_pending', None), None
+        if pending is None:
+            raise RuntimeError('fetch() without a preceding decode_batch_async()')
+        B, cap, nms = pending
+        st = stream if stream is not None else torch.cuda.current_stream(self.device)
         counts = np.zeros((B,), dtype=np.int32)
         rec = np.empty((B, cap, 8), dtype=np.float32)
-        _lib.check(_lib.lib().pifpaf_cifdet_fetch(handle, counts.ctypes.data, rec.ctypes.data, cap,
+        _lib.check(_lib.lib().pifpaf_cifdet_fetch(self._handle, counts.ctypes.data, rec.ctypes.data, cap,
                                                   ctypes.c_void_p(st.cuda_stream)))
-        return [self._unpack(rec[b], int(counts[b]), bool(nms)) for b in range(B)]
+        return [self._unpack(rec[b], int(counts[b]), nms) for b in range(B)]
 
 
 def grow_connection_blend(caf, x, y, s, filter_sigmas=1.0, only_max=False):

@@ -50,6 +50,11 @@ def pad16(v):
 
 # ----------------------------------------------------------------------------- plans
 
+class UnsupportedModel(RuntimeError):
+    """plan_from_shell refuses the model: a module, option or head the compiled forward does not implement.  Callers
+    that have another way to run the model (the plugin's reference fallback) catch this and nothing else."""
+
+
 def _fold(conv, bn):
     """conv (bias-free) followed by eval BatchNorm -> (weight, bias) float32 numpy."""
     w = conv.weight.detach().double()
@@ -85,27 +90,78 @@ def _heads_plan(shell, base):
             'ops': head_ops(m.n_confidences, m.n_vectors, m.n_scales, tuple(m.vector_offsets)),
             'stride': int(base.stride) // up})
     if len({hd['upsample'] for hd in heads}) > 1:
-        raise RuntimeError('heads with different upsample_stride values are not supported')
+        raise UnsupportedModel('heads with different upsample_stride values are not supported')
     return heads
 
 
+def _resnet_input_block(input_block):
+    """The input block of basenetworks.py:71-150 as [(kind, modules)]: ('conv', (conv, bn)) for each conv + BN + ReLU
+    (the stem, and the optional --resnet-input-conv2-stride conv, nested in a Sequential of its own) and ('pool',
+    maxpool) for torchvision's max pool kept by --resnet-pool0-stride.  Anything else is refused."""
+    mods = []
+    for m in input_block:
+        mods += list(m) if isinstance(m, torch.nn.Sequential) else [m]
+    parts, i = [], 0
+    while i < len(mods):
+        m = mods[i]
+        if isinstance(m, torch.nn.Conv2d) and i + 2 < len(mods) and isinstance(mods[i + 1], torch.nn.BatchNorm2d) \
+                and isinstance(mods[i + 2], torch.nn.ReLU):
+            parts.append(('conv', (m, mods[i + 1])))
+            i += 3
+        elif isinstance(m, torch.nn.MaxPool2d):
+            if (_pair(m.kernel_size), _pair(m.padding), _pair(m.dilation), m.ceil_mode) != ((3, 3), (1, 1), (1, 1), False) \
+                    or _pair(m.stride) not in ((1, 1), (2, 2)):
+                raise UnsupportedModel('only a 3x3 max pool with padding 1 and stride 1 or 2 is supported')
+            parts.append(('pool', m))
+            i += 1
+        else:
+            raise UnsupportedModel(f'unsupported Resnet input block module {type(m).__name__}')
+    kinds = [k for k, _ in parts]
+    if kinds not in (['conv'], ['conv', 'pool'], ['conv', 'conv']):
+        raise UnsupportedModel(f'unsupported Resnet input block {kinds}: expected the stem conv, then a max pool or '
+                               'a second conv')
+    return parts
+
+
+def _pair(v):
+    return tuple(v) if isinstance(v, (tuple, list)) else (v, v)
+
+
 def _plan_from_resnet(shell):
-    """basenetworks.py:71-150: torchvision ResNet without the max-pool (input_block = conv1, bn1, relu;
-    block2..block5 = layer1..layer4 of BasicBlock / Bottleneck)."""
+    """basenetworks.py:71-150: torchvision ResNet (input_block = conv1, bn1, relu, then the max pool under
+    --resnet-pool0-stride or a 3x3 conv + BN + ReLU under --resnet-input-conv2-stride; block2..block5 = layer1..layer4
+    of BasicBlock / Bottleneck, layer4 dilated under --resnet-block5-dilation)."""
     base = shell.base_net
-    if len(base.input_block) != 3:
-        raise RuntimeError('only the default Resnet input block (conv, bn, relu; pool0_stride=0) is supported')
-    conv, bn = base.input_block[0], base.input_block[1]
+    if base.block5 is None:
+        # basenetworks.py:116-119,149: --resnet-remove-last-block leaves block5 = None, which the reference's own
+        # forward then calls
+        raise UnsupportedModel('Resnet with remove_last_block (block5 = None) is not supported: its forward fails')
+    for m in base.modules():
+        if isinstance(m, torch.nn.Conv2d) and m.groups != 1:
+            raise UnsupportedModel('grouped convolutions (ResNeXt) are not supported')
+
+    def conv_entry(c, n):
+        if len(set(_pair(c.kernel_size))) != 1 or len(set(_pair(c.stride))) != 1 or \
+                len(set(_pair(c.padding))) != 1 or len(set(_pair(c.dilation))) != 1:
+            raise UnsupportedModel('only square ResNet convolutions are supported')
+        w_, b_ = _fold(c, n)
+        e = {'w': w_, 'b': b_, 'kernel': int(c.kernel_size[0]), 'stride': int(c.stride[0]), 'pad': int(c.padding[0])}
+        if c.dilation[0] != 1:
+            if c.stride[0] != 1:
+                raise UnsupportedModel('dilated convolutions with a stride are not supported')
+            e['dilation'] = int(c.dilation[0])
+        return e
+
+    parts = _resnet_input_block(base.input_block)
+    conv, bn = parts[0][1]
     w, b = _fold(conv, bn)
     plan = {'kind': 'resnet',
             'input': {'w': w, 'b': b, 'stride': int(conv.stride[0]), 'pad': int(conv.padding[0])},
             'blocks': [], 'heads': _heads_plan(shell, base)}
-
-    def conv_entry(c, n):
-        if c.dilation[0] != 1 or c.groups != 1:
-            raise RuntimeError('dilated / grouped ResNet convolutions are not supported')
-        w_, b_ = _fold(c, n)
-        return {'w': w_, 'b': b_, 'kernel': int(c.kernel_size[0]), 'stride': int(c.stride[0]), 'pad': int(c.padding[0])}
+    if len(parts) == 2 and parts[1][0] == 'pool':
+        plan['pool'] = {'stride': int(_pair(parts[1][1].stride)[0])}
+    elif len(parts) == 2:
+        plan['input2'] = conv_entry(*parts[1][1])
 
     for stage in (base.block2, base.block3, base.block4, base.block5):
         for blk in stage:
@@ -121,21 +177,21 @@ def plan_from_shell(shell):
     """Extract a folded plan from a reference-style Shell (ShuffleNetV2K or Resnet base net)."""
     base = shell.base_net
     if shell.training:
-        raise RuntimeError('the Shell must be in eval() mode (BatchNorm is folded)')
+        raise UnsupportedModel('the Shell must be in eval() mode (BatchNorm is folded)')
     # network/nets.py:12-13,36-46: optional pre/post-processing hooks -- not lowered, so refuse them loudly
     if getattr(shell, 'process_input', None) is not None or getattr(shell, 'process_heads', None) is not None:
-        raise RuntimeError('Shell.process_input / process_heads are not supported by the compiled forward')
+        raise UnsupportedModel('Shell.process_input / process_heads are not supported by the compiled forward')
     for m in base.modules():
         # the kernels fuse max(x, 0); --shufflenetv2k-leaky-relu etc. would be folded wrongly
         if isinstance(m, (torch.nn.LeakyReLU, torch.nn.ELU, torch.nn.PReLU, torch.nn.SiLU, torch.nn.GELU,
                           torch.nn.Hardswish, torch.nn.InstanceNorm2d, torch.nn.GroupNorm)):
-            raise RuntimeError(f'unsupported module in the base network: {type(m).__name__} (only ReLU + BatchNorm)')
+            raise UnsupportedModel(f'unsupported module in the base network: {type(m).__name__} (only ReLU + BatchNorm)')
     if all(hasattr(base, a) for a in ('input_block', 'block2', 'block3', 'block4', 'block5')):
         return _plan_from_resnet(shell)
     if not all(hasattr(base, a) for a in ('input_block', 'stage2', 'stage3', 'stage4', 'conv5')):
-        raise RuntimeError(f'unsupported base network {type(base).__name__}: expected ShuffleNetV2K or Resnet')
+        raise UnsupportedModel(f'unsupported base network {type(base).__name__}: expected ShuffleNetV2K or Resnet')
     if len(base.input_block) != 1:
-        raise RuntimeError('input_conv2 variants are not supported')
+        raise UnsupportedModel('input_conv2 variants are not supported')
     conv, bn = base.input_block[0][0], base.input_block[0][1]
     w, b = _fold(conv, bn)
     plan = {'kind': 'shufflenetv2k',
@@ -147,7 +203,7 @@ def plan_from_shell(shell):
             b2 = blk.branch2
             dw = b2[3]
             if dw.dilation[0] != 1:
-                raise RuntimeError('dilated stages are not supported')
+                raise UnsupportedModel('dilated stages are not supported')
             entry = {'first': blk.branch1 is not None, 'stride': int(dw.stride[0]),
                      'kernel': int(dw.kernel_size[0]), 'pad': int(dw.padding[0])}
             entry['b2_pw1'] = _fold(b2[0], b2[1])
@@ -159,7 +215,7 @@ def plan_from_shell(shell):
             blocks.append(entry)
         plan['stages'].append(blocks)
     if not isinstance(base.conv5[0], torch.nn.Conv2d):
-        raise RuntimeError('conv5_as_stage is not supported')
+        raise UnsupportedModel('conv5_as_stage is not supported')
     plan['conv5'] = _fold(base.conv5[0], base.conv5[1])
     plan['heads'] = _heads_plan(shell, base)
     return plan
@@ -222,42 +278,70 @@ RESNET_CONFIGS = {      # torchvision.models.resnet: (block, layers); network/fa
 }
 
 
-def random_resnet_plan(base_name='resnet50', heads=((17, 1, 1, 1), (19, 1, 2, 2)), seed=0, confidence_bias=-4.0):
+def random_resnet_plan(base_name='resnet50', heads=((17, 1, 1, 1), (19, 1, 2, 2)), seed=0, confidence_bias=-4.0, *,
+                       pool0_stride=0, input_conv_stride=2, input_conv2_stride=0, block5_dilation=1, upsample=1):
     """Random-init folded plan of the reference's Resnet base network (basenetworks.py:71-150: torchvision ResNet,
     max-pool removed, stride 16; BasicBlock 3x3-3x3 / Bottleneck 1x1-3x3(stride)-1x1 with expansion 4, 1x1
     downsample on the first block of a stage) -- the same dict layout `_plan_from_resnet` extracts from a Shell.
     The last conv of a block and the downsample conv get half the He variance so that the residual sum keeps the
-    activation scale over 16 blocks."""
+    activation scale over 16 blocks.  The keyword options are the reference's --resnet-pool0-stride,
+    --resnet-input-conv-stride, --resnet-input-conv2-stride and --resnet-block5-dilation; upsample is the heads'
+    upsample_stride (--cocodet-upsample).  A head may carry its vector offsets as a fifth entry (CifDet:
+    (n_categories, 1, 2, 0, (True, False))); without it every vector has an offset."""
     kind, layers = RESNET_CONFIGS[base_name]
     rng = np.random.Generator(np.random.PCG64(seed))
 
-    def conv(cout, cin, k, stride, gain=2.0):
+    def conv(cout, cin, k, stride, gain=2.0, dilation=1):
         w = rng.standard_normal((cout, cin, k, k)).astype(np.float32) * np.float32(np.sqrt(gain / (cin * k * k)))
         b = (rng.standard_normal(cout) * 0.05).astype(np.float32)
-        return {'w': w, 'b': b, 'kernel': k, 'stride': stride, 'pad': (k - 1) // 2}
+        e = {'w': w, 'b': b, 'kernel': k, 'stride': stride, 'pad': (k - 1) // 2 * dilation}
+        if dilation != 1:
+            e['dilation'] = dilation
+        return e
 
-    stem = conv(64, 3, 7, 2)
-    plan = {'kind': 'resnet', 'input': {'w': stem['w'], 'b': stem['b'], 'stride': 2, 'pad': 3}, 'blocks': [], 'heads': []}
+    stem = conv(64, 3, 7, input_conv_stride)
+    plan = {'kind': 'resnet', 'input': {'w': stem['w'], 'b': stem['b'], 'stride': input_conv_stride, 'pad': 3},
+            'blocks': [], 'heads': []}
+    # output stride as basenetworks.py:79-128 tracks it: 32, times 2 / pool stride (16 without the pool), times
+    # 2 / input conv stride, times 2 with the second input conv, halved by block5 dilation
+    base_stride = 32 * 2 // pool0_stride if pool0_stride else 16
+    base_stride = base_stride * 2 // input_conv_stride
+    if pool0_stride:
+        plan['pool'] = {'stride': pool0_stride}
+    if input_conv2_stride:
+        plan['input2'] = conv(64, 64, 3, 2)         # Conv2d(channels, channels, 3, 2, 1), basenetworks.py:100-112
+        base_stride *= 2
+    if block5_dilation != 1:
+        base_stride //= 2
     expansion = 1 if kind == 'basic' else 4
     cin = 64
     for si, (planes, n) in enumerate(zip((64, 128, 256, 512), layers)):
+        dil = block5_dilation if si == 3 else 1
         for bi in range(n):
-            stride = 2 if (bi == 0 and si > 0) else 1
+            stride = 2 if (bi == 0 and si > 0 and dil == 1) else 1
             cout = planes * expansion
             if kind == 'basic':
-                convs = [conv(planes, cin, 3, stride), conv(planes, planes, 3, 1, gain=1.0)]
+                convs = [conv(planes, cin, 3, stride, dilation=dil), conv(planes, planes, 3, 1, gain=1.0, dilation=dil)]
             else:
-                convs = [conv(planes, cin, 1, 1), conv(planes, planes, 3, stride), conv(cout, planes, 1, 1, gain=1.0)]
+                convs = [conv(planes, cin, 1, 1), conv(planes, planes, 3, stride, dilation=dil),
+                         conv(cout, planes, 1, 1, gain=1.0)]
             down = conv(cout, cin, 1, stride, gain=1.0) if (stride != 1 or cin != cout) else None
             plan['blocks'].append({'convs': convs, 'downsample': down})
             cin = cout
-    for (nf, nconf, nvec, nsc) in heads:
+    for spec in heads:
+        nf, nconf, nvec, nsc = spec[:4]
+        offsets = tuple(spec[4]) if len(spec) > 4 else (True,) * nvec
         ncomp = 1 + nconf + 2 * nvec + nsc
-        w = (rng.standard_normal((nf * ncomp, cin)) * np.sqrt(1.0 / cin)).astype(np.float32)
-        b = (rng.standard_normal(nf * ncomp) * 0.1).astype(np.float32)
-        b.reshape(nf, ncomp)[:, 1:1 + nconf] += np.float32(confidence_bias)
-        plan['heads'].append({'w': w, 'b': b, 'n_fields': nf, 'n_comp': ncomp,
-                              'ops': head_ops(nconf, nvec, nsc, (True,) * nvec), 'stride': 16})
+        nc = nf * ncomp * upsample * upsample
+        w = (rng.standard_normal((nc, cin)) * np.sqrt(1.0 / cin)).astype(np.float32)
+        b = (rng.standard_normal(nc) * 0.1).astype(np.float32)
+        # conv channel (field * n_comp + comp) * up^2 + sub (PixelShuffle order, heads.py:333-343)
+        b.reshape(nf, ncomp, upsample * upsample)[:, 1:1 + nconf] += np.float32(confidence_bias)
+        hd = {'w': w, 'b': b, 'n_fields': nf, 'n_comp': ncomp,
+              'ops': head_ops(nconf, nvec, nsc, offsets), 'stride': base_stride // upsample}
+        if upsample != 1:
+            hd['upsample'] = upsample
+        plan['heads'].append(hd)
     return plan
 
 
@@ -439,7 +523,8 @@ def build_ops(plan, in_h, in_w, layout=None, fuse_dw=None):
     """Lower a plan to the op list of libpifpaf_b200 (pure Python; no GPU needed).
 
     Returns (tensors, ops): tensors[i] = (h, w, c_phys); ops are dicts with a 'kind' in
-    {'input_conv', 'conv1x1', 'dwconv', 'heads'} whose fields are the C ABI arguments."""
+    {'input_conv', 'conv1x1', 'dwconv', 'dw_conv1x1', 'conv', 'maxpool', 'heads'} whose fields are the C ABI
+    arguments."""
     if plan.get('kind') == 'resnet':
         return _build_ops_resnet(plan, in_h, in_w)
     if plan.get('kind') == 'heads_only':
@@ -638,12 +723,13 @@ def _build_ops_resnet(plan, in_h, in_w):
 
     def conv(tin, e, relu, tout, residual=-1):
         ops.append({'kind': 'conv', 'in': tin, 'in_off': 0, 'c_in': e['w'].shape[1], 'kernel': e['kernel'],
-                    'stride': e['stride'], 'pad': e['pad'], 'n_out': e['w'].shape[0], 'w': _f32(e['w']),
-                    'b': _f32(e['b']), 'relu': int(relu), 'out': tout, 'out_off': 0,
+                    'stride': e['stride'], 'pad': e['pad'], 'dilation': e.get('dilation', 1), 'n_out': e['w'].shape[0],
+                    'w': _f32(e['w']), 'b': _f32(e['b']), 'relu': int(relu), 'out': tout, 'out_off': 0,
                     'residual': residual, 'residual_off': 0})
 
     def out_hw(h, w, e):
-        return ((h + 2 * e['pad'] - e['kernel']) // e['stride'] + 1, (w + 2 * e['pad'] - e['kernel']) // e['stride'] + 1)
+        span = e.get('dilation', 1) * (e['kernel'] - 1) + 1
+        return ((h + 2 * e['pad'] - span) // e['stride'] + 1, (w + 2 * e['pad'] - span) // e['stride'] + 1)
 
     inp = plan['input']
     k = inp['w'].shape[-1]
@@ -653,6 +739,18 @@ def _build_ops_resnet(plan, in_h, in_w):
     cur = tensor(h, w, pad16(c0))
     ops.append({'kind': 'input_conv', 'in_h': in_h, 'in_w': in_w, 'kernel': k, 'stride': inp['stride'],
                 'pad': inp['pad'], 'c_out': c0, 'w': _f32(inp['w']), 'b': _f32(inp['b']), 'relu': 1, 'out': cur})
+    if plan.get('pool') is not None:
+        s = plan['pool']['stride']
+        h, w = (h - 1) // s + 1, (w - 1) // s + 1          # 3x3, padding 1
+        t_pool = tensor(h, w, pad16(c0))
+        ops.append({'kind': 'maxpool', 'in': cur, 'in_off': 0, 'channels': c0, 'stride': s, 'out': t_pool, 'out_off': 0})
+        cur = t_pool
+    if plan.get('input2') is not None:
+        e2 = plan['input2']
+        h, w = out_hw(h, w, e2)
+        t2 = tensor(h, w, pad16(e2['w'].shape[0]))
+        conv(cur, e2, True, t2)
+        cur, c0 = t2, e2['w'].shape[0]
     c_cur = c0
     block_outputs = []
     for e in plan['blocks']:
@@ -750,9 +848,13 @@ class CompiledNet:
                                                 _ptr(o['b']), o['relu'], o['out'], o['out_off'],
                                                 o['shuffle_src'], o['shuffle_off']))
             elif o['kind'] == 'conv':
-                _lib.check(L.pifpaf_net_conv(H, o['in'], o['in_off'], o['c_in'], o['kernel'], o['stride'], o['pad'],
-                                             o['n_out'], _ptr(o['w']), _ptr(o['b']), o['relu'], o['out'],
-                                             o['out_off'], o['residual'], o['residual_off']))
+                _lib.check(L.pifpaf_net_conv_dilated(H, o['in'], o['in_off'], o['c_in'], o['kernel'], o['stride'],
+                                                     o['pad'], o['n_out'], _ptr(o['w']), _ptr(o['b']), o['relu'],
+                                                     o['out'], o['out_off'], o['residual'], o['residual_off'],
+                                                     o['dilation']))
+            elif o['kind'] == 'maxpool':
+                _lib.check(L.pifpaf_net_maxpool(H, o['in'], o['in_off'], o['channels'], o['stride'], o['out'],
+                                                o['out_off']))
             elif o['kind'] == 'dwconv':
                 _lib.check(L.pifpaf_net_dwconv(H, o['in'], o['in_off'], o['channels'], o['kernel'], o['stride'],
                                                o['pad'], _ptr(o['w']), _ptr(o['b']), o['relu'], o['out'], o['out_off']))
@@ -839,7 +941,7 @@ class CompiledNet:
     def forward_timed(self, image_batch, *, gemm_impl=0):
         """Profiling pass: per-op (ms, kind, flops, bytes); kind 0 input conv, 1 wgmma GEMM, 2 depthwise,
         3 fused kernels (depthwise -> GEMM, or 1x1 GEMM -> stride-2 depthwise: there the GEMM op launches nothing and
-        reports 0 FLOPs and 0 bytes, and the depthwise op reports the fused launch with the FLOPs of both)."""
+        reports 0 FLOPs and 0 bytes, and the depthwise op reports the fused launch with the FLOPs of both), 4 max pool."""
         b, n = int(image_batch.shape[0]), self.num_ops
         ms = np.zeros((n,), dtype=np.float32)
         kind = np.zeros((n,), dtype=np.int32)

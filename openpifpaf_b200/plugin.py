@@ -11,8 +11,10 @@ Two levels of drop-in:
     tensors) -> ``List[Annotation]``; decoding happens on the GPU through libpifpaf_b200.
   * ``CifCafB200.batch(model, image_batch, device=...)``: the whole hot loop on the GPU -- the model is
     compiled once per input shape into wgmma kernels and the head tensors never visit the host.
-    ``register()`` makes ``Multi.batch`` (what ``Predictor`` calls, predictor.py:131) delegate to it when
-    it is the selected decoder.
+    ``CifDetB200.batch`` does the same for detection models (one CifDet head); a model the compiled forward does
+    not implement (network.UnsupportedModel, e.g. MobileNetV3) takes the reference's ``Decoder.batch`` instead.
+    ``register()`` makes ``Multi.batch`` (what ``Predictor`` calls, predictor.py:131) delegate to either when
+    it is the only decoder.
 """
 import collections
 import logging
@@ -23,9 +25,48 @@ import numpy as np
 import torch
 
 from . import decoder as b200_decoder
+from . import network as b200_network
 from . import predictor as b200_predictor
 
 LOG = logging.getLogger(__name__)
+
+
+class _CompileCache:
+    """The compiled models of the GPU batch path (CifCafB200.batch, CifDetB200.batch): an LRU of
+    `compile_cache_size` predictors keyed by (model, input shape); the class using it sets ``self._compiled`` to an
+    OrderedDict and implements ``_compile(shell, h, w, batch, device_index)``."""
+    #: compiled (model, input shape) entries kept alive; each owns every activation buffer of its max batch
+    compile_cache_size = 2
+
+    @staticmethod
+    def _weights_version(shell):
+        # torch bumps Tensor._version on every in-place write (optimizer step, load_state_dict, .copy_)
+        return sum(int(p._version) for p in shell.parameters()) + sum(int(b._version) for b in shell.buffers())
+
+    def _predictor_for(self, shell, batch, h, w, device):
+        """Compile `shell` for this input shape once; LRU of `compile_cache_size` entries.  An entry is reused only
+        for the same live module object (weak reference, so a recycled id() cannot alias), unchanged weights and a
+        batch that fits; evicted entries free their GPU buffers at once."""
+        key = (id(shell), h, w)
+        hit = self._compiled.get(key)
+        if hit is not None:
+            ref, version, pred = hit
+            if ref() is shell and version == self._weights_version(shell) and pred.net.max_batch >= batch:
+                self._compiled.move_to_end(key)
+                return pred
+            self._evict(key)
+        dev_index = torch.device(device).index if device is not None else None
+        if dev_index is None:
+            dev_index = torch.cuda.current_device()
+        pred = self._compile(shell, h, w, max(batch, 1), dev_index)
+        self._compiled[key] = (weakref.ref(shell), self._weights_version(shell), pred)
+        while len(self._compiled) > self.compile_cache_size:
+            self._evict(next(iter(self._compiled)))
+        return pred
+
+    def _evict(self, key):
+        _, _, pred = self._compiled.pop(key)
+        pred.close()
 
 
 def _build_class():
@@ -34,13 +75,11 @@ def _build_class():
     from openpifpaf.annotation import Annotation
     from openpifpaf.decoder import Decoder
 
-    class CifCafB200(Decoder):
+    class CifCafB200(_CompileCache, Decoder):
         """CifCaf decoding on an H100 (same CLI knobs as the reference's CifCaf)."""
         fast_batch = True
         #: read by TrackingPose.soft_nms (tracking_pose.py:160) when this class is its pose generator
         occupancy_visualizer = None
-        #: compiled (model, input shape) entries kept alive; each owns every activation buffer of its max batch
-        compile_cache_size = 2
 
         def __init__(self, cif_metas, caf_metas):
             super().__init__()
@@ -143,36 +182,9 @@ def _build_class():
             LOG.debug('b200 annotations = %d (%.1fms)', len(ann_t), (time.perf_counter() - start) * 1000.0)
             return self._annotations(ann_t.numpy(), ids.numpy())
 
-        @staticmethod
-        def _weights_version(shell):
-            # torch bumps Tensor._version on every in-place write (optimizer step, load_state_dict, .copy_)
-            return sum(int(p._version) for p in shell.parameters()) + sum(int(b._version) for b in shell.buffers())
-
-        def _predictor_for(self, shell, batch, h, w, device):
-            """Compile `shell` for this input shape once; LRU of `compile_cache_size` entries.  An entry is reused only
-            for the same live module object (weak reference, so a recycled id() cannot alias), unchanged weights and a
-            batch that fits; evicted entries free their GPU buffers at once."""
-            key = (id(shell), h, w)
-            hit = self._compiled.get(key)
-            if hit is not None:
-                ref, version, pred = hit
-                if ref() is shell and version == self._weights_version(shell) and pred.net.max_batch >= batch:
-                    self._compiled.move_to_end(key)
-                    return pred
-                self._evict(key)
-            dev_index = torch.device(device).index if device is not None else None
-            if dev_index is None:
-                dev_index = torch.cuda.current_device()
-            pred = b200_predictor.from_shell(shell, h, w, max(batch, 1), device=dev_index,
+        def _compile(self, shell, h, w, batch, device_index):
+            return b200_predictor.from_shell(shell, h, w, batch, device=device_index,
                                              cif_meta=self.cif_metas[0], caf_meta=self.caf_metas[0])
-            self._compiled[key] = (weakref.ref(shell), self._weights_version(shell), pred)
-            while len(self._compiled) > self.compile_cache_size:
-                self._evict(next(iter(self._compiled)))
-            return pred
-
-        def _evict(self, key):
-            _, _, pred = self._compiled.pop(key)
-            pred.close()
 
         def batch(self, model, image_batch, *, device=None, gt_anns_batch=None):
             """decoder/decoder.py:114-137 with everything on the GPU."""
@@ -219,10 +231,11 @@ def _build_class():
             cifcaf_fields[self.caf_meta.head_index] = caf
             return self.cifcaf(cifcaf_fields, initial_annotations=initial_annotations)
 
-    class CifDetB200(Decoder):
+    class CifDetB200(_CompileCache, Decoder):
         """decoder/cifdet.py:15-96 with the C++ CifDet call AND the torchvision NMS / score filter on the GPU
         (libpifpaf_b200 pifpaf_cifdet_*).  Class attributes are read from the reference's CifDet at call time, so
         decoder.factory.configure (decoder/factory.py:68,78) keeps configuring one source of truth."""
+        fast_batch = True
 
         def __init__(self, head_metas):
             super().__init__()
@@ -230,6 +243,13 @@ def _build_class():
             self.priority = -1.0 + 0.5                      # decoder/cifdet.py:29 is -1.0: outrank it, stay below poses
             self.priority += sum(m.n_fields for m in head_metas) / 1000.0
             self.native = b200_decoder.CifDet(head_metas[0].n_fields)
+            self._compiled = collections.OrderedDict()
+
+        @classmethod
+        def configure(cls, args):
+            """The flags CifCafB200.cli owns (--b200-no-fast-batch, --b200-compile-cache) apply here too."""
+            cls.fast_batch = getattr(args, 'b200_fast_batch', True)
+            cls.compile_cache_size = max(1, int(getattr(args, 'b200_compile_cache', cls.compile_cache_size)))
 
         @classmethod
         def factory(cls, head_metas):
@@ -244,17 +264,47 @@ def _build_class():
             b200_decoder.CifDet.set_max_detections_before_nms(
                 torch.classes.openpifpaf_decoder.CifDet.get_max_detections_before_nms())
 
-        def __call__(self, fields):
-            from openpifpaf.annotation import AnnotationDet
+        @staticmethod
+        def nms_params():
+            """the NMS and score filter of the reference's CifDet wrapper (decoder/cifdet.py:55-64), by value"""
             ref = openpifpaf.decoder.CifDet
+            return dict(iou_threshold=ref.iou_threshold, nms_by_category=ref.nms_by_category,
+                        suppression=ref.suppression, instance_threshold=ref.instance_threshold)
+
+        def __call__(self, fields):
             self.sync_statics()
             field = fields[self.metas[0].head_index]
             if not field.is_cuda:
                 field = field.cuda(self.native.device)
-            cats, scores, boxes = self.native.decode_batch(
-                field[:, :6].unsqueeze(0), self.metas[0].stride, nms=True, iou_threshold=ref.iou_threshold,
-                nms_by_category=ref.nms_by_category, suppression=ref.suppression,
-                instance_threshold=ref.instance_threshold)[0]
+            return self._annotations(*self.native.decode_batch(
+                field[:, :6].unsqueeze(0), self.metas[0].stride, nms=True, **self.nms_params())[0])
+
+        def _compile(self, shell, h, w, batch, device_index):
+            if len(shell.head_metas) != 1:
+                raise b200_network.UnsupportedModel('the GPU detection path compiles Shells with one CifDet head')
+            return b200_predictor.from_shell(shell, h, w, batch, device=device_index)
+
+        def batch(self, model, image_batch, *, device=None, gt_anns_batch=None):
+            """decoder/decoder.py:114-137 with the forward, the decode and the NMS on the GPU.  A model the compiled
+            forward does not implement takes the reference's Decoder.batch (stock forward, then __call__ per image)."""
+            if not self.fast_batch or not torch.cuda.is_available():
+                return super().batch(model, image_batch, device=device, gt_anns_batch=gt_anns_batch)
+            start = time.perf_counter()
+            shell = model.module if hasattr(model, 'module') else model     # DataParallel (predictor.py:33-37)
+            b, _, h, w = image_batch.shape
+            try:
+                pred = self._predictor_for(shell, int(b), int(h), int(w), device)
+            except b200_network.UnsupportedModel as e:
+                LOG.info('CifDetB200: %s; decoding through the reference batch path', e)
+                return super().batch(model, image_batch, device=device, gt_anns_batch=gt_anns_batch)
+            self.sync_statics()
+            pred.nms_params = self.nms_params()
+            results = pred.batch(image_batch if image_batch.dtype == torch.float32 else image_batch.float())
+            self.last_nn_time = self.last_decoder_time = time.perf_counter() - start
+            return [self._annotations(*r) for r in results]
+
+        def _annotations(self, cats, scores, boxes):
+            from openpifpaf.annotation import AnnotationDet
             boxes_np = boxes.numpy()
             boxes_np[:, 2:] -= boxes_np[:, :2]              # xyxy -> xywh (decoder/cifdet.py:86-87)
             out = []
@@ -316,7 +366,7 @@ def register():
 
         def batch(self, model, image_batch, *, device=None, gt_anns_batch=None):
             decs = [d for d in self.decoders if d is not None]
-            if len(decs) == 1 and isinstance(decs[0], cls) and cls.fast_batch:
+            if len(decs) == 1 and isinstance(decs[0], (cls, det_cls)) and type(decs[0]).fast_batch:
                 res = decs[0].batch(model, image_batch, device=device, gt_anns_batch=gt_anns_batch)
                 self.last_nn_time, self.last_decoder_time = decs[0].last_nn_time, 0.0
                 return res

@@ -32,14 +32,18 @@ class Predictor:
 
     def __init__(self, net, n_keypoints, skeleton, *, device=0, cif_head=0, caf_head=1,
                  overlap_decode=False, reserve_sms=None):
-        self.net = net
-        self.device = torch.device('cuda', device)
         sk = torch.as_tensor(skeleton, dtype=torch.int64).reshape(-1, 2) - 1     # decoder/cifcaf.py:121
         self.decoder = _decoder.CifCaf(n_keypoints, sk, device=device)
         # size the native handle once, from the net (never re-created while results are in flight)
         hd = net.heads[cif_head]
         self.decoder.reserve(net.max_batch, hd['h'], hd['w'], max(net.heads[cif_head]['stride'], net.heads[caf_head]['stride']))
         self.cif_head, self.caf_head = int(cif_head), int(caf_head)
+        self._setup(net, device, overlap_decode, reserve_sms)
+
+    def _setup(self, net, device, overlap_decode, reserve_sms):
+        """What every predictor has besides its decoder: the net, the streams, the overlap policy."""
+        self.net = net
+        self.device = torch.device('cuda', device)
         self.stream = torch.cuda.Stream(device=self.device)
         self.copy_stream = torch.cuda.Stream(device=self.device)
         self.dec_stream = torch.cuda.Stream(device=self.device)
@@ -88,6 +92,10 @@ class Predictor:
         return (heads[self.cif_head], self.net.heads[self.cif_head]['stride'],
                 heads[self.caf_head], self.net.heads[self.caf_head]['stride'])
 
+    def _decode_async(self, heads, batch, stream=None):
+        cif, cs, caf, fs = self._decode_inputs(heads, batch)
+        self.decoder.decode_batch_async(cif, cs, caf, fs, stream=stream)
+
     def batch_device(self, image_batch_dev):
         """Device-resident images -> enqueue forward + decode (no host sync).  The forward goes to the current
         stream; the decode to the current stream too, or, with overlap_decode, to the decode stream behind an event
@@ -95,8 +103,7 @@ class Predictor:
         cur = torch.cuda.current_stream(self.device)
         if not self.overlap_decode:
             heads = self._forward(image_batch_dev)
-            cif, cs, caf, fs = self._decode_inputs(heads, int(image_batch_dev.shape[0]))
-            self.decoder.decode_batch_async(cif, cs, caf, fs)
+            self._decode_async(heads, int(image_batch_dev.shape[0]))
             return
         slot = self._step & 1
         self._step += 1
@@ -106,8 +113,7 @@ class Predictor:
         ready = torch.cuda.Event()
         ready.record(cur)
         self.dec_stream.wait_event(ready)
-        cif, cs, caf, fs = self._decode_inputs(heads, int(image_batch_dev.shape[0]))
-        self.decoder.decode_batch_async(cif, cs, caf, fs, stream=self.dec_stream)
+        self._decode_async(heads, int(image_batch_dev.shape[0]), stream=self.dec_stream)
         done = torch.cuda.Event()
         done.record(self.dec_stream)
         self._dec_done[slot] = done
@@ -200,13 +206,53 @@ class Predictor:
             self.join()
 
 
+class DetPredictor(Predictor):
+    """Predictor of a detection Shell (one CifDet head, headmeta.py:117-125): `batch`, `batch_device` + `fetch`
+    and `fields_batch` as for poses; per image the result is (categories [N] int64 (1-based), scores [N], boxes [N, 4]
+    (x1, y1, x2, y2)) of `decoder.CifDet.decode_batch(nms=True)`, with the NMS and score filter of the reference's
+    CifDet wrapper (decoder/cifdet.py:55-64).  Those four parameters (`nms_params`) go by value into every decode.
+    Overlapped decode, `batches()` and `raw_images()` are not implemented for detection."""
+
+    def __init__(self, net, n_categories, *, device=0, head=0, iou_threshold=0.5, nms_by_category=True,
+                 suppression=0.1, instance_threshold=0.15, overlap_decode=False):
+        if overlap_decode:
+            raise RuntimeError('overlap_decode is not implemented for detection (it needs a double-buffered CifDet '
+                               'fetch)')
+        self.decoder = _decoder.CifDet(n_categories, device=device)
+        self.head = int(head)
+        self.nms_params = dict(iou_threshold=iou_threshold, nms_by_category=nms_by_category, suppression=suppression,
+                               instance_threshold=instance_threshold)
+        self._setup(net, device, False, None)
+
+    def _decode_async(self, heads, batch, stream=None):
+        self.decoder.decode_batch_async(heads[self.head][:batch], self.net.heads[self.head]['stride'], nms=True,
+                                        stream=stream, **self.nms_params)
+
+    def batches(self, host_batches):
+        raise RuntimeError('batches() is not implemented for detection (it needs a double-buffered CifDet fetch); '
+                           'call batch() per batch')
+
+    def raw_images(self, images, **kwargs):
+        raise RuntimeError('raw_images() is not implemented for detection (no inverse transform of boxes); '
+                           'preprocess on the host and call batch()')
+
+
+def is_cifdet_meta(meta):
+    """headmeta.CifDet by its component layout: one confidence, two vectors (offset, no offset), no scale."""
+    return ((int(meta.n_confidences), int(meta.n_vectors), int(meta.n_scales), tuple(meta.vector_offsets))
+            == (1, 2, 0, (True, False)))
+
+
 def from_shell(shell, in_h, in_w, max_batch, *, device=0, cif_meta=None, caf_meta=None, **kwargs):
-    """Compile a reference-style Shell (network/nets.py:7-48) with a (Cif, Caf) head pair into a Predictor.
+    """Compile a reference-style Shell (network/nets.py:7-48) with a (Cif, Caf) head pair into a Predictor, or a
+    Shell whose only head is a CifDet into a DetPredictor (kwargs: its NMS parameters).
     cif_meta / caf_meta: the head metas the decoder was built for (decoder/cifcaf.py:212-222); default: the
     first Cif-like meta followed by a Caf-like one."""
     plan = _network.plan_from_shell(shell)
     net = _network.CompiledNet(plan, in_h, in_w, max_batch, device=device)
     metas = list(shell.head_metas)
+    if len(metas) == 1 and is_cifdet_meta(metas[0]):
+        return DetPredictor(net, metas[0].n_fields, device=device, **kwargs)
     if cif_meta is None or caf_meta is None:
         cif_meta, caf_meta = metas[0], metas[1]
     skeleton = getattr(caf_meta, 'skeleton', None)
