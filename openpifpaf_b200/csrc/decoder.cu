@@ -23,6 +23,9 @@
 #include <climits>
 #include <cstdlib>
 #include <cstring>
+#include <map>
+#include <mutex>
+#include <utility>
 #include <vector>
 
 #include "common.cuh"
@@ -1398,6 +1401,20 @@ __global__ void k_blend_single(const float* __restrict__ L, int n, double x, dou
     if (threadIdx.x == 0) { out[0] = j.x; out[1] = j.y; out[2] = j.s; out[3] = j.v; }
 }
 
+// The dynamic shared-memory limit of a kernel is state of the kernel in the device's context, shared by every handle
+// of the process.  Each handle only ever raises it: a handle created later with a smaller plan (another skeleton, a
+// smaller detection capacity) must not lower it below what an older handle launches with.
+cudaError_t raise_smem_limit(const void* kernel, int device, size_t bytes) {
+    static std::mutex mu;
+    static std::map<std::pair<const void*, int>, size_t> limit;
+    std::lock_guard<std::mutex> lock(mu);
+    size_t& cur = limit[{kernel, device}];
+    if (bytes <= cur) return cudaSuccess;
+    const cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+    if (e == cudaSuccess) cur = bytes;
+    return e;
+}
+
 template <typename T>
 int dev_alloc(T** p, size_t n) {
     cudaError_t e = cudaMalloc(reinterpret_cast<void**>(p), sizeof(T) * (n ? n : 1));
@@ -1634,12 +1651,12 @@ int pifpaf_decoder_create(pifpaf_decoder_t** out, int32_t device, int32_t n_keyp
 
     dec->grow = plan_grow(K, C);
     if (const char* e = std::getenv("PIFPAF_GROW_DEFER")) dec->defer_radius = (float)std::atof(e);
-    TRY_D(cudaFuncSetAttribute(k_grow, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dec->grow.smem));
-    TRY_D(cudaFuncSetAttribute(k_force_complete, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dec->grow.smem));
+    TRY_D(raise_smem_limit((const void*)k_grow, device, dec->grow.smem));
+    TRY_D(raise_smem_limit((const void*)k_force_complete, device, dec->grow.smem));
     const size_t ns = (sizeof(double) + 2 * sizeof(int)) * A + 16;
-    TRY_D(cudaFuncSetAttribute(k_nms, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ns));
+    TRY_D(raise_smem_limit((const void*)k_nms, device, ns));
     const size_t ss = sizeof(int) * (((size_t)F + 1 + 3) / 4 * 4 + 256 + 256 + 8) + 2 * 32 * 256 + 16;
-    TRY_D(cudaFuncSetAttribute(k_seed_sort, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ss));
+    TRY_D(raise_smem_limit((const void*)k_seed_sort, device, ss));
     // the memsets / table uploads above ran on the legacy default stream; decodes are enqueued on caller streams
     // (possibly non-blocking ones) that do not order themselves behind it
     TRY_D(cudaDeviceSynchronize());
@@ -2210,9 +2227,8 @@ int pifpaf_cifdet_create(pifpaf_cifdet_t** out, int32_t device, int32_t n_catego
     ALLOC(det->d_in_field, F * 6 * hw);
     TRY_D(cudaStreamCreateWithFlags(&det->own_stream, cudaStreamNonBlocking));
     const size_t ss = sizeof(int) * (((size_t)F + 1 + 3) / 4 * 4 + 256 + 256 + 8) + 2 * 32 * 256 + 16;
-    TRY_D(cudaFuncSetAttribute(k_seed_sort, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max(ss, (size_t)48 * 1024)));
-    TRY_D(cudaFuncSetAttribute(k_det_nms, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                               (int)std::max(det_nms_smem(max_detections), (size_t)48 * 1024)));
+    TRY_D(raise_smem_limit((const void*)k_seed_sort, device, std::max(ss, (size_t)48 * 1024)));
+    TRY_D(raise_smem_limit((const void*)k_det_nms, device, std::max(det_nms_smem(max_detections), (size_t)48 * 1024)));
     TRY_D(cudaDeviceSynchronize());
 #undef ALLOC
 #undef TRY_D
