@@ -240,7 +240,13 @@ int pifpaf_image_fill_rgb(uint8_t* dst_dev, int64_t n_pixels, int32_t r, int32_t
  * modules (openpifpaf_b200/network.py) walks a Shell-like module, folds
  * BatchNorm (eval) into weights+bias and channel_shuffle/chunk into physical
  * channel placement, and emits these ops once; forward() replays them.
- * All weights are HOST f32 pointers (copied/converted at emit time).         */
+ * All weights are HOST f32 pointers (copied/converted at emit time).
+ *
+ * Activation code: the `relu` argument of pifpaf_net_input_conv, pifpaf_net_conv1x1, pifpaf_net_conv(_dilated)
+ * and pifpaf_net_dwconv selects the function applied after bias (and residual):
+ *   0 = none, 1 = ReLU max(x, 0), 2 = ReLU6 min(max(x, 0), 6) (torchvision MobileNetV2's ReLU6).
+ * Any other value is PIFPAF_E_ARG.  The shuffle output of pifpaf_net_conv1x1, pifpaf_net_conv1x1_scatter and
+ * pifpaf_net_dw_conv1x1_scatter take 0 and 1 only (PIFPAF_E_ARG for 2).                                      */
 typedef struct pifpaf_net pifpaf_net_t;
 
 int pifpaf_net_create(pifpaf_net_t** out, int32_t device, int32_t max_batch);
@@ -250,14 +256,15 @@ void pifpaf_net_destroy(pifpaf_net_t* net);
  * c_phys % 16 == 0: rows start on 32-byte boundaries).  *id receives its handle. */
 int pifpaf_net_tensor(pifpaf_net_t* net, int32_t h, int32_t w, int32_t c_phys, int32_t* id);
 
-/* Input block conv (basenetworks.py:275-280; torchvision resnet conv1): dense kxk conv on the
- * f32 NCHW image [B][3][in_h][in_w] -> bf16 NHWC, + bias (folded BN) (+ReLU). weight [c_out][3][k][k]. */
+/* Input block conv (basenetworks.py:275-280; torchvision resnet conv1, mobilenet_v2 features[0]): dense kxk conv on
+ * the f32 NCHW image [B][3][in_h][in_w] -> bf16 NHWC, + bias (folded BN), activation code `relu`.
+ * weight [c_out][3][k][k]. */
 int pifpaf_net_input_conv(pifpaf_net_t* net, int32_t in_h, int32_t in_w, int32_t kernel, int32_t stride,
                           int32_t pad, int32_t c_out, const float* weight, const float* bias,
                           int32_t relu, int32_t out_tensor);
 
 /* 1x1 conv == GEMM on tensor cores (wgmma, TMA-fed): reads columns [in_col_off, in_col_off+k_cols)
- * of in_tensor; weight [n_out][k_cols] in the same physical column order; + bias (+ReLU).
+ * of in_tensor; weight [n_out][k_cols] in the same physical column order; + bias, activation code `relu`.
  * shuffle_src_tensor < 0: plain output at columns [out_col_off, out_col_off+n_out) of out_tensor.
  * shuffle_src_tensor >= 0: fused cat + channel_shuffle(2) (basenetworks.py:233-242): output logical
  *   channel 2n <- shuffle_src[n], 2n+1 <- this conv[n], written contiguously (physical == logical order);
@@ -285,7 +292,8 @@ int pifpaf_net_conv1x1_scatter(pifpaf_net_t* net, int32_t in_tensor, int32_t in_
 /* Dense kxk conv (k <= 7, stride 1 or 2) as an implicit GEMM on tensor cores (torchvision ResNet blocks behind
  * basenetworks.py:71-150): reads channels [in_col_off, in_col_off+c_in) of in_tensor through a 4-D TMA map
  * (zero padding by out-of-bounds fill); weight [n_out][c_in][k][k] (torch layout); + bias (folded BN);
- * optional residual add (residual_tensor >= 0) BEFORE the optional ReLU (BasicBlock / Bottleneck tail). */
+ * optional residual add (residual_tensor >= 0) BEFORE the activation (BasicBlock / Bottleneck tail; the
+ * MobileNetV2 projection adds its block input with code 0). */
 int pifpaf_net_conv(pifpaf_net_t* net, int32_t in_tensor, int32_t in_col_off, int32_t c_in,
                     int32_t kernel, int32_t stride, int32_t pad, int32_t n_out, const float* weight,
                     const float* bias, int32_t relu, int32_t out_tensor, int32_t out_col_off,
@@ -306,7 +314,9 @@ int pifpaf_net_conv_dilated(pifpaf_net_t* net, int32_t in_tensor, int32_t in_col
 int pifpaf_net_maxpool(pifpaf_net_t* net, int32_t in_tensor, int32_t in_col_off, int32_t channels, int32_t stride,
                        int32_t out_tensor, int32_t out_col_off);
 
-/* Depthwise kxk conv (basenetworks.py:228-231), weight [channels][k][k], + bias (folded BN) (+ReLU). */
+/* Depthwise kxk conv (basenetworks.py:228-231; torchvision InvertedResidual), weight [channels][k][k], + bias
+ * (folded BN), activation code `relu`.  k = 5 and k = 3 with stride 1 or 2 run the TMA-fed kernel; other shapes, and
+ * gemm_impl = 1, the generic one. */
 int pifpaf_net_dwconv(pifpaf_net_t* net, int32_t in_tensor, int32_t in_col_off, int32_t channels,
                       int32_t kernel, int32_t stride, int32_t pad, const float* weight, const float* bias,
                       int32_t relu, int32_t out_tensor, int32_t out_col_off);

@@ -268,6 +268,17 @@ __device__ __forceinline__ float softplus_f(float x) {   // torch softplus beta=
 }
 __device__ __forceinline__ float sigmoid_f(float x) { return 1.0f / (1.0f + expf(-x)); }
 
+// activation code of the conv entry points (include/pifpaf_b200.h): 0 none, 1 ReLU, 2 ReLU6 (MobileNetV2,
+// torchvision's ReLU6 = hardtanh(x, 0, 6); exact in f32 and after rounding to bf16, 6 is a bf16 value)
+constexpr int ACT_NONE = 0, ACT_RELU = 1, ACT_RELU6 = 2;
+__device__ __forceinline__ float act_f(float x, int act) {
+    if (act) {
+        x = fmaxf(x, 0.f);
+        if (act == ACT_RELU6) x = fminf(x, 6.f);
+    }
+    return x;
+}
+
 // 32 bytes (one sector) as two 128-bit global stores: p must be 32-byte aligned
 __device__ __forceinline__ void st_global_256(void* p, uint32_t a, uint32_t b, uint32_t c, uint32_t d,
                                               uint32_t e, uint32_t f, uint32_t g, uint32_t h) {
@@ -375,6 +386,7 @@ __device__ __forceinline__ void epilogue_chunk(const GemmArgs& g, int m, int n0,
         for (int j = 0; j < CHUNK; j += 2) {
             float a0 = acc[j] + bv[j] + rv[j], a1 = acc[j + 1] + bv[j + 1] + rv[j + 1];
             if (g.relu) { a0 = fmaxf(a0, 0.f); a1 = fmaxf(a1, 0.f); }
+            if (g.relu == ACT_RELU6) { a0 = fminf(a0, 6.f); a1 = fminf(a1, 6.f); }
             w[j >> 1] = pack_bf16(a0, a1);
         }
         // 16 bf16 = 32 bytes, 32-byte aligned (ldo % 16 == 0, out_col_off % 16 == 0, n0 % 16 == 0)
@@ -842,10 +854,8 @@ __global__ void __launch_bounds__(256) k_dwconv5(DwArgs a) {
         for (int o = 0; o < DW_OX; o++) {
             const int ox = ox0 + o;
             if (ox >= a.Wout) continue;
-            if (a.relu) {
 #pragma unroll
-                for (int j = 0; j < 8; j++) acc[o][j] = fmaxf(acc[o][j], 0.f);
-            }
+            for (int j = 0; j < 8; j++) acc[o][j] = act_f(acc[o][j], a.relu);
             uint4 ov;
             ov.x = pack_bf16(acc[o][0], acc[o][1]); ov.y = pack_bf16(acc[o][2], acc[o][3]);
             ov.z = pack_bf16(acc[o][4], acc[o][5]); ov.w = pack_bf16(acc[o][6], acc[o][7]);
@@ -854,24 +864,25 @@ __global__ void __launch_bounds__(256) k_dwconv5(DwArgs a) {
     }
 }
 
-// Depthwise 5x5 with TMA-staged input tiles.  A persistent CTA walks (channel block, image, tile) work items; the
-// input window of an item ((TH-1)*S+5 x (TW-1)*S+5 pixels x 64 channels, 4-D tensor map, out-of-bounds zero fill
+// Depthwise KS x KS (5x5: ShuffleNetV2K; 3x3: MobileNetV2) with TMA-staged input tiles.  A persistent CTA walks
+// (channel block, image, tile) work items; the input window of an item ((TH-1)*S+KS x (TW-1)*S+KS pixels x 64
+// channels, 4-D tensor map, out-of-bounds zero fill
 // == the conv padding) is streamed by TMA into an NSTAGE-deep shared-memory ring.  There is no CTA-wide barrier in
 // the steady state: every warp counts itself out of a ring slot with one shared-memory atomic, and the warp that
 // finishes a slot LAST re-arms it with the TMA of the item NSTAGE rounds ahead, so fast warps (edge tiles with
 // out-of-range blocks) run ahead of slow ones by up to NSTAGE-1 items.
 // Compute mapping (register blocking in BOTH spatial directions): one warp = one 4 x BW block of output pixels,
-// one lane = one channel pair.  The lane keeps its 25x2 weights and a 4 x BW x 2 f32 accumulator in registers and
+// one lane = one channel pair.  The lane keeps its KS*KS x 2 weights and a 4 x BW x 2 f32 accumulator in registers and
 // reads every input pixel of the block's window exactly once (4 bytes per lane, 128 bytes per warp request: one
 // conflict-free wavefront).
-template <int S, int TH, int TW, int BW, int NSTAGE>
+template <int S, int TH, int TW, int BW, int NSTAGE, int KS = 5>
 struct DwTile {
-    static constexpr int IH = (TH - 1) * S + 5, IW = (TW - 1) * S + 5;
+    static constexpr int IH = (TH - 1) * S + KS, IW = (TW - 1) * S + KS;
     static constexpr int BYTES = IH * IW * 64 * 2;
     static constexpr int WARPS = (TH / 4) * (TW / BW);
     static constexpr int THREADS = WARPS * 32;
-    static constexpr int WIN_Y = 3 * S + 5;            // input window of a 4 x BW output block
-    static constexpr int WIN_X = (BW - 1) * S + 5;
+    static constexpr int WIN_Y = 3 * S + KS;           // input window of a 4 x BW output block
+    static constexpr int WIN_X = (BW - 1) * S + KS;
     static constexpr int SMEM = NSTAGE * BYTES + 128;
 };
 
@@ -912,17 +923,18 @@ __device__ __forceinline__ void dw_advance_cf(DwPos& p, const DwPos& d, int cblk
     p.b += d.b + carry;
 }
 
-// One warp's share of a depthwise 5x5 item: the 4 x BW output pixels at (oy0, ox0) of image b, lane = the channel
-// pair c0, c0 + 1; bias initialises the f32 sums, the 25 taps run in (ky, kx) order, a.relu, bf16 stores.
+// One warp's share of a depthwise KS x KS item (KS = 5 or 3): the 4 x BW output pixels at (oy0, ox0) of image b,
+// lane = the channel pair c0, c0 + 1; bias initialises the f32 sums, the KS * KS taps run in (ky, kx) order (the
+// order of k_dwconv, so the 3x3 results equal its bit for bit), activation a.relu, bf16 stores.
 // win: the item's input window in shared memory, IW pixels per row, 128 bytes (64 channels) per pixel; p0: the
 // window pixel at the block's first tap.  SWZ: the 16-byte units of pixel p sit at unit ^ (p & 7) (k_pw_dw's
 // intermediate window, which its wgmma epilogue writes without bank conflicts that way); the eight possible units
 // are resolved once per block, so the loads need no address arithmetic.
-template <int S, int BW, int IW, bool SWZ>
+template <int S, int BW, int IW, bool SWZ, int KS = 5>
 __device__ __forceinline__ void dw5_block(const DwArgs& a, const unsigned char* win, int p0, int lane,
-                                          const float (&wgt)[25][2], float bias0, float bias1, int b, int oy0,
+                                          const float (&wgt)[KS * KS][2], float bias0, float bias1, int b, int oy0,
                                           int ox0, int c0) {
-    constexpr int WIN_Y = 3 * S + 5, WIN_X = (BW - 1) * S + 5;
+    constexpr int WIN_Y = 3 * S + KS, WIN_X = (BW - 1) * S + KS;
     const unsigned char* tile = win + p0 * 128 + (SWZ ? (lane & 3) * 4 : lane * 4);
     const unsigned char* rows[SWZ ? 8 : 1];          // SWZ: the lane's word in a pixel p with p & 7 == c
 #pragma unroll
@@ -945,13 +957,13 @@ __device__ __forceinline__ void dw5_block(const DwArgs& a, const unsigned char* 
 #pragma unroll
         for (int i = 0; i < 4; i++) {
             const int ky = ry - i * S;                    // compile-time after unrolling
-            if (ky < 0 || ky >= 5) continue;
+            if (ky < 0 || ky >= KS) continue;
 #pragma unroll
-            for (int kx = 0; kx < 5; kx++) {
+            for (int kx = 0; kx < KS; kx++) {
 #pragma unroll
                 for (int j = 0; j < BW; j++) {
-                    acc[i][j][0] = fmaf(f[j * S + kx][0], wgt[ky * 5 + kx][0], acc[i][j][0]);
-                    acc[i][j][1] = fmaf(f[j * S + kx][1], wgt[ky * 5 + kx][1], acc[i][j][1]);
+                    acc[i][j][0] = fmaf(f[j * S + kx][0], wgt[ky * KS + kx][0], acc[i][j][0]);
+                    acc[i][j][1] = fmaf(f[j * S + kx][1], wgt[ky * KS + kx][1], acc[i][j][1]);
                 }
             }
         }
@@ -963,6 +975,19 @@ __device__ __forceinline__ void dw5_block(const DwArgs& a, const unsigned char* 
             for (int j = 0; j < BW; j++) {
                 acc[i][j][0] = fmaxf(acc[i][j][0], 0.f); acc[i][j][1] = fmaxf(acc[i][j][1], 0.f);
             }
+    }
+    // ReLU6 is compiled into the 3x3 instantiations only: any change to the epilogue moves the register allocation of
+    // the 5x5 ones (k_dwconv5_tma and k_pw_dw), so a 5x5 depthwise conv with ReLU6 -- no network has one -- runs
+    // k_dwconv5 (pifpaf_net_dwconv)
+    if constexpr (KS == 3) {
+        if (a.relu == ACT_RELU6) {
+#pragma unroll
+            for (int i = 0; i < 4; i++)
+#pragma unroll
+                for (int j = 0; j < BW; j++) {
+                    acc[i][j][0] = fminf(acc[i][j][0], 6.f); acc[i][j][1] = fminf(acc[i][j][1], 6.f);
+                }
+        }
     }
     const size_t out_row = (size_t)a.Wout * a.ld_out;           // elements per output image row
     __nv_bfloat16* orow = a.out + ((size_t)(b * a.Hout + oy0) * a.Wout + ox0) * a.ld_out + a.out_col_off + c0;
@@ -988,10 +1013,11 @@ __device__ __forceinline__ void dw5_block(const DwArgs& a, const unsigned char* 
     }
 }
 
-template <int S, int TH, int TW, int BW, int NSTAGE, bool CBF = false>
-__global__ void __launch_bounds__(DwTile<S, TH, TW, BW, NSTAGE>::THREADS, 2)
+template <int S, int TH, int TW, int BW, int NSTAGE, bool CBF = false, int KS = 5>
+__global__ void __launch_bounds__(DwTile<S, TH, TW, BW, NSTAGE, KS>::THREADS, 2)
 k_dwconv5_tma(const __grid_constant__ CUtensorMap tmap_in, DwArgs a) {
-    using T = DwTile<S, TH, TW, BW, NSTAGE>;
+    using T = DwTile<S, TH, TW, BW, NSTAGE, KS>;
+    constexpr int TAPS = KS * KS;
     extern __shared__ __align__(128) unsigned char dsm_raw[];
     // align inside the shared window with pointer arithmetic on the array itself (keeps the address space known to
     // the compiler: LDS instead of generic loads)
@@ -1004,13 +1030,13 @@ k_dwconv5_tma(const __grid_constant__ CUtensorMap tmap_in, DwArgs a) {
     const int per_c = a.B * tiles_y * tiles_x;
     const int total = per_c * cblks;
     const int C = a.C8 * 8;
-    // CBF: the channel block changes with (almost) every item, so the weights [25][C] + bias [C] are staged in
-    // shared memory once per CTA and re-read from there (26 LDS.64 per item)
+    // CBF: the channel block changes with (almost) every item, so the weights [TAPS][C] + bias [C] are staged in
+    // shared memory once per CTA and re-read from there (TAPS + 1 LDS.64 per item)
     const float* s_w = reinterpret_cast<const float*>(dsm + (size_t)NSTAGE * T::BYTES);
     if (CBF) {
         float* sw = reinterpret_cast<float*>(dsm + (size_t)NSTAGE * T::BYTES);
-        for (int i = tid; i < 25 * C; i += T::THREADS) sw[i] = a.weight[i];
-        for (int i = tid; i < C; i += T::THREADS) sw[25 * C + i] = a.bias[i];
+        for (int i = tid; i < TAPS * C; i += T::THREADS) sw[i] = a.weight[i];
+        for (int i = tid; i < C; i += T::THREADS) sw[TAPS * C + i] = a.bias[i];
     }
     auto decompose = [&](int w) { return CBF ? dw_decompose_cf(w, cblks, tiles_y, tiles_x) : dw_decompose(w, per_c, tiles_y, tiles_x); };
     auto advance = [&](DwPos& p, const DwPos& d) {
@@ -1044,7 +1070,7 @@ k_dwconv5_tma(const __grid_constant__ CUtensorMap tmap_in, DwArgs a) {
     DwPos pos = decompose(blockIdx.x);
     int buf = 0; uint32_t phase = 0;
     int w_cblk = -1;
-    float wgt[25][2];
+    float wgt[TAPS][2];
     float bias0 = 0.f, bias1 = 0.f;
     for (int w = blockIdx.x; w < total; w += gridDim.x) {
         const int c0 = pos.c * 64 + lane * 2;
@@ -1052,14 +1078,14 @@ k_dwconv5_tma(const __grid_constant__ CUtensorMap tmap_in, DwArgs a) {
             w_cblk = pos.c;
             const bool cok = c0 < C;
 #pragma unroll
-            for (int tp = 0; tp < 25; tp++) {
+            for (int tp = 0; tp < TAPS; tp++) {
                 const float2 wv = !cok ? make_float2(0.f, 0.f)
                                   : CBF ? *reinterpret_cast<const float2*>(s_w + (size_t)tp * C + c0)
                                         : __ldg(reinterpret_cast<const float2*>(a.weight + (size_t)tp * C + c0));
                 wgt[tp][0] = wv.x; wgt[tp][1] = wv.y;
             }
             const float2 bv = !cok ? make_float2(0.f, 0.f)
-                              : CBF ? *reinterpret_cast<const float2*>(s_w + 25 * (size_t)C + c0)
+                              : CBF ? *reinterpret_cast<const float2*>(s_w + TAPS * (size_t)C + c0)
                                     : __ldg(reinterpret_cast<const float2*>(a.bias + c0));
             bias0 = bv.x; bias1 = bv.y;
         }
@@ -1068,8 +1094,8 @@ k_dwconv5_tma(const __grid_constant__ CUtensorMap tmap_in, DwArgs a) {
         // warps counted out of the slot's previous item, so the per-slot count never mixes two items
         mbar_wait(&full[buf], phase);
         if (oy0 < a.Hout && ox0 < a.Wout && c0 < C)
-            dw5_block<S, BW, T::IW, false>(a, dsm + (size_t)buf * T::BYTES, (by * 4 * S) * T::IW + bx * BW * S, lane,
-                                           wgt, bias0, bias1, pos.b, oy0, ox0, c0);
+            dw5_block<S, BW, T::IW, false, KS>(a, dsm + (size_t)buf * T::BYTES, (by * 4 * S) * T::IW + bx * BW * S,
+                                               lane, wgt, bias0, bias1, pos.b, oy0, ox0, c0);
         // count this warp out of the slot; the last one out re-arms it.  Every shared-memory read of the slot has
         // been consumed by an fma above (results are in registers), the fence orders them before the count.
         __syncwarp();
@@ -1093,9 +1119,13 @@ k_dwconv5_tma(const __grid_constant__ CUtensorMap tmap_in, DwArgs a) {
 //              stride 2 -> 8x16 outputs, 4x4 blocks (8 warps, 85 KB window, 2-deep ring, 1 CTA per SM): the
 //              stride-2 launches are DRAM-bound on halo re-reads, the wide tile has the smaller halo (1.30x
 //              against 1.41x for 8x8)
+// 3x3: the same tiles and blocks; the smaller windows buy one more ring slot at the same bytes in flight per SM:
+//              stride 1 -> 23 KB window, 4-deep ring, 2 CTAs per SM; stride 2 -> 72 KB window, 3-deep ring, 1 CTA per SM
 constexpr int DW1_TH = 8, DW1_TW = 16, DW2_TH = 8, DW2_TW = 16;
 using DwS1 = DwTile<1, DW1_TH, DW1_TW, 4, 3>;
 using DwS2 = DwTile<2, DW2_TH, DW2_TW, 4, 2>;
+using DwS1K3 = DwTile<1, DW1_TH, DW1_TW, 4, 4, 3>;
+using DwS2K3 = DwTile<2, DW2_TH, DW2_TW, 4, 3, 3>;
 
 // 3x3 max pool, pad 1, stride a.stride (torchvision's MaxPool2d(3, 2, 1) in the ResNet input block,
 // basenetworks.py:85-93): one output pixel x 8 channels (one 16-byte vector) per thread.  Taps outside the image are
@@ -1169,10 +1199,8 @@ __global__ void __launch_bounds__(256) k_dwconv(DwArgs a) {
                 acc[6] = fmaf(f3.x, w1.z, acc[6]); acc[7] = fmaf(f3.y, w1.w, acc[7]);
             }
         }
-        if (a.relu) {
 #pragma unroll
-            for (int j = 0; j < 8; j++) acc[j] = fmaxf(acc[j], 0.f);
-        }
+        for (int j = 0; j < 8; j++) acc[j] = act_f(acc[j], a.relu);
         uint4 o;
         o.x = pack_bf16(acc[0], acc[1]); o.y = pack_bf16(acc[2], acc[3]);
         o.z = pack_bf16(acc[4], acc[5]); o.w = pack_bf16(acc[6], acc[7]);
@@ -1688,10 +1716,8 @@ __global__ void __launch_bounds__(256) k_input_conv(InConvArgs a) {
                 acc[4] = fmaf(v, w1.x, acc[4]); acc[5] = fmaf(v, w1.y, acc[5]);
                 acc[6] = fmaf(v, w1.z, acc[6]); acc[7] = fmaf(v, w1.w, acc[7]);
             }
-            if (a.relu) {
 #pragma unroll
-                for (int j = 0; j < 8; j++) acc[j] = fmaxf(acc[j], 0.f);
-            }
+            for (int j = 0; j < 8; j++) acc[j] = act_f(acc[j], a.relu);
             uint4 o;
             o.x = pack_bf16(acc[0], acc[1]); o.y = pack_bf16(acc[2], acc[3]);
             o.z = pack_bf16(acc[4], acc[5]); o.w = pack_bf16(acc[6], acc[7]);
@@ -2085,9 +2111,11 @@ int emit_gemm(pifpaf_net* net, Op& op, int in_tensor, int in_col_off, int k_cols
     return rc;
 }
 
-// plain 1x1 GEMM without residual: the TMA-store epilogue writes the window [out_col_off, + pad8(N)) of `to`
+// plain 1x1 GEMM without residual: the TMA-store epilogue writes the window [out_col_off, + pad8(N)) of `to`.
+// ReLU6 GEMMs keep the per-lane epilogue: a ReLU6 clamp in the TMA-store epilogue (a uniform branch per fragment
+// group) slowed the ShuffleNetV2K forward, which never uses it, by 0.15 ms of 24.7 (64 images at 641 px, H100)
 void plan_tma_store_plain(const pifpaf_net* net, Op& op, const Tensor& to) {
-    if (!net->gemm_tma_store) return;
+    if (!net->gemm_tma_store || op.g.relu == ACT_RELU6) return;
     op.g.tma_store = 1;
     op.store_views = {Op::StoreView{to.data + op.g.out_col_off, pad8(op.g.N), to.c}};
 }
@@ -2107,9 +2135,11 @@ int plan_pw_dw(pifpaf_net* net) {
         const GemmArgs& g = gop.g;
         const DwArgs& d = dop.dw;
         if (g.mode != MODE_PLAIN || g.conv_k != 0 || g.res != nullptr || g.num_k_blocks != 1 || g.a_col0 != 0 ||
-            g.out_col_off != 0)
+            g.out_col_off != 0 || g.relu == ACT_RELU6)
             continue;
-        if (d.kernel != 5 || d.stride != 2 || d.pad != 2 || d.in != g.out || d.in_col_off != 0) continue;
+        // k_pw_dw is built for the 5x5 stride-2 depthwise conv with ReLU at most (not MobileNetV2's 3x3 + ReLU6 pairs)
+        if (d.kernel != 5 || d.stride != 2 || d.pad != 2 || d.relu == ACT_RELU6 || d.in != g.out || d.in_col_off != 0)
+            continue;
         const Tensor& tin = net->tensors[gop.a_tensor];
         if (tin.c > PWDW_K) continue;
         int t_mid = -1;
@@ -2212,6 +2242,10 @@ int pifpaf_net_create(pifpaf_net_t** out, int32_t device, int32_t max_batch) {
                                          cudaFuncAttributeMaxDynamicSharedMemorySize, DwS2::SMEM));
     PIFPAF_CUDA_TRY(cudaFuncSetAttribute(k_dwconv5_tma<2, DW2_TH, DW2_TW, 4, 2, true>,
                                          cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024));
+    PIFPAF_CUDA_TRY(cudaFuncSetAttribute(k_dwconv5_tma<1, DW1_TH, DW1_TW, 4, 4, false, 3>,
+                                         cudaFuncAttributeMaxDynamicSharedMemorySize, DwS1K3::SMEM));
+    PIFPAF_CUDA_TRY(cudaFuncSetAttribute(k_dwconv5_tma<2, DW2_TH, DW2_TW, 4, 3, false, 3>,
+                                         cudaFuncAttributeMaxDynamicSharedMemorySize, DwS2K3::SMEM));
     // the stem stages its weights in shared memory: 7x7 with more than 72 channels is past the default 48 KB
     PIFPAF_CUDA_TRY(cudaFuncSetAttribute(k_input_conv<1, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, INCONV_SMEM_MAX));
     PIFPAF_CUDA_TRY(cudaFuncSetAttribute(k_input_conv<3, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, INCONV_SMEM_MAX));
@@ -2250,6 +2284,7 @@ int pifpaf_net_input_conv(pifpaf_net_t* net, int32_t in_h, int32_t in_w, int32_t
                           int32_t relu, int32_t out_tensor) {
     PIFPAF_CHECK_ARG(net != nullptr && weight != nullptr, "null argument");
     PIFPAF_CHECK_ARG(out_tensor >= 0 && out_tensor < (int)net->tensors.size(), "bad tensor id");
+    PIFPAF_CHECK_ARG(relu >= ACT_NONE && relu <= ACT_RELU6, "activation code must be 0 (none), 1 (ReLU) or 2 (ReLU6)");
     const Tensor& to = net->tensors[out_tensor];
     const int ho = (in_h + 2 * pad - kernel) / stride + 1, wo = (in_w + 2 * pad - kernel) / stride + 1;
     PIFPAF_CHECK_ARG(to.h == ho && to.w == wo && to.c >= pad8(c_out), "output tensor shape mismatch");
@@ -2291,6 +2326,8 @@ int pifpaf_net_conv1x1(pifpaf_net_t* net, int32_t in_tensor, int32_t in_col_off,
     const int nt = (int)net->tensors.size();
     PIFPAF_CHECK_ARG(in_tensor >= 0 && in_tensor < nt && out_tensor >= 0 && out_tensor < nt, "bad tensor id");
     PIFPAF_CHECK_ARG(k_cols >= 1 && n_out >= 1, "bad conv size");
+    PIFPAF_CHECK_ARG(relu == ACT_NONE || relu == ACT_RELU || (relu == ACT_RELU6 && shuffle_src_tensor < 0),
+                     "activation code must be 0 (none), 1 (ReLU) or 2 (ReLU6); the shuffle epilogue takes 0 or 1");
     PIFPAF_CUDA_TRY(cudaSetDevice(net->device));
     const Tensor& tin = net->tensors[in_tensor];
     const Tensor& to = net->tensors[out_tensor];
@@ -2340,6 +2377,7 @@ int pifpaf_net_conv1x1_scatter(pifpaf_net_t* net, int32_t in_tensor, int32_t in_
     const int nt = (int)net->tensors.size();
     PIFPAF_CHECK_ARG(in_tensor >= 0 && in_tensor < nt, "bad tensor id");
     PIFPAF_CHECK_ARG(k_cols >= 1 && n_out >= 16 && n_out % 16 == 0 && n_pieces >= 1, "bad conv size");
+    PIFPAF_CHECK_ARG(relu == ACT_NONE || relu == ACT_RELU, "the scatter epilogue takes activation codes 0 (none) and 1 (ReLU)");
     PIFPAF_CUDA_TRY(cudaSetDevice(net->device));
     const Tensor& tin = net->tensors[in_tensor];
     Op op; op.kind = OP_GEMM;
@@ -2405,6 +2443,7 @@ int pifpaf_net_conv_dilated(pifpaf_net_t* net, int32_t in_tensor, int32_t in_col
     PIFPAF_CHECK_ARG(in_tensor >= 0 && in_tensor < nt && out_tensor >= 0 && out_tensor < nt, "bad tensor id");
     PIFPAF_CHECK_ARG(kernel >= 1 && kernel <= 7 && stride >= 1 && stride <= 2 && pad >= 0, "unsupported conv geometry");
     PIFPAF_CHECK_ARG(dilation >= 1 && dilation <= 64, "conv dilation must be 1 to 64");
+    PIFPAF_CHECK_ARG(relu >= ACT_NONE && relu <= ACT_RELU6, "activation code must be 0 (none), 1 (ReLU) or 2 (ReLU6)");
     // the stride-2 tensor map steps over every other input pixel; dilated taps would need their own traversal
     PIFPAF_CHECK_ARG(dilation == 1 || stride == 1, "a dilated conv (dilation > 1) must have stride 1");
     PIFPAF_CHECK_ARG(c_in >= 1 && n_out >= 1, "bad conv size");
@@ -2495,6 +2534,7 @@ int pifpaf_net_dwconv(pifpaf_net_t* net, int32_t in_tensor, int32_t in_col_off, 
     PIFPAF_CHECK_ARG(net != nullptr && weight != nullptr, "null argument");
     const int nt = (int)net->tensors.size();
     PIFPAF_CHECK_ARG(in_tensor >= 0 && in_tensor < nt && out_tensor >= 0 && out_tensor < nt, "bad tensor id");
+    PIFPAF_CHECK_ARG(relu >= ACT_NONE && relu <= ACT_RELU6, "activation code must be 0 (none), 1 (ReLU) or 2 (ReLU6)");
     const Tensor& tin = net->tensors[in_tensor];
     const Tensor& to = net->tensors[out_tensor];
     const int ho = (tin.h + 2 * pad - kernel) / stride + 1, wo = (tin.w + 2 * pad - kernel) / stride + 1;
@@ -2520,9 +2560,9 @@ int pifpaf_net_dwconv(pifpaf_net_t* net, int32_t in_tensor, int32_t in_col_off, 
     a.kernel = kernel; a.stride = stride; a.pad = pad; a.relu = relu;
     op.flops_per_image = 2.0 * ho * wo * channels * (double)kernel * kernel;
     op.bytes_per_image = ((double)tin.h * tin.w + (double)ho * wo) * channels * 2.0;
-    if (kernel == 5 && (stride == 1 || stride == 2)) {
-        const uint32_t bw = stride == 1 ? DwS1::IW : DwS2::IW;
-        const uint32_t bh = stride == 1 ? DwS1::IH : DwS2::IH;
+    if ((kernel == 3 || (kernel == 5 && relu != ACT_RELU6)) && (stride == 1 || stride == 2)) {
+        const uint32_t bw = kernel == 3 ? (stride == 1 ? DwS1K3::IW : DwS2K3::IW) : (stride == 1 ? DwS1::IW : DwS2::IW);
+        const uint32_t bh = kernel == 3 ? (stride == 1 ? DwS1K3::IH : DwS2K3::IH) : (stride == 1 ? DwS1::IH : DwS2::IH);
         rc = make_tmap_dw(&op.tmap_dw, tin.data + in_col_off, (uint64_t)C, (uint64_t)tin.w, (uint64_t)tin.h,
                           (uint64_t)net->max_batch, (uint64_t)tin.c, bw, bh);
         if (rc != PIFPAF_OK) return rc;
@@ -2572,6 +2612,8 @@ int pifpaf_net_dw_conv1x1_scatter(pifpaf_net_t* net, int32_t in_tensor, int32_t 
     const int nt = (int)net->tensors.size();
     PIFPAF_CHECK_ARG(in_tensor >= 0 && in_tensor < nt, "bad tensor id");
     PIFPAF_CHECK_ARG(kernel == 5 && stride == 1 && pad == 2, "the fused depthwise -> 1x1 op covers 5x5, stride 1, pad 2");
+    PIFPAF_CHECK_ARG(dw_relu >= ACT_NONE && dw_relu <= ACT_RELU && relu >= ACT_NONE && relu <= ACT_RELU,
+                     "the fused depthwise -> 1x1 op takes activation codes 0 (none) and 1 (ReLU)");
     PIFPAF_CHECK_ARG(n_out >= 16 && n_out % 16 == 0 && n_out <= 512 && n_pieces >= 1, "n_out: multiple of 16, at most 512");
     const Tensor& tin = net->tensors[in_tensor];
     const int C = pad8(channels);
@@ -2800,6 +2842,19 @@ static int net_forward_impl(pifpaf_net_t* net, const float* images_dev, int32_t 
                 const int grid = (int)std::min<long long>(total, (long long)n_sm);     // 1 CTA per SM by shared memory
                 PIFPAF_CUDA_TRY(launch_k(pdl, k_pw_dw<2, PWDW_TH, PWDW_TW, PWDW_BW>, dim3(grid), dim3(PwDwS2::THREADS),
                                          op.pw_smem, st, op.tmap_pw, p));
+            } else if (op.dw_tma && gemm_impl == 0 && a.kernel == 3) {
+                const int cblks = (a.C8 + 7) / 8;
+                const int th = a.stride == 1 ? DW1_TH : DW2_TH, tw = a.stride == 1 ? DW1_TW : DW2_TW;
+                const long long total = (long long)batch * ((a.Hout + th - 1) / th) * ((a.Wout + tw - 1) / tw) * cblks;
+                // persistent grid == resident CTAs (stride 1: 2 per SM, stride 2: 1 per SM by shared memory)
+                if (a.stride == 1)
+                    PIFPAF_CUDA_TRY(launch_k(pdl, k_dwconv5_tma<1, DW1_TH, DW1_TW, 4, 4, false, 3>,
+                                             dim3((int)std::min<long long>(total, (long long)n_sm * 2)),
+                                             dim3(DwS1K3::THREADS), (size_t)DwS1K3::SMEM, st, op.tmap_dw, a));
+                else
+                    PIFPAF_CUDA_TRY(launch_k(pdl, k_dwconv5_tma<2, DW2_TH, DW2_TW, 4, 3, false, 3>,
+                                             dim3((int)std::min<long long>(total, (long long)n_sm)),
+                                             dim3(DwS2K3::THREADS), (size_t)DwS2K3::SMEM, st, op.tmap_dw, a));
             } else if (op.dw_tma && gemm_impl == 0) {
                 const int cblks = (a.C8 + 7) / 8;
                 // persistent grid == resident CTAs (stride 1: 2 per SM, stride 2: 1 per SM by shared memory)

@@ -3,6 +3,7 @@
 Reference (paths relative to the reference's src/openpifpaf/):
   Shell.forward                       network/nets.py:35-48
   ShuffleNetV2K / InvertedResidualK   network/basenetworks.py:186-355
+  MobileNetV2 (torchvision features)  network/basenetworks.py:407-417
   CompositeField4 (eval)              network/heads.py:330-378
 
 `plan_from_shell(shell)` walks a reference-style ``Shell`` (duck-typed: the
@@ -32,6 +33,8 @@ import torch
 from . import _lib
 
 OP_RAW, OP_SIGMOID, OP_ADD_X, OP_ADD_Y, OP_SOFTPLUS = 0, 1, 2, 3, 4
+# activation codes of the conv ops (the `relu` field; include/pifpaf_b200.h)
+ACT_NONE, ACT_RELU, ACT_RELU6 = 0, 1, 2
 
 SHUFFLENETV2K_CONFIGS = {     # network/factory.py:68-79
     'shufflenetv2k16': ([4, 8, 4], [24, 348, 696, 1392, 1392]),
@@ -173,8 +176,65 @@ def _plan_from_resnet(shell):
     return plan
 
 
+def _conv_bn_relu6(m, what):
+    """torchvision's Conv2dNormActivation (ConvBNReLU in older releases) with ReLU6 -> (conv, bn)"""
+    parts = list(m) if isinstance(m, torch.nn.Sequential) else []
+    if len(parts) != 3 or not isinstance(parts[0], torch.nn.Conv2d) or not isinstance(parts[1], torch.nn.BatchNorm2d):
+        raise UnsupportedModel(f'MobileNetV2 {what}: expected Conv2d + BatchNorm2d + ReLU6, got {type(m).__name__}')
+    if not isinstance(parts[2], torch.nn.ReLU6):
+        raise UnsupportedModel(f'MobileNetV2 {what}: unsupported activation {type(parts[2]).__name__} (only ReLU6)')
+    return parts[0], parts[1]
+
+
+def _mobilenet_conv(conv, bn, what, kernel, stride=None, depthwise=False):
+    """one conv of the MobileNetV2 backbone, checked against the shapes torchvision builds, folded"""
+    k, s, p, d = _pair(conv.kernel_size), _pair(conv.stride), _pair(conv.padding), _pair(conv.dilation)
+    groups_ok = conv.groups == conv.in_channels == conv.out_channels if depthwise else conv.groups == 1
+    if k != (kernel, kernel) or s[0] != s[1] or s[0] not in ((1, 2) if stride is None else (stride,)) or \
+            p != ((kernel - 1) // 2,) * 2 or d != (1, 1) or not groups_ok:
+        raise UnsupportedModel(f'MobileNetV2 {what}: unsupported conv {conv}')
+    # torchvision rounds every width to a multiple of 8 (_make_divisible); the channel padding of the lowering
+    # (16-channel rows, 8-channel depthwise vectors) is laid out for that
+    if conv.out_channels % 8 or (conv.in_channels % 8 and conv.in_channels != 3):
+        raise UnsupportedModel(f'MobileNetV2 {what}: channel counts must be multiples of 8, got {conv}')
+    w, b = _fold(conv, bn)
+    return {'w': w, 'b': b, 'kernel': kernel, 'stride': int(s[0]), 'pad': (kernel - 1) // 2}
+
+
+def _plan_from_mobilenetv2(shell):
+    """basenetworks.py:407-417: base_net.backbone = torchvision mobilenet_v2().features -- the 3x3 stride-2 stem,
+    17 InvertedResidual blocks (1x1 expand + ReLU6 unless the expansion is 1, 3x3 depthwise + ReLU6, 1x1 linear
+    projection, plus the block input when stride 1 and in == out) and the final 1x1 conv + ReLU6; stride 32."""
+    base = shell.base_net
+    mods = list(base.backbone)
+    if len(mods) < 3:
+        raise UnsupportedModel('MobileNetV2 backbone: expected a stem, InvertedResidual blocks and a last conv')
+    conv, bn = _conv_bn_relu6(mods[0], 'stem')
+    stem = _mobilenet_conv(conv, bn, 'stem', 3, 2)
+    if conv.in_channels != 3:
+        raise UnsupportedModel('MobileNetV2 stem: expected 3 input channels')
+    blocks = []
+    for i, m in enumerate(mods[1:-1], start=1):
+        layers = list(m.conv) if isinstance(getattr(m, 'conv', None), torch.nn.Sequential) else []
+        if not hasattr(m, 'use_res_connect') or len(layers) not in (3, 4) or \
+                not isinstance(layers[-2], torch.nn.Conv2d) or not isinstance(layers[-1], torch.nn.BatchNorm2d):
+            raise UnsupportedModel(f'MobileNetV2 backbone[{i}]: expected an InvertedResidual, got {type(m).__name__}')
+        what = f'backbone[{i}]'
+        e = {'expand': _mobilenet_conv(*_conv_bn_relu6(layers[0], what), what, 1) if len(layers) == 4 else None}
+        e['dw'] = _mobilenet_conv(*_conv_bn_relu6(layers[-3], what), what, 3, depthwise=True)
+        e['project'] = _mobilenet_conv(layers[-2], layers[-1], what, 1, 1)
+        c_in = e['expand']['w'].shape[1] if e['expand'] is not None else e['dw']['w'].shape[0]
+        e['residual'] = bool(m.use_res_connect)
+        if e['residual'] != (e['dw']['stride'] == 1 and c_in == e['project']['w'].shape[0]):
+            raise UnsupportedModel(f'MobileNetV2 {what}: residual connection does not match stride and widths')
+        blocks.append(e)
+    conv, bn = _conv_bn_relu6(mods[-1], 'last conv')
+    last = _mobilenet_conv(conv, bn, 'last conv', 1, 1)
+    return {'kind': 'mobilenetv2', 'input': stem, 'blocks': blocks, 'last': last, 'heads': _heads_plan(shell, base)}
+
+
 def plan_from_shell(shell):
-    """Extract a folded plan from a reference-style Shell (ShuffleNetV2K or Resnet base net)."""
+    """Extract a folded plan from a reference-style Shell (ShuffleNetV2K, Resnet or MobileNetV2 base net)."""
     base = shell.base_net
     if shell.training:
         raise UnsupportedModel('the Shell must be in eval() mode (BatchNorm is folded)')
@@ -188,8 +248,11 @@ def plan_from_shell(shell):
             raise UnsupportedModel(f'unsupported module in the base network: {type(m).__name__} (only ReLU + BatchNorm)')
     if all(hasattr(base, a) for a in ('input_block', 'block2', 'block3', 'block4', 'block5')):
         return _plan_from_resnet(shell)
+    if isinstance(getattr(base, 'backbone', None), torch.nn.Sequential):
+        return _plan_from_mobilenetv2(shell)
     if not all(hasattr(base, a) for a in ('input_block', 'stage2', 'stage3', 'stage4', 'conv5')):
-        raise UnsupportedModel(f'unsupported base network {type(base).__name__}: expected ShuffleNetV2K or Resnet')
+        raise UnsupportedModel(f'unsupported base network {type(base).__name__}: expected ShuffleNetV2K, Resnet or '
+                               'MobileNetV2')
     if len(base.input_block) != 1:
         raise UnsupportedModel('input_conv2 variants are not supported')
     conv, bn = base.input_block[0][0], base.input_block[0][1]
@@ -527,6 +590,8 @@ def build_ops(plan, in_h, in_w, layout=None, fuse_dw=None):
     arguments."""
     if plan.get('kind') == 'resnet':
         return _build_ops_resnet(plan, in_h, in_w)
+    if plan.get('kind') == 'mobilenetv2':
+        return _build_ops_mobilenetv2(plan, in_h, in_w)
     if plan.get('kind') == 'heads_only':
         # in_h x in_w is the FEATURE map here; the feature tensor is filled through CompiledNet.forward_features
         c_in = int(plan['c_in'])
@@ -773,6 +838,57 @@ def _build_ops_resnet(plan, in_h, in_w):
         block_outputs.append((cur, _Layout(c_cur, split=False)))
     ops.append(_heads_op(plan['heads'], cur, c_cur))
     return tensors, ops, {'block_outputs': block_outputs, 'feature': (cur, _Layout(c_cur, split=False))}
+
+
+def _build_ops_mobilenetv2(plan, in_h, in_w):
+    """torchvision InvertedResidual (eval): the expand 1x1 and the linear projection are pointwise conv ops (the
+    projection adds the block input in its epilogue), the 3x3 depthwise conv a dwconv op; every activation is ReLU6.
+    Tensors are padded to 16 channels (24 -> 32)."""
+    tensors, ops = [], []
+
+    def tensor(h, w, c):
+        tensors.append((h, w, c))
+        return len(tensors) - 1
+
+    def conv(tin, e, act, tout, residual=-1):
+        ops.append({'kind': 'conv', 'in': tin, 'in_off': 0, 'c_in': e['w'].shape[1], 'kernel': e['kernel'],
+                    'stride': e['stride'], 'pad': e['pad'], 'dilation': 1, 'n_out': e['w'].shape[0],
+                    'w': _f32(e['w']), 'b': _f32(e['b']), 'relu': act, 'out': tout, 'out_off': 0,
+                    'residual': residual, 'residual_off': 0})
+
+    inp = plan['input']
+    k, s, p = inp['kernel'], inp['stride'], inp['pad']
+    h, w = (in_h + 2 * p - k) // s + 1, (in_w + 2 * p - k) // s + 1
+    c = inp['w'].shape[0]
+    cur = tensor(h, w, pad16(c))
+    ops.append({'kind': 'input_conv', 'in_h': in_h, 'in_w': in_w, 'kernel': k, 'stride': s, 'pad': p, 'c_out': c,
+                'w': _f32(inp['w']), 'b': _f32(inp['b']), 'relu': ACT_RELU6, 'out': cur})
+    block_outputs = []
+    for e in plan['blocks']:
+        x = cur
+        if e['expand'] is not None:
+            c = e['expand']['w'].shape[0]
+            t_e = tensor(h, w, pad16(c))
+            conv(cur, e['expand'], ACT_RELU6, t_e)
+            cur = t_e
+        dw = e['dw']
+        st = dw['stride']
+        ho, wo = (h + 2 * dw['pad'] - 3) // st + 1, (w + 2 * dw['pad'] - 3) // st + 1
+        t_d = tensor(ho, wo, pad16(c))
+        ops.append({'kind': 'dwconv', 'in': cur, 'in_off': 0, 'channels': c, 'kernel': 3, 'stride': st,
+                    'pad': dw['pad'], 'w': _f32(dw['w'].reshape(c, 9)), 'b': _f32(dw['b']), 'relu': ACT_RELU6,
+                    'out': t_d, 'out_off': 0})
+        h, w = ho, wo
+        c = e['project']['w'].shape[0]
+        t_p = tensor(h, w, pad16(c))
+        conv(t_d, e['project'], ACT_NONE, t_p, residual=x if e['residual'] else -1)
+        cur = t_p
+        block_outputs.append((cur, _Layout(c, split=False)))
+    c = plan['last']['w'].shape[0]
+    t_l = tensor(h, w, pad16(c))
+    conv(cur, plan['last'], ACT_RELU6, t_l)
+    ops.append(_heads_op(plan['heads'], t_l, c))
+    return tensors, ops, {'block_outputs': block_outputs, 'feature': (t_l, _Layout(c, split=False))}
 
 
 class CompiledNet:
