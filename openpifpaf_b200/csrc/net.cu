@@ -21,6 +21,7 @@
 #include <cuda_bf16.h>
 
 #include <cmath>
+#include <cstdio>
 #include <cstdlib>
 #include <cstring>
 #include <utility>
@@ -1747,7 +1748,10 @@ typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_
                                     const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
                                     CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 
-PFN_encodeTiled get_encode_fn() {
+// bf16 tensor map of `rank` dimensions (innermost first; row pitches in elements); a failure names the map and its shape
+int encode_tmap(CUtensorMap* map, const char* what, const void* base, int rank, const cuuint64_t* dims,
+                const cuuint64_t* ld, const cuuint32_t* box, const cuuint32_t* estr, CUtensorMapSwizzle swz,
+                CUtensorMapL2promotion l2) {
     static PFN_encodeTiled fn = nullptr;
     if (!fn) {
         void* p = nullptr;
@@ -1756,88 +1760,57 @@ PFN_encodeTiled get_encode_fn() {
             qres == cudaDriverEntryPointSuccess)
             fn = reinterpret_cast<PFN_encodeTiled>(p);
     }
-    return fn;
+    if (!fn) { pifpaf::set_error("cuTensorMapEncodeTiled entry point not available"); return PIFPAF_E_CUDA; }
+    cuuint64_t strides[3];
+    for (int i = 0; i + 1 < rank; i++) strides[i] = ld[i] * 2;
+    const CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, rank, const_cast<void*>(base), dims, strides, box, estr,
+                          CU_TENSOR_MAP_INTERLEAVE_NONE, swz, l2, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) {
+        char shape[256] = "";      // " dim/box" per dimension, then " ld" per pitch: at most 4 x 32 + 3 x 22 bytes
+        for (int i = 0; i < rank; i++)
+            snprintf(shape + strlen(shape), sizeof(shape) - strlen(shape), " %llu/%u", (unsigned long long)dims[i], box[i]);
+        for (int i = 0; i + 1 < rank; i++)
+            snprintf(shape + strlen(shape), sizeof(shape) - strlen(shape), " ld=%llu", (unsigned long long)ld[i]);
+        pifpaf::set_error("cuTensorMapEncodeTiled (%s) failed (%d): dim/box%s base=%p", what, (int)r, shape, base);
+        return PIFPAF_E_CUDA;
+    }
+    return PIFPAF_OK;
 }
 
 // 2-D bf16 row-major view [rows][cols] with row pitch ld (elements); box = [box_rows][64 cols], 128B swizzle
 int make_tmap(CUtensorMap* map, const void* base, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_rows) {
-    PFN_encodeTiled fn = get_encode_fn();
-    if (!fn) { pifpaf::set_error("cuTensorMapEncodeTiled entry point not available"); return PIFPAF_E_CUDA; }
     const cuuint64_t dims[2] = {cols, rows};
-    const cuuint64_t strides[1] = {ld * 2};
-    const cuuint32_t box[2] = {BK, box_rows};
-    const cuuint32_t estr[2] = {1, 1};
-    CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), dims, strides, box, estr,
-                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) {
-        pifpaf::set_error("cuTensorMapEncodeTiled failed (%d): rows=%llu cols=%llu ld=%llu box_rows=%u base=%p",
-                          (int)r, (unsigned long long)rows, (unsigned long long)cols, (unsigned long long)ld,
-                          box_rows, base);
-        return PIFPAF_E_CUDA;
-    }
-    return PIFPAF_OK;
+    const cuuint32_t box[2] = {BK, box_rows}, estr[2] = {1, 1};
+    return encode_tmap(map, "gemm", base, 2, dims, &ld, box, estr, CU_TENSOR_MAP_SWIZZLE_128B,
+                       CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
 }
 
 // 2-D bf16 row-major view, un-swizzled box [box_rows][box_cols] (dense rows in shared memory)
 int make_tmap_plain(CUtensorMap* map, const void* base, uint64_t rows, uint64_t cols, uint64_t ld,
                     uint32_t box_cols, uint32_t box_rows) {
-    PFN_encodeTiled fn = get_encode_fn();
-    if (!fn) { pifpaf::set_error("cuTensorMapEncodeTiled entry point not available"); return PIFPAF_E_CUDA; }
     const cuuint64_t dims[2] = {cols, rows};
-    const cuuint64_t strides[1] = {ld * 2};
-    const cuuint32_t box[2] = {box_cols, box_rows};
-    const cuuint32_t estr[2] = {1, 1};
-    CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), dims, strides, box, estr,
-                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) {
-        pifpaf::set_error("cuTensorMapEncodeTiled (plain) failed (%d): rows=%llu cols=%llu ld=%llu box=%ux%u", (int)r,
-                          (unsigned long long)rows, (unsigned long long)cols, (unsigned long long)ld, box_rows, box_cols);
-        return PIFPAF_E_CUDA;
-    }
-    return PIFPAF_OK;
+    const cuuint32_t box[2] = {box_cols, box_rows}, estr[2] = {1, 1};
+    return encode_tmap(map, "plain", base, 2, dims, &ld, box, estr, CU_TENSOR_MAP_SWIZZLE_NONE,
+                       CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
 }
 
 // 2-D bf16 output view for the TMA-store epilogue: box = 16 rows x 16 columns (32 bytes), 32-byte swizzle
 int make_tmap_store(CUtensorMap* map, const void* base, uint64_t rows, uint64_t cols, uint64_t ld) {
-    PFN_encodeTiled fn = get_encode_fn();
-    if (!fn) { pifpaf::set_error("cuTensorMapEncodeTiled entry point not available"); return PIFPAF_E_CUDA; }
     const cuuint64_t dims[2] = {cols, rows};
-    const cuuint64_t strides[1] = {ld * 2};
-    const cuuint32_t box[2] = {OUT_BOX_COLS, OUT_BOX_ROWS};
-    const cuuint32_t estr[2] = {1, 1};
-    CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), dims, strides, box, estr,
-                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_32B, CU_TENSOR_MAP_L2_PROMOTION_NONE,
-                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) {
-        pifpaf::set_error("cuTensorMapEncodeTiled (store) failed (%d): rows=%llu cols=%llu ld=%llu base=%p", (int)r,
-                          (unsigned long long)rows, (unsigned long long)cols, (unsigned long long)ld, base);
-        return PIFPAF_E_CUDA;
-    }
-    return PIFPAF_OK;
+    const cuuint32_t box[2] = {OUT_BOX_COLS, OUT_BOX_ROWS}, estr[2] = {1, 1};
+    return encode_tmap(map, "store", base, 2, dims, &ld, box, estr, CU_TENSOR_MAP_SWIZZLE_32B,
+                       CU_TENSOR_MAP_L2_PROMOTION_NONE);
 }
 
 // 4-D bf16 NHWC activation view {C, W, H, B} for implicit-GEMM convolutions: box = 64 channels x the
 // input window of a PH x PW output patch, traversed with the conv stride
 int make_tmap_conv(CUtensorMap* map, const void* base, uint64_t c, uint64_t w, uint64_t h, uint64_t b, uint64_t ld,
                    int stride) {
-    PFN_encodeTiled fn = get_encode_fn();
-    if (!fn) { pifpaf::set_error("cuTensorMapEncodeTiled entry point not available"); return PIFPAF_E_CUDA; }
-    const cuuint64_t dims[4] = {c, w, h, b};
-    const cuuint64_t strides[3] = {ld * 2, w * ld * 2, h * w * ld * 2};
+    const cuuint64_t dims[4] = {c, w, h, b}, lds[3] = {ld, w * ld, h * w * ld};
     const cuuint32_t box[4] = {BK, (cuuint32_t)((PW - 1) * stride + 1), (cuuint32_t)((PH - 1) * stride + 1), 1};
     const cuuint32_t estr[4] = {1, (cuuint32_t)stride, (cuuint32_t)stride, 1};
-    CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(base), dims, strides, box, estr,
-                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) {
-        pifpaf::set_error("cuTensorMapEncodeTiled (conv) failed (%d): c=%llu w=%llu h=%llu b=%llu ld=%llu stride=%d",
-                          (int)r, (unsigned long long)c, (unsigned long long)w, (unsigned long long)h,
-                          (unsigned long long)b, (unsigned long long)ld, stride);
-        return PIFPAF_E_CUDA;
-    }
-    return PIFPAF_OK;
+    return encode_tmap(map, "conv", base, 4, dims, lds, box, estr, CU_TENSOR_MAP_SWIZZLE_128B,
+                       CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
 }
 
 // 4-D bf16 NHWC view {C, W, H, B}, dense (un-swizzled) box of 64 channels x box_w x box_h pixels.
@@ -1848,22 +1821,9 @@ int make_tmap_conv(CUtensorMap* map, const void* base, uint64_t c, uint64_t w, u
 int make_tmap_dw(CUtensorMap* map, const void* base, uint64_t c, uint64_t w, uint64_t h, uint64_t b, uint64_t ld,
                  uint32_t box_w, uint32_t box_h, uint32_t box_c = 64,
                  CUtensorMapSwizzle swz = CU_TENSOR_MAP_SWIZZLE_NONE) {
-    PFN_encodeTiled fn = get_encode_fn();
-    if (!fn) { pifpaf::set_error("cuTensorMapEncodeTiled entry point not available"); return PIFPAF_E_CUDA; }
-    const cuuint64_t dims[4] = {c, w, h, b};
-    const cuuint64_t strides[3] = {ld * 2, w * ld * 2, h * w * ld * 2};
-    const cuuint32_t box[4] = {box_c, box_w, box_h, 1};
-    const cuuint32_t estr[4] = {1, 1, 1, 1};
-    CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(base), dims, strides, box, estr,
-                    CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_NONE,
-                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) {
-        pifpaf::set_error("cuTensorMapEncodeTiled (dw) failed (%d): c=%llu w=%llu h=%llu b=%llu ld=%llu box=%ux%u", (int)r,
-                          (unsigned long long)c, (unsigned long long)w, (unsigned long long)h, (unsigned long long)b,
-                          (unsigned long long)ld, box_w, box_h);
-        return PIFPAF_E_CUDA;
-    }
-    return PIFPAF_OK;
+    const cuuint64_t dims[4] = {c, w, h, b}, lds[3] = {ld, w * ld, h * w * ld};
+    const cuuint32_t box[4] = {box_c, box_w, box_h, 1}, estr[4] = {1, 1, 1, 1};
+    return encode_tmap(map, "dw", base, 4, dims, lds, box, estr, swz, CU_TENSOR_MAP_L2_PROMOTION_NONE);
 }
 
 // launch with (or without) the programmatic-stream-serialization attribute
@@ -1881,6 +1841,35 @@ cudaError_t launch_k(bool pdl, void (*kernel)(KArgs...), dim3 grid, dim3 block, 
     cfg.attrs = attr; cfg.numAttrs = n;
     return cudaLaunchKernelEx(&cfg, kernel, std::forward<Args>(args)...);
 }
+
+// the TMA depthwise kernels, one entry per instantiation: pifpaf_net_dwconv picks the entry of an op (and encodes
+// its box), the launch takes kernel, block, shared memory and grid from it, pifpaf_net_create sets its shared-memory limit
+using DwTmaKernel = decltype(&k_dwconv5_tma<1, DW1_TH, DW1_TW, 4, 3>);
+struct DwTmaVariant {
+    DwTmaKernel kernel;
+    int threads;
+    int smem;                 // dynamic shared memory (DW_K5_S2_CBF: the limit; a launch takes what its weights need)
+    int th, tw;               // output tile
+    int ctas_per_sm;          // persistent grid == resident CTAs (by shared memory)
+    uint32_t box_w, box_h;    // input window (TMA box)
+};
+enum { DW_K5_S1, DW_K5_S2, DW_K5_S2_CBF, DW_K3_S1, DW_K3_S2, DW_TMA_VARIANTS };
+const DwTmaVariant DW_TMA[DW_TMA_VARIANTS] = {
+    {k_dwconv5_tma<1, DW1_TH, DW1_TW, 4, 3>, DwS1::THREADS, DwS1::SMEM, DW1_TH, DW1_TW, 2, DwS1::IW, DwS1::IH},
+    {k_dwconv5_tma<2, DW2_TH, DW2_TW, 4, 2>, DwS2::THREADS, DwS2::SMEM, DW2_TH, DW2_TW, 1, DwS2::IW, DwS2::IH},
+    // channel-block-fastest item order with the weights staged in shared memory (PIFPAF_DW_CBF=1): DW_K5_S2's
+    // window and grid, chosen at launch while the weights fit
+    {k_dwconv5_tma<2, DW2_TH, DW2_TW, 4, 2, true>, DwS2::THREADS, 226 * 1024, DW2_TH, DW2_TW, 1, DwS2::IW, DwS2::IH},
+    {k_dwconv5_tma<1, DW1_TH, DW1_TW, 4, 4, false, 3>, DwS1K3::THREADS, DwS1K3::SMEM, DW1_TH, DW1_TW, 2, DwS1K3::IW,
+     DwS1K3::IH},
+    {k_dwconv5_tma<2, DW2_TH, DW2_TW, 4, 3, false, 3>, DwS2K3::THREADS, DwS2K3::SMEM, DW2_TH, DW2_TW, 1, DwS2K3::IW,
+     DwS2K3::IH}};
+
+// the stem instantiations, indexed [U8][KS / 2] (KS = 1, 3, 5, 7)
+using InConvKernel = decltype(&k_input_conv<1, false>);
+const InConvKernel INPUT_CONV_KERNELS[2][4] = {
+    {k_input_conv<1, false>, k_input_conv<3, false>, k_input_conv<5, false>, k_input_conv<7, false>},
+    {k_input_conv<1, true>, k_input_conv<3, true>, k_input_conv<5, true>, k_input_conv<7, true>}};
 
 struct Tensor { int h, w, c; __nv_bfloat16* data; };
 
@@ -1901,12 +1890,12 @@ struct Op {
     int store_rows = -1;
     // dw, max pool
     DwArgs dw{};
-    CUtensorMap tmap_dw{}; bool dw_tma = false;
+    CUtensorMap tmap_dw{};
+    const DwTmaVariant* dw_tma = nullptr;     // the TMA kernel of a depthwise op (nullptr: k_dwconv5 / k_dwconv)
     // fused depthwise -> GEMM (OP_FUSED): g + tmap_dw (windows) + tmap_b
     FusedArgs fu{};
     // input conv
     InConvArgs ic{};
-    int n_out_pixels = 0;
     double flops_per_image = 0;
     double bytes_per_image = 0;      // algorithmic activation bytes (inputs once + outputs once)
     double weight_bytes = 0;
@@ -2018,23 +2007,68 @@ int choose_stages(int block_n, int n_blocks, int num_k_blocks, bool shuffle) {
     return stages;
 }
 
-// weights-resident mode if the whole weight tile plus >= 3 A stages (and the pass-through double buffer) fit
-void plan_gemm_smem(GemmArgs& g, size_t* smem, bool src_tma) {
-    g.b_resident = 0;
-    if (g.conv_k == 0 && g.mode != MODE_HEADS &&
-        gemm_smem_bytes(g.block_n, g.n_blocks, 3, src_tma, true, g.num_k_blocks) <= GEMM_SMEM_BUDGET) {
-        int stages = 8;
-        while (gemm_smem_bytes(g.block_n, g.n_blocks, stages, src_tma, true, g.num_k_blocks) > GEMM_SMEM_BUDGET) stages--;
-        g.b_resident = 1;
-        g.stages = stages;
-        *smem = gemm_smem_bytes(g.block_n, g.n_blocks, stages, src_tma, true, g.num_k_blocks);
-        return;
-    }
-    g.stages = choose_stages(g.block_n, g.n_blocks, g.num_k_blocks, src_tma);
-    *smem = gemm_smem_bytes(g.block_n, g.n_blocks, g.stages, src_tma);
+// A stages of the weights-resident mode: as many as fit next to the whole weight tile (at most 8); 0 if 3 do not
+int resident_stages(int block_n, int n_blocks, int num_k_blocks, bool shuffle) {
+    if (gemm_smem_bytes(block_n, n_blocks, 3, shuffle, true, num_k_blocks) > GEMM_SMEM_BUDGET) return 0;
+    int stages = 8;
+    while (gemm_smem_bytes(block_n, n_blocks, stages, shuffle, true, num_k_blocks) > GEMM_SMEM_BUDGET) stages--;
+    return stages;
 }
 
-// common GEMM emit: weights [n_out][k_cols] f32 host -> bf16 [n_pad][k_pad8] device, bias padded
+// ring depth and shared memory of a GEMM op, once its mode is set: weights-resident mode if the whole weight tile plus
+// >= 3 A stages (and the pass-through double buffer) fit; implicit convolutions and the heads stream their weights
+void plan_gemm_smem(Op& op) {
+    GemmArgs& g = op.g;
+    const bool src_tma = g.src_tma != 0;
+    const int res = g.conv_k == 0 && g.mode != MODE_HEADS ? resident_stages(g.block_n, g.n_blocks, g.num_k_blocks, src_tma) : 0;
+    g.b_resident = res > 0 ? 1 : 0;
+    g.stages = res > 0 ? res : choose_stages(g.block_n, g.n_blocks, g.num_k_blocks, src_tma);
+    op.smem = gemm_smem_bytes(g.block_n, g.n_blocks, g.stages, src_tma, res > 0, g.num_k_blocks);
+}
+
+// GEMM weights on the device: torch's f32 [n_out][c_in][taps] -> bf16 [n_pad][taps * pitch] (tap t of channel c at
+// column t * pitch + c, zeros elsewhere) and the bias padded to n_pad.  The ALGORITHMIC work of the weights: padding
+// columns / rows (zero weights: view lead-ins of the 'shuffle' layout, 16-channel padding of the 'bins' pieces) are not
+// counted -- nnz MACs, the input channels some weight reads (k_real), the output channels some weight or bias produces
+// (n_real)
+struct GemmWeights { __nv_bfloat16* w = nullptr; float* bias = nullptr; long long nnz = 0; int k_real = 0, n_real = 0; };
+
+int upload_gemm_weights(pifpaf_net* net, const float* weight, const float* bias, int n_out, int c_in, int taps,
+                        int pitch, int n_pad, GemmWeights* gw) {
+    const size_t ld = (size_t)taps * pitch;
+    std::vector<__nv_bfloat16> w((size_t)n_pad * ld, __float2bfloat16(0.f));
+    std::vector<float> b(n_pad, 0.f);
+    std::vector<char> k_used(c_in, 0);
+    *gw = GemmWeights{};
+    for (int n = 0; n < n_out; n++) {
+        bool row = bias != nullptr && bias[n] != 0.f;
+        for (int c = 0; c < c_in; c++)
+            for (int t = 0; t < taps; t++) {
+                const float v = weight[((size_t)n * c_in + c) * taps + t];
+                w[(size_t)n * ld + (size_t)t * pitch + c] = __float2bfloat16(v);
+                if (v != 0.f) { gw->nnz++; k_used[c] = 1; row = true; }
+            }
+        gw->n_real += row ? 1 : 0;
+        b[n] = bias ? bias[n] : 0.f;
+    }
+    for (int c = 0; c < c_in; c++) gw->k_real += k_used[c];
+    const int rc = net_upload(net, &gw->w, w);
+    return rc != PIFPAF_OK ? rc : net_upload(net, &gw->bias, b);
+}
+
+// depthwise weights on the device: torch's f32 [channels][taps] -> tap-major [taps][C], the bias padded to C
+int upload_dw_weights(pifpaf_net* net, const float* weight, const float* bias, int channels, int C, int taps,
+                      float** d_w, float** d_b) {
+    std::vector<float> w((size_t)taps * C, 0.f), b(C, 0.f);
+    for (int c = 0; c < channels; c++) {
+        for (int t = 0; t < taps; t++) w[(size_t)t * C + c] = weight[(size_t)c * taps + t];
+        b[c] = bias ? bias[c] : 0.f;
+    }
+    const int rc = net_upload(net, d_w, w);
+    return rc != PIFPAF_OK ? rc : net_upload(net, d_b, b);
+}
+
+// common 1x1 GEMM emit: weights [n_out][k_cols] f32 host -> bf16 [n_pad][k_pad8] device, bias padded
 int emit_gemm(pifpaf_net* net, Op& op, int in_tensor, int in_col_off, int k_cols, int n_out,
               const float* weight, const float* bias) {
     const Tensor& tin = net->tensors[in_tensor];
@@ -2043,81 +2077,106 @@ int emit_gemm(pifpaf_net* net, Op& op, int in_tensor, int in_col_off, int k_cols
                      "conv1x1 input column window must start on a multiple of 8 channels and lie inside the tensor");
     int block_n, n_blocks;
     choose_block_n(n_out, &block_n, &n_blocks);
+    const int num_k_blocks = (k_cols + BK - 1) / BK;
     // weights-resident GEMMs stream A through what the resident weight tile leaves of the shared memory: with
     // K = 352..416 and a 176..208-column tile that is 4-5 stages of 16 KB, too few bytes in flight per SM to cover
     // the DRAM latency.  Narrower tiles (more
     // n blocks, A re-read from L2 by each of them) buy the stages back.
     if (net->gemm_res_stages > 0) {
-        const int kb = (k_cols + BK - 1) / BK, np = pad16(n_out);
-        auto res_stages = [&](int bn, int nb) {
-            if (gemm_smem_bytes(bn, nb, 3, false, true, kb) > GEMM_SMEM_BUDGET) return 0;       // not resident at all
-            int st = 8;
-            while (gemm_smem_bytes(bn, nb, st, false, true, kb) > GEMM_SMEM_BUDGET) st--;
-            return st;
-        };
-        int st = res_stages(block_n, n_blocks);
+        const int np = pad16(n_out);
+        int st = resident_stages(block_n, n_blocks, num_k_blocks, false);
         while (st > 0 && st < net->gemm_res_stages && block_n > 64) {
             const int nb = n_blocks + 1, bn = pad16((np + nb - 1) / nb);
             if (bn < 64) break;
             n_blocks = nb; block_n = bn;
-            st = res_stages(block_n, n_blocks);
+            st = resident_stages(block_n, n_blocks, num_k_blocks, false);
         }
     }
     const int n_pad = block_n * n_blocks;
     const int k_pad = pad8(k_cols);
-    std::vector<__nv_bfloat16> w((size_t)n_pad * k_pad, __float2bfloat16(0.f));
-    for (int n = 0; n < n_out; n++)
-        for (int k = 0; k < k_cols; k++) w[(size_t)n * k_pad + k] = __float2bfloat16(weight[(size_t)n * k_cols + k]);
-    std::vector<float> b(n_pad, 0.f);
-    for (int n = 0; n < n_out; n++) b[n] = bias ? bias[n] : 0.f;
-    __nv_bfloat16* d_w = nullptr; float* d_b = nullptr;
-    int rc = net_upload(net, &d_w, w); if (rc != PIFPAF_OK) return rc;
-    rc = net_upload(net, &d_b, b); if (rc != PIFPAF_OK) return rc;
+    GemmWeights gw;
+    int rc = upload_gemm_weights(net, weight, bias, n_out, k_cols, 1, k_pad, n_pad, &gw);
+    if (rc != PIFPAF_OK) return rc;
 
     GemmArgs& g = op.g;
     const size_t rows_max = (size_t)net->max_batch * tin.h * tin.w;
     g.N = n_out; g.K = k_cols; g.a_col0 = in_col_off;
     g.block_n = block_n; g.n_blocks = n_blocks;
-    g.num_k_blocks = (k_cols + BK - 1) / BK;
-    g.stages = choose_stages(block_n, n_blocks, g.num_k_blocks, false);
-    g.bias = d_b;
-    g.a = tin.data + in_col_off; g.lda = tin.c; g.wgt = d_w; g.ldw = k_pad;
+    g.num_k_blocks = num_k_blocks;
+    g.bias = gw.bias;
+    g.a = tin.data + in_col_off; g.lda = tin.c; g.wgt = gw.w; g.ldw = k_pad;
     op.a_tensor = in_tensor; op.rows_per_image = tin.h * tin.w;
-    op.smem = gemm_smem_bytes(block_n, n_blocks, g.stages, false);
-    // ALGORITHMIC work: padding columns / rows (zero weights: view lead-ins of the 'shuffle' layout, 16-channel
-    // padding of the 'bins' pieces) are not counted -- nnz MACs, the input channels some weight reads, the output
-    // channels some weight or bias produces
-    long long nnz = 0; int k_real = 0, n_real = 0;
-    {
-        std::vector<char> k_used(k_cols, 0);
-        for (int n = 0; n < n_out; n++) {
-            bool row = bias != nullptr && bias[n] != 0.f;
-            for (int k = 0; k < k_cols; k++)
-                if (weight[(size_t)n * k_cols + k] != 0.f) { nnz++; k_used[k] = 1; row = true; }
-            n_real += row ? 1 : 0;
-        }
-        for (int k = 0; k < k_cols; k++) k_real += k_used[k];
-    }
-    op.n_real = n_real;
-    op.flops_per_image = 2.0 * (double)op.rows_per_image * (double)nnz;
-    op.bytes_per_image = (double)op.rows_per_image * k_real * 2.0;      // A read once (bf16); outputs added by the caller
+    op.n_real = gw.n_real;
+    op.flops_per_image = 2.0 * (double)op.rows_per_image * (double)gw.nnz;
+    op.bytes_per_image = (double)op.rows_per_image * gw.k_real * 2.0;      // A read once (bf16); outputs added by the caller
     op.a_bytes_per_image = op.bytes_per_image;
-    op.weight_bytes = (double)nnz * 2.0;
+    op.weight_bytes = (double)gw.nnz * 2.0;
     // the map covers the whole tensor; the view's first column is a TMA coordinate (16-byte aligned).
     // Columns past the view multiply zero weight rows (B is zero padded), columns past the tensor are zero filled.
     rc = make_tmap(&op.tmap_a, tin.data, rows_max, (uint64_t)tin.c, (uint64_t)tin.c, BM);
     if (rc != PIFPAF_OK) return rc;
-    rc = make_tmap(&op.tmap_b, d_w, (uint64_t)n_pad, (uint64_t)k_pad, (uint64_t)k_pad, (uint32_t)block_n);
+    rc = make_tmap(&op.tmap_b, gw.w, (uint64_t)n_pad, (uint64_t)k_pad, (uint64_t)k_pad, (uint32_t)block_n);
     return rc;
 }
 
-// plain 1x1 GEMM without residual: the TMA-store epilogue writes the window [out_col_off, + pad8(N)) of `to`.
+// the residual a plain GEMM epilogue adds: columns [residual_col_off, + N) of an ho x wo tensor
+int set_residual(const pifpaf_net* net, GemmArgs& g, int residual_tensor, int residual_col_off, int ho, int wo) {
+    PIFPAF_CHECK_ARG(residual_tensor < (int)net->tensors.size(), "bad residual tensor");
+    const Tensor& tr = net->tensors[residual_tensor];
+    PIFPAF_CHECK_ARG(tr.h == ho && tr.w == wo && residual_col_off % 8 == 0 && residual_col_off + g.N <= tr.c,
+                     "residual tensor shape mismatch");
+    g.res = tr.data; g.ld_res = tr.c; g.res_col_off = residual_col_off;
+    return PIFPAF_OK;
+}
+
+// plain 1x1 GEMM epilogue into the window [out_col_off, + pad8(N)) of `to`: with a residual (residual_tensor >= 0)
+// the per-lane epilogue adds it, without one the TMA-store epilogue writes the window.
 // ReLU6 GEMMs keep the per-lane epilogue: a ReLU6 clamp in the TMA-store epilogue (a uniform branch per fragment
 // group) slowed the ShuffleNetV2K forward, which never uses it, by 0.15 ms of 24.7 (64 images at 641 px, H100)
-void plan_tma_store_plain(const pifpaf_net* net, Op& op, const Tensor& to) {
-    if (!net->gemm_tma_store || op.g.relu == ACT_RELU6) return;
-    op.g.tma_store = 1;
-    op.store_views = {Op::StoreView{to.data + op.g.out_col_off, pad8(op.g.N), to.c}};
+int set_plain_epilogue(const pifpaf_net* net, Op& op, int relu, const Tensor& to, int out_col_off,
+                       int residual_tensor, int residual_col_off) {
+    GemmArgs& g = op.g;
+    g.mode = MODE_PLAIN; g.relu = relu; g.out = to.data; g.ldo = to.c; g.out_col_off = out_col_off;
+    op.bytes_per_image += (double)op.rows_per_image * op.n_real * 2.0 * (residual_tensor >= 0 ? 2.0 : 1.0);
+    if (residual_tensor >= 0) return set_residual(net, g, residual_tensor, residual_col_off, to.h, to.w);
+    if (net->gemm_tma_store && g.relu != ACT_RELU6) {
+        g.tma_store = 1;
+        op.store_views = {Op::StoreView{to.data + g.out_col_off, pad8(g.N), to.c}};
+    }
+    return PIFPAF_OK;
+}
+
+// destination table of a scatter epilogue, uploaded: the pieces tile [0, n_out) in order, in multiples of 16 columns;
+// piece i lands in the columns [piece_tensor_col[i], + piece_count[i]) of tensor piece_tensor[i] (h x w pixels).
+// Entry j covers the 16 columns from 16 j: base, row pitch and `store` = (store map << 16) | first column, for the
+// TMA-store epilogue with one store map per destination tensor (map_tensor, in order of first use)
+int upload_dest_groups(pifpaf_net* net, int n_pad, int n_out, int h, int w, int n_pieces, const int32_t* piece_col0,
+                       const int32_t* piece_count, const int32_t* piece_tensor, const int32_t* piece_tensor_col,
+                       const DestGroup** d_groups, std::vector<int>* map_tensor) {
+    std::vector<DestGroup> groups((size_t)n_pad / 16, DestGroup{nullptr, 0, 0});
+    map_tensor->clear();
+    int expect = 0;
+    for (int i = 0; i < n_pieces; i++) {
+        PIFPAF_CHECK_ARG(piece_col0[i] == expect && piece_count[i] >= 16 && piece_count[i] % 16 == 0,
+                         "pieces must tile [0, n_out) in order, in multiples of 16 columns");
+        PIFPAF_CHECK_ARG(piece_tensor[i] >= 0 && piece_tensor[i] < (int)net->tensors.size(), "bad piece tensor id");
+        const Tensor& to = net->tensors[piece_tensor[i]];
+        PIFPAF_CHECK_ARG(to.h == h && to.w == w, "a piece tensor must have the output's spatial shape");
+        PIFPAF_CHECK_ARG(piece_tensor_col[i] >= 0 && piece_tensor_col[i] % 16 == 0 &&
+                         piece_tensor_col[i] + piece_count[i] <= to.c, "piece window outside its tensor");
+        int mi = 0;
+        while (mi < (int)map_tensor->size() && (*map_tensor)[mi] != piece_tensor[i]) mi++;
+        if (mi == (int)map_tensor->size()) map_tensor->push_back(piece_tensor[i]);
+        for (int c = 0; c < piece_count[i]; c += 16)
+            groups[(size_t)(expect + c) / 16] = DestGroup{to.data + piece_tensor_col[i] + c, to.c,
+                                                          (mi << 16) | (piece_tensor_col[i] + c)};
+        expect += piece_count[i];
+    }
+    PIFPAF_CHECK_ARG(expect == n_out, "pieces must cover all n_out columns");
+    DestGroup* d = nullptr;
+    const int rc = net_upload(net, &d, groups);
+    *d_groups = d;
+    return rc;
 }
 
 // Decides, once all ops are known, which 1x1 GEMM -> depthwise pairs run as one k_pw_dw launch.  The GEMM qualifies
@@ -2131,15 +2190,14 @@ int plan_pw_dw(pifpaf_net* net) {
     for (size_t i = 0; i + 1 < net->ops.size(); i++) {
         Op& gop = net->ops[i];
         Op& dop = net->ops[i + 1];
-        if (gop.kind != OP_GEMM || dop.kind != OP_DW || !dop.dw_tma) continue;
+        if (gop.kind != OP_GEMM || dop.kind != OP_DW || dop.dw_tma != &DW_TMA[DW_K5_S2]) continue;
         const GemmArgs& g = gop.g;
         const DwArgs& d = dop.dw;
         if (g.mode != MODE_PLAIN || g.conv_k != 0 || g.res != nullptr || g.num_k_blocks != 1 || g.a_col0 != 0 ||
             g.out_col_off != 0 || g.relu == ACT_RELU6)
             continue;
-        // k_pw_dw is built for the 5x5 stride-2 depthwise conv with ReLU at most (not MobileNetV2's 3x3 + ReLU6 pairs)
-        if (d.kernel != 5 || d.stride != 2 || d.pad != 2 || d.relu == ACT_RELU6 || d.in != g.out || d.in_col_off != 0)
-            continue;
+        // k_pw_dw is built for the 5x5 stride-2 depthwise conv (DW_K5_S2: ReLU at most, not MobileNetV2's 3x3 + ReLU6 pairs)
+        if (d.pad != 2 || d.in != g.out || d.in_col_off != 0) continue;
         const Tensor& tin = net->tensors[gop.a_tensor];
         if (tin.c > PWDW_K) continue;
         int t_mid = -1;
@@ -2230,31 +2288,18 @@ int pifpaf_net_create(pifpaf_net_t** out, int32_t device, int32_t max_batch) {
     if (const char* e = std::getenv("PIFPAF_GEMM_RES_STAGES")) net->gemm_res_stages = std::atoi(e);
     if (const char* e = std::getenv("PIFPAF_GEMM_TMA_STORE")) net->gemm_tma_store = std::atoi(e) != 0;
     if (const char* e = std::getenv("PIFPAF_FUSE_PW_DW")) net->fuse_pw_dw = std::atoi(e) != 0;
+    // the shared-memory limit of every kernel the forward launches with more than the default 48 KB, from the tables the
+    // launches index (the stem stages its weights: 7x7 with more than 72 channels is past 48 KB)
     PIFPAF_CUDA_TRY(cudaFuncSetAttribute(k_pw_dw<2, PWDW_TH, PWDW_TW, PWDW_BW>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                          226 * 1024));
     for (auto& row : GEMM_KERNELS)
         for (auto* k : row) PIFPAF_CUDA_TRY(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024));
     for (auto& row : DW_GEMM_KERNELS)
         for (auto* k : row) PIFPAF_CUDA_TRY(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024));
-    PIFPAF_CUDA_TRY(cudaFuncSetAttribute(k_dwconv5_tma<1, DW1_TH, DW1_TW, 4, 3>,
-                                         cudaFuncAttributeMaxDynamicSharedMemorySize, DwS1::SMEM));
-    PIFPAF_CUDA_TRY(cudaFuncSetAttribute(k_dwconv5_tma<2, DW2_TH, DW2_TW, 4, 2>,
-                                         cudaFuncAttributeMaxDynamicSharedMemorySize, DwS2::SMEM));
-    PIFPAF_CUDA_TRY(cudaFuncSetAttribute(k_dwconv5_tma<2, DW2_TH, DW2_TW, 4, 2, true>,
-                                         cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024));
-    PIFPAF_CUDA_TRY(cudaFuncSetAttribute(k_dwconv5_tma<1, DW1_TH, DW1_TW, 4, 4, false, 3>,
-                                         cudaFuncAttributeMaxDynamicSharedMemorySize, DwS1K3::SMEM));
-    PIFPAF_CUDA_TRY(cudaFuncSetAttribute(k_dwconv5_tma<2, DW2_TH, DW2_TW, 4, 3, false, 3>,
-                                         cudaFuncAttributeMaxDynamicSharedMemorySize, DwS2K3::SMEM));
-    // the stem stages its weights in shared memory: 7x7 with more than 72 channels is past the default 48 KB
-    PIFPAF_CUDA_TRY(cudaFuncSetAttribute(k_input_conv<1, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, INCONV_SMEM_MAX));
-    PIFPAF_CUDA_TRY(cudaFuncSetAttribute(k_input_conv<3, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, INCONV_SMEM_MAX));
-    PIFPAF_CUDA_TRY(cudaFuncSetAttribute(k_input_conv<5, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, INCONV_SMEM_MAX));
-    PIFPAF_CUDA_TRY(cudaFuncSetAttribute(k_input_conv<7, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, INCONV_SMEM_MAX));
-    PIFPAF_CUDA_TRY(cudaFuncSetAttribute(k_input_conv<1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, INCONV_SMEM_MAX));
-    PIFPAF_CUDA_TRY(cudaFuncSetAttribute(k_input_conv<3, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, INCONV_SMEM_MAX));
-    PIFPAF_CUDA_TRY(cudaFuncSetAttribute(k_input_conv<5, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, INCONV_SMEM_MAX));
-    PIFPAF_CUDA_TRY(cudaFuncSetAttribute(k_input_conv<7, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, INCONV_SMEM_MAX));
+    for (const DwTmaVariant& v : DW_TMA)
+        PIFPAF_CUDA_TRY(cudaFuncSetAttribute(v.kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, v.smem));
+    for (auto& row : INPUT_CONV_KERNELS)
+        for (auto* k : row) PIFPAF_CUDA_TRY(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, INCONV_SMEM_MAX));
     *out = net;
     return PIFPAF_OK;
 }
@@ -2336,14 +2381,11 @@ int pifpaf_net_conv1x1(pifpaf_net_t* net, int32_t in_tensor, int32_t in_col_off,
     int rc = emit_gemm(net, op, in_tensor, in_col_off, k_cols, n_out, weight, bias);
     if (rc != PIFPAF_OK) return rc;
     GemmArgs& g = op.g;
-    g.relu = relu; g.out = to.data; g.ldo = to.c; g.out_col_off = out_col_off;
-    // outputs: n_out bf16 per row; the fused shuffle also reads and re-writes the pass-through half
-    op.bytes_per_image += (double)op.rows_per_image * op.n_real * 2.0 * (shuffle_src_tensor >= 0 ? 3.0 : 1.0);
     PIFPAF_CHECK_ARG(out_col_off % 16 == 0, "output column offset must be a multiple of 16");
     if (shuffle_src_tensor < 0) {
-        g.mode = MODE_PLAIN;
         PIFPAF_CHECK_ARG(out_col_off + pad8(n_out) <= to.c, "output window outside the tensor");
-        plan_tma_store_plain(net, op, to);
+        rc = set_plain_epilogue(net, op, relu, to, out_col_off, -1, 0);
+        if (rc != PIFPAF_OK) return rc;
     } else {
         PIFPAF_CHECK_ARG(shuffle_src_tensor < nt, "bad shuffle source tensor");
         const Tensor& ts = net->tensors[shuffle_src_tensor];
@@ -2352,7 +2394,9 @@ int pifpaf_net_conv1x1(pifpaf_net_t* net, int32_t in_tensor, int32_t in_col_off,
         PIFPAF_CHECK_ARG(shuffle_src_col_off % 8 == 0 && shuffle_src_col_off + pad16(n_out) <= ts.c + 8,
                          "shuffle source window");
         PIFPAF_CHECK_ARG(out_col_off == 0 && to.c >= 2 * n_out, "shuffle output tensor must hold 2*n_out channels");
-        g.mode = MODE_SHUFFLE;
+        g.mode = MODE_SHUFFLE; g.relu = relu; g.out = to.data; g.ldo = to.c; g.out_col_off = out_col_off;
+        // outputs: n_out bf16 per row, and the pass-through half read and re-written
+        op.bytes_per_image += (double)op.rows_per_image * op.n_real * 2.0 * 3.0;
         g.src0 = ts.data; g.ld0 = ts.c; g.src0_col_off = shuffle_src_col_off;
         g.half = n_out; g.gap = 0;
         g.src_tma = gemm_smem_bytes(g.block_n, g.n_blocks, 2, true) <= GEMM_SMEM_BUDGET ? 1 : 0;
@@ -2362,7 +2406,7 @@ int pifpaf_net_conv1x1(pifpaf_net_t* net, int32_t in_tensor, int32_t in_col_off,
                              (uint32_t)g.block_n, BM);
         if (rc != PIFPAF_OK) return rc;
     }
-    plan_gemm_smem(g, &op.smem, g.src_tma != 0);
+    plan_gemm_smem(op);
     op.touches = {in_tensor, out_tensor, shuffle_src_tensor};
     net->ops.push_back(op);
     return PIFPAF_OK;
@@ -2385,28 +2429,12 @@ int pifpaf_net_conv1x1_scatter(pifpaf_net_t* net, int32_t in_tensor, int32_t in_
     if (rc != PIFPAF_OK) return rc;
     GemmArgs& g = op.g;
     g.mode = MODE_SCATTER; g.relu = relu;
-    std::vector<DestGroup> groups((size_t)g.n_blocks * g.block_n / 16, DestGroup{nullptr, 0, 0});
-    // TMA-store epilogue: one store map per destination tensor (a chunk's box covers exactly its 16 columns)
     std::vector<int> map_tensor;
-    int expect = 0;
-    for (int i = 0; i < n_pieces; i++) {
-        PIFPAF_CHECK_ARG(piece_col0[i] == expect && piece_count[i] >= 16 && piece_count[i] % 16 == 0,
-                         "pieces must tile [0, n_out) in order, in multiples of 16 columns");
-        PIFPAF_CHECK_ARG(piece_tensor[i] >= 0 && piece_tensor[i] < nt, "bad piece tensor id");
-        const Tensor& to = net->tensors[piece_tensor[i]];
-        PIFPAF_CHECK_ARG(to.h == tin.h && to.w == tin.w, "conv1x1 keeps the spatial shape");
-        PIFPAF_CHECK_ARG(piece_tensor_col[i] >= 0 && piece_tensor_col[i] % 16 == 0 &&
-                         piece_tensor_col[i] + piece_count[i] <= to.c, "piece window outside its tensor");
-        int mi = 0;
-        while (mi < (int)map_tensor.size() && map_tensor[mi] != piece_tensor[i]) mi++;
-        if (mi == (int)map_tensor.size()) map_tensor.push_back(piece_tensor[i]);
-        for (int c = 0; c < piece_count[i]; c += 16)
-            groups[(size_t)(expect + c) / 16] = DestGroup{to.data + piece_tensor_col[i] + c, to.c,
-                                                          (mi << 16) | (piece_tensor_col[i] + c)};
-        expect += piece_count[i];
-    }
-    PIFPAF_CHECK_ARG(expect == n_out, "pieces must cover all n_out columns");
-    // more destination tensors than store maps: the per-lane store epilogue
+    rc = upload_dest_groups(net, g.n_blocks * g.block_n, n_out, tin.h, tin.w, n_pieces, piece_col0, piece_count,
+                            piece_tensor, piece_tensor_col, &g.dest, &map_tensor);
+    if (rc != PIFPAF_OK) return rc;
+    // TMA-store epilogue: one store map per destination tensor (a chunk's box covers exactly its 16 columns); more
+    // destination tensors than store maps: the per-lane store epilogue
     if (net->gemm_tma_store && (int)map_tensor.size() <= MAX_STORE_MAPS) {
         g.tma_store = 1;
         for (int t : map_tensor) {
@@ -2414,12 +2442,8 @@ int pifpaf_net_conv1x1_scatter(pifpaf_net_t* net, int32_t in_tensor, int32_t in_
             op.store_views.push_back(Op::StoreView{to.data, to.c, to.c});
         }
     }
-    DestGroup* d_groups = nullptr;
-    rc = net_upload(net, &d_groups, groups);
-    if (rc != PIFPAF_OK) return rc;
-    g.dest = d_groups;
     op.bytes_per_image += (double)op.rows_per_image * op.n_real * 2.0;
-    plan_gemm_smem(g, &op.smem, false);
+    plan_gemm_smem(op);
     op.touches.assign(piece_tensor, piece_tensor + n_pieces);
     op.touches.push_back(in_tensor);
     net->ops.push_back(op);
@@ -2461,19 +2485,9 @@ int pifpaf_net_conv_dilated(pifpaf_net_t* net, int32_t in_tensor, int32_t in_col
         Op op; op.kind = OP_GEMM;
         int rc = emit_gemm(net, op, in_tensor, in_col_off, c_in, n_out, weight, bias);
         if (rc != PIFPAF_OK) return rc;
-        GemmArgs& g = op.g;
-        g.mode = MODE_PLAIN; g.relu = relu; g.out = to.data; g.ldo = to.c; g.out_col_off = out_col_off;
-        op.bytes_per_image += (double)op.rows_per_image * op.n_real * 2.0 * (residual_tensor >= 0 ? 2.0 : 1.0);
-        if (residual_tensor >= 0) {
-            PIFPAF_CHECK_ARG(residual_tensor < nt, "bad residual tensor");
-            const Tensor& tr = net->tensors[residual_tensor];
-            PIFPAF_CHECK_ARG(tr.h == ho && tr.w == wo && residual_col_off % 8 == 0 && residual_col_off + n_out <= tr.c,
-                             "residual tensor shape mismatch");
-            g.res = tr.data; g.ld_res = tr.c; g.res_col_off = residual_col_off;
-        } else {
-            plan_tma_store_plain(net, op, to);
-        }
-        plan_gemm_smem(g, &op.smem, false);
+        rc = set_plain_epilogue(net, op, relu, to, out_col_off, residual_tensor, residual_col_off);
+        if (rc != PIFPAF_OK) return rc;
+        plan_gemm_smem(op);
         op.touches = {in_tensor, out_tensor, residual_tensor};
         net->ops.push_back(op);
         return PIFPAF_OK;
@@ -2484,44 +2498,34 @@ int pifpaf_net_conv_dilated(pifpaf_net_t* net, int32_t in_tensor, int32_t in_col
     const int n_pad = block_n * n_blocks;
     const int taps = kernel * kernel, cblocks = (c_in + BK - 1) / BK;
     const int k_total = taps * cblocks * BK;
-    // torch weight [n_out][c_in][k][k] -> bf16 [n_pad][tap][cblocks*64]
-    std::vector<__nv_bfloat16> w((size_t)n_pad * k_total, __float2bfloat16(0.f));
-    for (int n = 0; n < n_out; n++)
-        for (int c = 0; c < c_in; c++)
-            for (int t = 0; t < taps; t++)
-                w[(size_t)n * k_total + (size_t)t * cblocks * BK + c] = __float2bfloat16(weight[((size_t)n * c_in + c) * taps + t]);
-    std::vector<float> b(n_pad, 0.f);
-    for (int n = 0; n < n_out; n++) b[n] = bias ? bias[n] : 0.f;
-    __nv_bfloat16* d_w = nullptr; float* d_b = nullptr;
-    int rc = net_upload(net, &d_w, w); if (rc != PIFPAF_OK) return rc;
-    rc = net_upload(net, &d_b, b); if (rc != PIFPAF_OK) return rc;
+    // bf16 [n_pad][tap][cblocks*64]
+    GemmWeights gw;
+    int rc = upload_gemm_weights(net, weight, bias, n_out, c_in, taps, cblocks * BK, n_pad, &gw);
+    if (rc != PIFPAF_OK) return rc;
     GemmArgs& g = op.g;
     g.N = n_out; g.K = c_in;
     g.block_n = block_n; g.n_blocks = n_blocks;
     g.num_k_blocks = taps * cblocks;
-    g.stages = choose_stages(block_n, n_blocks, g.num_k_blocks, false);
-    g.bias = d_b; g.mode = MODE_PLAIN; g.relu = relu;
+    g.bias = gw.bias; g.mode = MODE_PLAIN; g.relu = relu;
     g.out = to.data; g.ldo = to.c; g.out_col_off = out_col_off;
     g.conv_k = kernel; g.conv_stride = stride; g.conv_pad = pad; g.conv_dil = dilation; g.conv_cblocks = cblocks;
     g.Hi = tin.h; g.Wi = tin.w; g.Ho = ho; g.Wo = wo;
     g.tiles_x = (wo + PW - 1) / PW; g.tiles_y = (ho + PH - 1) / PH;
-    g.a = tin.data + in_col_off; g.lda = tin.c; g.wgt = d_w; g.ldw = k_total;
+    g.a = tin.data + in_col_off; g.lda = tin.c; g.wgt = gw.w; g.ldw = k_total;
     if (residual_tensor >= 0) {
-        PIFPAF_CHECK_ARG(residual_tensor < nt, "bad residual tensor");
-        const Tensor& tr = net->tensors[residual_tensor];
-        PIFPAF_CHECK_ARG(tr.h == ho && tr.w == wo && residual_col_off % 8 == 0 && residual_col_off + n_out <= tr.c,
-                         "residual tensor shape mismatch");
-        g.res = tr.data; g.ld_res = tr.c; g.res_col_off = residual_col_off;
+        rc = set_residual(net, g, residual_tensor, residual_col_off, ho, wo);
+        if (rc != PIFPAF_OK) return rc;
     }
     op.a_tensor = in_tensor; op.rows_per_image = ho * wo; op.tiles_per_image = g.tiles_x * g.tiles_y;
-    op.smem = gemm_smem_bytes(block_n, n_blocks, g.stages, false);
+    plan_gemm_smem(op);
+    // dense shapes: every weight and input channel counted
     op.flops_per_image = 2.0 * (double)ho * wo * n_out * c_in * taps;
     op.bytes_per_image = (double)tin.h * tin.w * c_in * 2.0 + (double)ho * wo * n_out * 2.0 * (residual_tensor >= 0 ? 2.0 : 1.0);
     op.weight_bytes = (double)n_out * c_in * taps * 2.0;
     rc = make_tmap_conv(&op.tmap_a, tin.data + in_col_off, (uint64_t)c_in, (uint64_t)tin.w, (uint64_t)tin.h,
                         (uint64_t)net->max_batch, (uint64_t)tin.c, stride);
     if (rc != PIFPAF_OK) return rc;
-    rc = make_tmap(&op.tmap_b, d_w, (uint64_t)n_pad, (uint64_t)k_total, (uint64_t)k_total, (uint32_t)block_n);
+    rc = make_tmap(&op.tmap_b, gw.w, (uint64_t)n_pad, (uint64_t)k_total, (uint64_t)k_total, (uint32_t)block_n);
     if (rc != PIFPAF_OK) return rc;
     op.touches = {in_tensor, out_tensor, residual_tensor};
     net->ops.push_back(op);
@@ -2543,15 +2547,10 @@ int pifpaf_net_dwconv(pifpaf_net_t* net, int32_t in_tensor, int32_t in_col_off, 
     PIFPAF_CHECK_ARG(in_col_off % 8 == 0 && out_col_off % 8 == 0 && in_col_off + C <= tin.c && out_col_off + C <= to.c,
                      "dwconv column windows");
     PIFPAF_CUDA_TRY(cudaSetDevice(net->device));
-    std::vector<float> w((size_t)kernel * kernel * C, 0.f), b(C, 0.f);
-    for (int c = 0; c < channels; c++) {
-        for (int t = 0; t < kernel * kernel; t++) w[(size_t)t * C + c] = weight[(size_t)c * kernel * kernel + t];
-        b[c] = bias ? bias[c] : 0.f;
-    }
     Op op; op.kind = OP_DW;
     float *d_w = nullptr, *d_b = nullptr;
-    int rc = net_upload(net, &d_w, w); if (rc != PIFPAF_OK) return rc;
-    rc = net_upload(net, &d_b, b); if (rc != PIFPAF_OK) return rc;
+    int rc = upload_dw_weights(net, weight, bias, channels, C, kernel * kernel, &d_w, &d_b);
+    if (rc != PIFPAF_OK) return rc;
     DwArgs& a = op.dw;
     a.in = tin.data; a.ld_in = tin.c; a.in_col_off = in_col_off;
     a.out = to.data; a.ld_out = to.c; a.out_col_off = out_col_off;
@@ -2561,12 +2560,10 @@ int pifpaf_net_dwconv(pifpaf_net_t* net, int32_t in_tensor, int32_t in_col_off, 
     op.flops_per_image = 2.0 * ho * wo * channels * (double)kernel * kernel;
     op.bytes_per_image = ((double)tin.h * tin.w + (double)ho * wo) * channels * 2.0;
     if ((kernel == 3 || (kernel == 5 && relu != ACT_RELU6)) && (stride == 1 || stride == 2)) {
-        const uint32_t bw = kernel == 3 ? (stride == 1 ? DwS1K3::IW : DwS2K3::IW) : (stride == 1 ? DwS1::IW : DwS2::IW);
-        const uint32_t bh = kernel == 3 ? (stride == 1 ? DwS1K3::IH : DwS2K3::IH) : (stride == 1 ? DwS1::IH : DwS2::IH);
+        op.dw_tma = &DW_TMA[kernel == 3 ? (stride == 1 ? DW_K3_S1 : DW_K3_S2) : (stride == 1 ? DW_K5_S1 : DW_K5_S2)];
         rc = make_tmap_dw(&op.tmap_dw, tin.data + in_col_off, (uint64_t)C, (uint64_t)tin.w, (uint64_t)tin.h,
-                          (uint64_t)net->max_batch, (uint64_t)tin.c, bw, bh);
+                          (uint64_t)net->max_batch, (uint64_t)tin.c, op.dw_tma->box_w, op.dw_tma->box_h);
         if (rc != PIFPAF_OK) return rc;
-        op.dw_tma = true;
     }
     op.touches = {in_tensor, out_tensor};
     op.dw_out_bytes_per_image = (double)ho * wo * channels * 2.0;
@@ -2620,62 +2617,28 @@ int pifpaf_net_dw_conv1x1_scatter(pifpaf_net_t* net, int32_t in_tensor, int32_t 
     PIFPAF_CHECK_ARG(in_col_off % 8 == 0 && in_col_off + C <= tin.c, "depthwise column window");
     PIFPAF_CUDA_TRY(cudaSetDevice(net->device));
     Op op; op.kind = OP_FUSED;
-    // depthwise weights [C][25] -> tap-major [25][C]
-    std::vector<float> dww((size_t)25 * C, 0.f), dwb(C, 0.f);
-    for (int c = 0; c < channels; c++) {
-        for (int t = 0; t < 25; t++) dww[(size_t)t * C + c] = dw_weight[(size_t)c * 25 + t];
-        dwb[c] = dw_bias ? dw_bias[c] : 0.f;
-    }
     float *d_dww = nullptr, *d_dwb = nullptr;
-    int rc = net_upload(net, &d_dww, dww); if (rc != PIFPAF_OK) return rc;
-    rc = net_upload(net, &d_dwb, dwb); if (rc != PIFPAF_OK) return rc;
-    // 1x1 weights [n_out][channels] -> bf16 [n_pad][k_pad]
+    int rc = upload_dw_weights(net, dw_weight, dw_bias, channels, C, 25, &d_dww, &d_dwb);
+    if (rc != PIFPAF_OK) return rc;
     FusedArgs& f = op.fu;
     // column blocks of at most FD_MAX_BLOCK_N: one CTA (and one depthwise pass) per block
     const int n_blocks = (n_out + FD_MAX_BLOCK_N - 1) / FD_MAX_BLOCK_N;
     const int block_n = pad16((n_out + n_blocks - 1) / n_blocks);
     const int n_pad = block_n * n_blocks;
     f.dw_weight = d_dww; f.dw_bias = d_dwb; f.C = C; f.dw_relu = dw_relu; f.pad = pad;
-    const int k_pad = C;
-    std::vector<__nv_bfloat16> w((size_t)n_pad * k_pad, __float2bfloat16(0.f));
-    long long nnz = 0; int n_real = 0;
-    for (int n = 0; n < n_out; n++) {
-        bool row = bias != nullptr && bias[n] != 0.f;
-        for (int k = 0; k < channels; k++) {
-            const float v = weight[(size_t)n * channels + k];
-            w[(size_t)n * k_pad + k] = __float2bfloat16(v);
-            if (v != 0.f) { nnz++; row = true; }
-        }
-        n_real += row ? 1 : 0;
-    }
-    std::vector<float> b(n_pad, 0.f);
-    for (int n = 0; n < n_out; n++) b[n] = bias ? bias[n] : 0.f;
-    __nv_bfloat16* d_w = nullptr; float* d_b = nullptr;
-    rc = net_upload(net, &d_w, w); if (rc != PIFPAF_OK) return rc;
-    rc = net_upload(net, &d_b, b); if (rc != PIFPAF_OK) return rc;
-    // scatter table
-    std::vector<DestGroup> groups((size_t)n_pad / 16, DestGroup{nullptr, 0, 0});
-    int expect = 0;
-    for (int i = 0; i < n_pieces; i++) {
-        PIFPAF_CHECK_ARG(piece_col0[i] == expect && piece_count[i] >= 16 && piece_count[i] % 16 == 0,
-                         "pieces must tile [0, n_out) in order, in multiples of 16 columns");
-        PIFPAF_CHECK_ARG(piece_tensor[i] >= 0 && piece_tensor[i] < nt, "bad piece tensor id");
-        const Tensor& to = net->tensors[piece_tensor[i]];
-        PIFPAF_CHECK_ARG(to.h == tin.h && to.w == tin.w, "stride 1 keeps the spatial shape");
-        PIFPAF_CHECK_ARG(piece_tensor_col[i] >= 0 && piece_tensor_col[i] % 16 == 0 &&
-                         piece_tensor_col[i] + piece_count[i] <= to.c, "piece window outside its tensor");
-        for (int c = 0; c < piece_count[i]; c += 16)
-            groups[(size_t)(expect + c) / 16] = DestGroup{to.data + piece_tensor_col[i] + c, to.c, 0};
-        expect += piece_count[i];
-    }
-    PIFPAF_CHECK_ARG(expect == n_out, "pieces must cover all n_out columns");
-    DestGroup* d_groups = nullptr;
-    rc = net_upload(net, &d_groups, groups); if (rc != PIFPAF_OK) return rc;
+    // 1x1 weights [n_out][channels] -> bf16 [n_pad][C]
+    GemmWeights gw;
+    rc = upload_gemm_weights(net, weight, bias, n_out, channels, 1, C, n_pad, &gw);
+    if (rc != PIFPAF_OK) return rc;
+    std::vector<int> map_tensor;      // k_dw_gemm has the per-lane scatter epilogue only: no store maps
+    rc = upload_dest_groups(net, n_pad, n_out, tin.h, tin.w, n_pieces, piece_col0, piece_count, piece_tensor,
+                            piece_tensor_col, &op.g.dest, &map_tensor);
+    if (rc != PIFPAF_OK) return rc;
 
     GemmArgs& g = op.g;
     g.N = n_out; g.K = C; g.block_n = block_n; g.n_blocks = n_blocks;
     g.num_k_blocks = (C + BK - 1) / BK;
-    g.bias = d_b; g.mode = MODE_SCATTER; g.relu = relu; g.dest = d_groups;
+    g.bias = gw.bias; g.mode = MODE_SCATTER; g.relu = relu;
     g.conv_k = kernel; g.conv_stride = stride; g.conv_pad = pad; g.conv_dil = 1; g.conv_cblocks = g.num_k_blocks;
     g.Hi = tin.h; g.Wi = tin.w; g.Ho = tin.h; g.Wo = tin.w;
     g.tiles_x = (g.Wo + PW - 1) / PW; g.tiles_y = (g.Ho + PH - 1) / PH;
@@ -2690,15 +2653,15 @@ int pifpaf_net_dw_conv1x1_scatter(pifpaf_net_t* net, int32_t in_tensor, int32_t 
     }
     PIFPAF_CHECK_ARG(fits, "fused depthwise -> 1x1 op does not fit in shared memory");
     op.smem = fused_smem_bytes(f.ws, f.bs, block_n, n_pad, C);
-    op.n_real = n_real;
-    op.flops_per_image = 2.0 * (double)op.rows_per_image * ((double)nnz + 25.0 * channels);
-    op.bytes_per_image = (double)op.rows_per_image * (channels + n_real) * 2.0;     // dw input once + 1x1 output once
-    op.weight_bytes = (double)nnz * 2.0 + 25.0 * channels * 4.0;
+    op.n_real = gw.n_real;
+    op.flops_per_image = 2.0 * (double)op.rows_per_image * ((double)gw.nnz + 25.0 * channels);
+    op.bytes_per_image = (double)op.rows_per_image * (channels + gw.n_real) * 2.0;     // dw input once + 1x1 output once
+    op.weight_bytes = (double)gw.nnz * 2.0 + 25.0 * channels * 4.0;
     using T = DwTile<1, PH, PW, 4, 1>;
     rc = make_tmap_dw(&op.tmap_dw, tin.data + in_col_off, (uint64_t)C, (uint64_t)tin.w, (uint64_t)tin.h,
                       (uint64_t)net->max_batch, (uint64_t)tin.c, T::IW, T::IH);
     if (rc != PIFPAF_OK) return rc;
-    rc = make_tmap(&op.tmap_b, d_w, (uint64_t)n_pad, (uint64_t)k_pad, (uint64_t)k_pad, (uint32_t)block_n);
+    rc = make_tmap(&op.tmap_b, gw.w, (uint64_t)n_pad, (uint64_t)C, (uint64_t)C, (uint32_t)block_n);
     if (rc != PIFPAF_OK) return rc;
     op.touches.assign(piece_tensor, piece_tensor + n_pieces);
     op.touches.push_back(in_tensor);
@@ -2755,6 +2718,7 @@ int pifpaf_net_heads_upsampled(pifpaf_net_t* net, int32_t in_tensor, int32_t k_c
     g.head_cols = d_cols;
     g.hw = tin.h * tin.w; g.w = tin.w;
     g.up = up; g.up_low = low; g.out_h = out_h; g.out_w = out_w;
+    plan_gemm_smem(op);
     net->n_heads = n_heads; net->head_h = out_h; net->head_w = out_w;
     op.touches = {in_tensor};
     net->ops.push_back(op);
@@ -2814,14 +2778,9 @@ static int net_forward_impl(pifpaf_net_t* net, const float* images_dev, int32_t 
             if (u8 != nullptr) {
                 a.in_u8 = u8->images;
                 for (int c = 0; c < 3; c++) { a.mean[c] = u8->mean[c]; a.stdev[c] = u8->stdev[c]; }
-                if (a.kernel == 3) k_input_conv<3, true><<<grid, 256, smem, st>>>(a);
-                else if (a.kernel == 7) k_input_conv<7, true><<<grid, 256, smem, st>>>(a);
-                else if (a.kernel == 5) k_input_conv<5, true><<<grid, 256, smem, st>>>(a);
-                else k_input_conv<1, true><<<grid, 256, smem, st>>>(a);
-            } else if (a.kernel == 3) k_input_conv<3, false><<<grid, 256, smem, st>>>(a);
-            else if (a.kernel == 7) k_input_conv<7, false><<<grid, 256, smem, st>>>(a);
-            else if (a.kernel == 5) k_input_conv<5, false><<<grid, 256, smem, st>>>(a);
-            else k_input_conv<1, false><<<grid, 256, smem, st>>>(a);
+            }
+            InConvKernel kern = INPUT_CONV_KERNELS[u8 != nullptr][a.kernel / 2];
+            kern<<<grid, 256, smem, st>>>(a);
             PIFPAF_LAUNCH_CHECK();
         } else if (op.kind == OP_FUSED) {
             PIFPAF_CHECK_ARG(gemm_impl == 0, "the fused depthwise -> 1x1 op has no SIMT debug variant (compile the net with fuse_dw=False)");
@@ -2842,41 +2801,19 @@ static int net_forward_impl(pifpaf_net_t* net, const float* images_dev, int32_t 
                 const int grid = (int)std::min<long long>(total, (long long)n_sm);     // 1 CTA per SM by shared memory
                 PIFPAF_CUDA_TRY(launch_k(pdl, k_pw_dw<2, PWDW_TH, PWDW_TW, PWDW_BW>, dim3(grid), dim3(PwDwS2::THREADS),
                                          op.pw_smem, st, op.tmap_pw, p));
-            } else if (op.dw_tma && gemm_impl == 0 && a.kernel == 3) {
-                const int cblks = (a.C8 + 7) / 8;
-                const int th = a.stride == 1 ? DW1_TH : DW2_TH, tw = a.stride == 1 ? DW1_TW : DW2_TW;
-                const long long total = (long long)batch * ((a.Hout + th - 1) / th) * ((a.Wout + tw - 1) / tw) * cblks;
-                // persistent grid == resident CTAs (stride 1: 2 per SM, stride 2: 1 per SM by shared memory)
-                if (a.stride == 1)
-                    PIFPAF_CUDA_TRY(launch_k(pdl, k_dwconv5_tma<1, DW1_TH, DW1_TW, 4, 4, false, 3>,
-                                             dim3((int)std::min<long long>(total, (long long)n_sm * 2)),
-                                             dim3(DwS1K3::THREADS), (size_t)DwS1K3::SMEM, st, op.tmap_dw, a));
-                else
-                    PIFPAF_CUDA_TRY(launch_k(pdl, k_dwconv5_tma<2, DW2_TH, DW2_TW, 4, 3, false, 3>,
-                                             dim3((int)std::min<long long>(total, (long long)n_sm)),
-                                             dim3(DwS2K3::THREADS), (size_t)DwS2K3::SMEM, st, op.tmap_dw, a));
             } else if (op.dw_tma && gemm_impl == 0) {
+                const DwTmaVariant* v = op.dw_tma;
                 const int cblks = (a.C8 + 7) / 8;
-                // persistent grid == resident CTAs (stride 1: 2 per SM, stride 2: 1 per SM by shared memory)
-                if (a.stride == 1) {
-                    const long long total = (long long)batch * ((a.Hout + DW1_TH - 1) / DW1_TH) *
-                                            ((a.Wout + DW1_TW - 1) / DW1_TW) * cblks;
-                    const int grid = (int)std::min<long long>(total, (long long)n_sm * 2);
-                    PIFPAF_CUDA_TRY(launch_k(pdl, k_dwconv5_tma<1, DW1_TH, DW1_TW, 4, 3, false>, dim3(grid), dim3(DwS1::THREADS),
-                                             (size_t)DwS1::SMEM, st, op.tmap_dw, a));
-                } else {
-                    const long long total = (long long)batch * ((a.Hout + DW2_TH - 1) / DW2_TH) *
-                                            ((a.Wout + DW2_TW - 1) / DW2_TW) * cblks;
-                    const int grid = (int)std::min<long long>(total, (long long)n_sm);
-                    // channel-block-fastest order with the weights staged in shared memory while they fit
-                    const size_t smem_cf = (size_t)DwS2::SMEM + (size_t)26 * a.C8 * 8 * sizeof(float);
-                    if (net->dw_cbf && cblks > 1 && smem_cf <= 226 * 1024)
-                        PIFPAF_CUDA_TRY(launch_k(pdl, k_dwconv5_tma<2, DW2_TH, DW2_TW, 4, 2, true>, dim3(grid), dim3(DwS2::THREADS),
-                                                 smem_cf, st, op.tmap_dw, a));
-                    else
-                        PIFPAF_CUDA_TRY(launch_k(pdl, k_dwconv5_tma<2, DW2_TH, DW2_TW, 4, 2, false>, dim3(grid), dim3(DwS2::THREADS),
-                                                 (size_t)DwS2::SMEM, st, op.tmap_dw, a));
+                const long long total = (long long)batch * ((a.Hout + v->th - 1) / v->th) * ((a.Wout + v->tw - 1) / v->tw) * cblks;
+                const int grid = (int)std::min<long long>(total, (long long)n_sm * v->ctas_per_sm);
+                size_t smem = v->smem;
+                // channel-block-fastest order with the weights staged in shared memory while they fit
+                const size_t smem_cf = smem + (size_t)26 * a.C8 * 8 * sizeof(float);
+                if (v == &DW_TMA[DW_K5_S2] && net->dw_cbf && cblks > 1 && smem_cf <= (size_t)DW_TMA[DW_K5_S2_CBF].smem) {
+                    v = &DW_TMA[DW_K5_S2_CBF];
+                    smem = smem_cf;
                 }
+                PIFPAF_CUDA_TRY(launch_k(pdl, v->kernel, dim3(grid), dim3(v->threads), smem, st, op.tmap_dw, a));
             } else if (a.kernel == 5 && (a.stride == 1 || a.stride == 2)) {
                 const long long total = (long long)batch * ((a.Hout + DW_OY - 1) / DW_OY) * DW_OY *
                                         ((a.Wout + DW_OX - 1) / DW_OX) * a.C8;

@@ -357,6 +357,7 @@ def test_conv_matches_float64(c, impl):
 # (H, W, kernel, stride, pad, c_out, u8, batch, max_batch)
 STEM_CASES = [
     (17, 19, 1, 1, 0, 8, False, 1, 2),
+    (17, 19, 1, 1, 0, 8, True, 1, 2),
     (33, 31, 3, 2, 1, 24, False, 2, 3),
     (33, 31, 3, 2, 1, 24, True, 2, 3),
     (21, 25, 5, 1, 2, 64, False, 1, 2),
