@@ -321,6 +321,17 @@ int pifpaf_net_dwconv(pifpaf_net_t* net, int32_t in_tensor, int32_t in_col_off, 
                       int32_t kernel, int32_t stride, int32_t pad, const float* weight, const float* bias,
                       int32_t relu, int32_t out_tensor, int32_t out_col_off);
 
+/* pifpaf_net_dwconv with dilated taps (ShuffleNetV2K stage 4 and conv5-as-stage under
+ * --shufflenetv2k-stage4-dilation, basenetworks.py:186-231,297-334): tap (ky, kx) reads input pixel
+ * (x - pad + kx * dilation, y - pad + ky * dilation); the output is (H + 2 * pad - dilation * (kernel - 1) - 1) / stride
+ * + 1 pixels high (likewise wide).  dilation < 1, and dilation > 1 with stride 2, are PIFPAF_E_ARG (the reference
+ * pairs dilation with stride 1).  5x5 with dilation 2 and no ReLU6 runs the TMA-fed kernel; every other dilated shape,
+ * and gemm_impl = 1, the generic one.  A dilated op is never fused with a neighbouring 1x1 conv.
+ * pifpaf_net_dwconv is this entry point with dilation 1. */
+int pifpaf_net_dwconv_dilated(pifpaf_net_t* net, int32_t in_tensor, int32_t in_col_off, int32_t channels,
+                              int32_t kernel, int32_t stride, int32_t pad, const float* weight, const float* bias,
+                              int32_t relu, int32_t out_tensor, int32_t out_col_off, int32_t dilation);
+
 /* Depthwise 5x5 (stride 1) -> BatchNorm -> 1x1 conv -> BatchNorm -> ReLU, the tail of InvertedResidualK.branch2
  * (basenetworks.py:219-226), as ONE kernel: the depthwise result is produced tile by tile straight into the
  * shared-memory A operand of the wgmma GEMM and never visits HBM.  Arguments: those of pifpaf_net_dwconv

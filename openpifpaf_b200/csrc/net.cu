@@ -865,9 +865,9 @@ __global__ void __launch_bounds__(256) k_dwconv5(DwArgs a) {
     }
 }
 
-// Depthwise KS x KS (5x5: ShuffleNetV2K; 3x3: MobileNetV2) with TMA-staged input tiles.  A persistent CTA walks
-// (channel block, image, tile) work items; the input window of an item ((TH-1)*S+KS x (TW-1)*S+KS pixels x 64
-// channels, 4-D tensor map, out-of-bounds zero fill
+// Depthwise KS x KS (5x5: ShuffleNetV2K, also with taps D = 2 pixels apart; 3x3: MobileNetV2) with TMA-staged input
+// tiles.  A persistent CTA walks (channel block, image, tile) work items; the input window of an item
+// ((TH-1)*S+(KS-1)*D+1 x (TW-1)*S+(KS-1)*D+1 pixels x 64 channels, 4-D tensor map, out-of-bounds zero fill
 // == the conv padding) is streamed by TMA into an NSTAGE-deep shared-memory ring.  There is no CTA-wide barrier in
 // the steady state: every warp counts itself out of a ring slot with one shared-memory atomic, and the warp that
 // finishes a slot LAST re-arms it with the TMA of the item NSTAGE rounds ahead, so fast warps (edge tiles with
@@ -876,14 +876,14 @@ __global__ void __launch_bounds__(256) k_dwconv5(DwArgs a) {
 // one lane = one channel pair.  The lane keeps its KS*KS x 2 weights and a 4 x BW x 2 f32 accumulator in registers and
 // reads every input pixel of the block's window exactly once (4 bytes per lane, 128 bytes per warp request: one
 // conflict-free wavefront).
-template <int S, int TH, int TW, int BW, int NSTAGE, int KS = 5>
+template <int S, int TH, int TW, int BW, int NSTAGE, int KS = 5, int D = 1>
 struct DwTile {
-    static constexpr int IH = (TH - 1) * S + KS, IW = (TW - 1) * S + KS;
+    static constexpr int IH = (TH - 1) * S + (KS - 1) * D + 1, IW = (TW - 1) * S + (KS - 1) * D + 1;
     static constexpr int BYTES = IH * IW * 64 * 2;
     static constexpr int WARPS = (TH / 4) * (TW / BW);
     static constexpr int THREADS = WARPS * 32;
-    static constexpr int WIN_Y = 3 * S + KS;           // input window of a 4 x BW output block
-    static constexpr int WIN_X = (BW - 1) * S + KS;
+    static constexpr int WIN_Y = 3 * S + (KS - 1) * D + 1;           // input window of a 4 x BW output block
+    static constexpr int WIN_X = (BW - 1) * S + (KS - 1) * D + 1;
     static constexpr int SMEM = NSTAGE * BYTES + 128;
 };
 
@@ -924,18 +924,19 @@ __device__ __forceinline__ void dw_advance_cf(DwPos& p, const DwPos& d, int cblk
     p.b += d.b + carry;
 }
 
-// One warp's share of a depthwise KS x KS item (KS = 5 or 3): the 4 x BW output pixels at (oy0, ox0) of image b,
-// lane = the channel pair c0, c0 + 1; bias initialises the f32 sums, the KS * KS taps run in (ky, kx) order (the
-// order of k_dwconv, so the 3x3 results equal its bit for bit), activation a.relu, bf16 stores.
+// One warp's share of a depthwise KS x KS item (KS = 5 or 3; taps D pixels apart): the 4 x BW output pixels at
+// (oy0, ox0) of image b, lane = the channel pair c0, c0 + 1; bias initialises the f32 sums, the KS * KS taps run in
+// (ky, kx) order (the order of k_dwconv, so the 3x3 and dilated results equal its bit for bit), activation a.relu,
+// bf16 stores.  Tap (ky, kx) of output (i, j) reads window row i * S + ky * D, column j * S + kx * D.
 // win: the item's input window in shared memory, IW pixels per row, 128 bytes (64 channels) per pixel; p0: the
 // window pixel at the block's first tap.  SWZ: the 16-byte units of pixel p sit at unit ^ (p & 7) (k_pw_dw's
 // intermediate window, which its wgmma epilogue writes without bank conflicts that way); the eight possible units
 // are resolved once per block, so the loads need no address arithmetic.
-template <int S, int BW, int IW, bool SWZ, int KS = 5>
+template <int S, int BW, int IW, bool SWZ, int KS = 5, int D = 1>
 __device__ __forceinline__ void dw5_block(const DwArgs& a, const unsigned char* win, int p0, int lane,
                                           const float (&wgt)[KS * KS][2], float bias0, float bias1, int b, int oy0,
                                           int ox0, int c0) {
-    constexpr int WIN_Y = 3 * S + KS, WIN_X = (BW - 1) * S + KS;
+    constexpr int WIN_Y = 3 * S + (KS - 1) * D + 1, WIN_X = (BW - 1) * S + (KS - 1) * D + 1;
     const unsigned char* tile = win + p0 * 128 + (SWZ ? (lane & 3) * 4 : lane * 4);
     const unsigned char* rows[SWZ ? 8 : 1];          // SWZ: the lane's word in a pixel p with p & 7 == c
 #pragma unroll
@@ -957,14 +958,15 @@ __device__ __forceinline__ void dw5_block(const DwArgs& a, const unsigned char* 
         }
 #pragma unroll
         for (int i = 0; i < 4; i++) {
-            const int ky = ry - i * S;                    // compile-time after unrolling
-            if (ky < 0 || ky >= KS) continue;
+            const int dy = ry - i * S;                    // compile-time after unrolling
+            if (dy < 0 || dy % D != 0 || dy / D >= KS) continue;
+            const int ky = dy / D;
 #pragma unroll
             for (int kx = 0; kx < KS; kx++) {
 #pragma unroll
                 for (int j = 0; j < BW; j++) {
-                    acc[i][j][0] = fmaf(f[j * S + kx][0], wgt[ky * KS + kx][0], acc[i][j][0]);
-                    acc[i][j][1] = fmaf(f[j * S + kx][1], wgt[ky * KS + kx][1], acc[i][j][1]);
+                    acc[i][j][0] = fmaf(f[j * S + kx * D][0], wgt[ky * KS + kx][0], acc[i][j][0]);
+                    acc[i][j][1] = fmaf(f[j * S + kx * D][1], wgt[ky * KS + kx][1], acc[i][j][1]);
                 }
             }
         }
@@ -1014,10 +1016,10 @@ __device__ __forceinline__ void dw5_block(const DwArgs& a, const unsigned char* 
     }
 }
 
-template <int S, int TH, int TW, int BW, int NSTAGE, bool CBF = false, int KS = 5>
-__global__ void __launch_bounds__(DwTile<S, TH, TW, BW, NSTAGE, KS>::THREADS, 2)
+template <int S, int TH, int TW, int BW, int NSTAGE, bool CBF = false, int KS = 5, int D = 1>
+__global__ void __launch_bounds__(DwTile<S, TH, TW, BW, NSTAGE, KS, D>::THREADS, 2)
 k_dwconv5_tma(const __grid_constant__ CUtensorMap tmap_in, DwArgs a) {
-    using T = DwTile<S, TH, TW, BW, NSTAGE, KS>;
+    using T = DwTile<S, TH, TW, BW, NSTAGE, KS, D>;
     constexpr int TAPS = KS * KS;
     extern __shared__ __align__(128) unsigned char dsm_raw[];
     // align inside the shared window with pointer arithmetic on the array itself (keeps the address space known to
@@ -1095,7 +1097,7 @@ k_dwconv5_tma(const __grid_constant__ CUtensorMap tmap_in, DwArgs a) {
         // warps counted out of the slot's previous item, so the per-slot count never mixes two items
         mbar_wait(&full[buf], phase);
         if (oy0 < a.Hout && ox0 < a.Wout && c0 < C)
-            dw5_block<S, BW, T::IW, false, KS>(a, dsm + (size_t)buf * T::BYTES, (by * 4 * S) * T::IW + bx * BW * S,
+            dw5_block<S, BW, T::IW, false, KS, D>(a, dsm + (size_t)buf * T::BYTES, (by * 4 * S) * T::IW + bx * BW * S,
                                                lane, wgt, bias0, bias1, pos.b, oy0, ox0, c0);
         // count this warp out of the slot; the last one out re-arms it.  Every shared-memory read of the slot has
         // been consumed by an fma above (results are in registers), the fence orders them before the count.
@@ -1122,8 +1124,12 @@ k_dwconv5_tma(const __grid_constant__ CUtensorMap tmap_in, DwArgs a) {
 //              against 1.41x for 8x8)
 // 3x3: the same tiles and blocks; the smaller windows buy one more ring slot at the same bytes in flight per SM:
 //              stride 1 -> 23 KB window, 4-deep ring, 2 CTAs per SM; stride 2 -> 72 KB window, 3-deep ring, 1 CTA per SM
+// 5x5 with dilation 2 (stride 1; ShuffleNetV2K stage 4 under --shufflenetv2k-stage4-dilation 2): the stride-1 tile
+//              and blocks with a 16 x 24 pixel window (48 KB; a 12 x 12 window per 4 x 4 block); 2-deep ring, 2 CTAs
+//              per SM (192 KB of windows per SM, 16 warps as DwS1).  A 3-deep ring would leave one CTA per SM.
 constexpr int DW1_TH = 8, DW1_TW = 16, DW2_TH = 8, DW2_TW = 16;
 using DwS1 = DwTile<1, DW1_TH, DW1_TW, 4, 3>;
+using DwS1D2 = DwTile<1, DW1_TH, DW1_TW, 4, 2, 5, 2>;
 using DwS2 = DwTile<2, DW2_TH, DW2_TW, 4, 2>;
 using DwS1K3 = DwTile<1, DW1_TH, DW1_TW, 4, 4, 3>;
 using DwS2K3 = DwTile<2, DW2_TH, DW2_TW, 4, 3, 3>;
@@ -1164,8 +1170,10 @@ __global__ void __launch_bounds__(256) k_maxpool(DwArgs a) {
     }
 }
 
-// generic depthwise kxk (any kernel/stride): one output pixel x 8 channels per thread
-__global__ void __launch_bounds__(256) k_dwconv(DwArgs a) {
+// generic depthwise kxk (any kernel / stride / dilation): one output pixel x 8 channels per thread.  The dilation is
+// a parameter of its own: a DwArgs field would move the layout of PwDwArgs (which embeds DwArgs) and with it the
+// register allocation of k_pw_dw
+__global__ void __launch_bounds__(256) k_dwconv(DwArgs a, int dil) {
     const long long total = (long long)a.B * a.Hout * a.Wout * a.C8;
     const int C = a.C8 * 8;
     for (long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x; t < total;
@@ -1181,10 +1189,10 @@ __global__ void __launch_bounds__(256) k_dwconv(DwArgs a) {
         acc[0] = b0.x; acc[1] = b0.y; acc[2] = b0.z; acc[3] = b0.w;
         acc[4] = b1.x; acc[5] = b1.y; acc[6] = b1.z; acc[7] = b1.w;
         for (int ky = 0; ky < a.kernel; ky++) {
-            const int iy = oy * a.stride - a.pad + ky;
+            const int iy = oy * a.stride - a.pad + ky * dil;
             if (iy < 0 || iy >= a.Hin) continue;
             for (int kx = 0; kx < a.kernel; kx++) {
-                const int ix = ox * a.stride - a.pad + kx;
+                const int ix = ox * a.stride - a.pad + kx * dil;
                 if (ix < 0 || ix >= a.Win) continue;
                 const uint4 v = __ldg(reinterpret_cast<const uint4*>(
                     a.in + ((size_t)(b * a.Hin + iy) * a.Win + ix) * a.ld_in + a.in_col_off + c8 * 8));
@@ -1853,7 +1861,7 @@ struct DwTmaVariant {
     int ctas_per_sm;          // persistent grid == resident CTAs (by shared memory)
     uint32_t box_w, box_h;    // input window (TMA box)
 };
-enum { DW_K5_S1, DW_K5_S2, DW_K5_S2_CBF, DW_K3_S1, DW_K3_S2, DW_TMA_VARIANTS };
+enum { DW_K5_S1, DW_K5_S2, DW_K5_S2_CBF, DW_K3_S1, DW_K3_S2, DW_K5_S1_D2, DW_TMA_VARIANTS };
 const DwTmaVariant DW_TMA[DW_TMA_VARIANTS] = {
     {k_dwconv5_tma<1, DW1_TH, DW1_TW, 4, 3>, DwS1::THREADS, DwS1::SMEM, DW1_TH, DW1_TW, 2, DwS1::IW, DwS1::IH},
     {k_dwconv5_tma<2, DW2_TH, DW2_TW, 4, 2>, DwS2::THREADS, DwS2::SMEM, DW2_TH, DW2_TW, 1, DwS2::IW, DwS2::IH},
@@ -1863,7 +1871,9 @@ const DwTmaVariant DW_TMA[DW_TMA_VARIANTS] = {
     {k_dwconv5_tma<1, DW1_TH, DW1_TW, 4, 4, false, 3>, DwS1K3::THREADS, DwS1K3::SMEM, DW1_TH, DW1_TW, 2, DwS1K3::IW,
      DwS1K3::IH},
     {k_dwconv5_tma<2, DW2_TH, DW2_TW, 4, 3, false, 3>, DwS2K3::THREADS, DwS2K3::SMEM, DW2_TH, DW2_TW, 1, DwS2K3::IW,
-     DwS2K3::IH}};
+     DwS2K3::IH},
+    {k_dwconv5_tma<1, DW1_TH, DW1_TW, 4, 2, false, 5, 2>, DwS1D2::THREADS, DwS1D2::SMEM, DW1_TH, DW1_TW, 2, DwS1D2::IW,
+     DwS1D2::IH}};
 
 // the stem instantiations, indexed [U8][KS / 2] (KS = 1, 3, 5, 7)
 using InConvKernel = decltype(&k_input_conv<1, false>);
@@ -1892,6 +1902,7 @@ struct Op {
     DwArgs dw{};
     CUtensorMap tmap_dw{};
     const DwTmaVariant* dw_tma = nullptr;     // the TMA kernel of a depthwise op (nullptr: k_dwconv5 / k_dwconv)
+    int dw_dil = 1;                           // depthwise tap spacing (> 1: DW_K5_S1_D2 or k_dwconv)
     // fused depthwise -> GEMM (OP_FUSED): g + tmap_dw (windows) + tmap_b
     FusedArgs fu{};
     // input conv
@@ -2535,13 +2546,24 @@ int pifpaf_net_conv_dilated(pifpaf_net_t* net, int32_t in_tensor, int32_t in_col
 int pifpaf_net_dwconv(pifpaf_net_t* net, int32_t in_tensor, int32_t in_col_off, int32_t channels,
                       int32_t kernel, int32_t stride, int32_t pad, const float* weight, const float* bias,
                       int32_t relu, int32_t out_tensor, int32_t out_col_off) {
+    return pifpaf_net_dwconv_dilated(net, in_tensor, in_col_off, channels, kernel, stride, pad, weight, bias, relu,
+                                     out_tensor, out_col_off, 1);
+}
+
+int pifpaf_net_dwconv_dilated(pifpaf_net_t* net, int32_t in_tensor, int32_t in_col_off, int32_t channels,
+                              int32_t kernel, int32_t stride, int32_t pad, const float* weight, const float* bias,
+                              int32_t relu, int32_t out_tensor, int32_t out_col_off, int32_t dilation) {
     PIFPAF_CHECK_ARG(net != nullptr && weight != nullptr, "null argument");
     const int nt = (int)net->tensors.size();
     PIFPAF_CHECK_ARG(in_tensor >= 0 && in_tensor < nt && out_tensor >= 0 && out_tensor < nt, "bad tensor id");
     PIFPAF_CHECK_ARG(relu >= ACT_NONE && relu <= ACT_RELU6, "activation code must be 0 (none), 1 (ReLU) or 2 (ReLU6)");
+    PIFPAF_CHECK_ARG(dilation >= 1, "dwconv dilation must be at least 1");
+    // the reference pairs dilation with stride 1 (basenetworks.py:297-306); the tiled kernels assume it
+    PIFPAF_CHECK_ARG(dilation == 1 || stride == 1, "a dilated dwconv (dilation > 1) must have stride 1");
     const Tensor& tin = net->tensors[in_tensor];
     const Tensor& to = net->tensors[out_tensor];
-    const int ho = (tin.h + 2 * pad - kernel) / stride + 1, wo = (tin.w + 2 * pad - kernel) / stride + 1;
+    const int span = dilation * (kernel - 1) + 1;
+    const int ho = (tin.h + 2 * pad - span) / stride + 1, wo = (tin.w + 2 * pad - span) / stride + 1;
     const int C = pad8(channels);
     PIFPAF_CHECK_ARG(to.h == ho && to.w == wo, "dwconv output tensor shape mismatch");
     PIFPAF_CHECK_ARG(in_col_off % 8 == 0 && out_col_off % 8 == 0 && in_col_off + C <= tin.c && out_col_off + C <= to.c,
@@ -2557,10 +2579,15 @@ int pifpaf_net_dwconv(pifpaf_net_t* net, int32_t in_tensor, int32_t in_col_off, 
     a.weight = d_w; a.bias = d_b;
     a.Hin = tin.h; a.Win = tin.w; a.Hout = ho; a.Wout = wo; a.C8 = C / 8;
     a.kernel = kernel; a.stride = stride; a.pad = pad; a.relu = relu;
+    op.dw_dil = dilation;
     op.flops_per_image = 2.0 * ho * wo * channels * (double)kernel * kernel;
     op.bytes_per_image = ((double)tin.h * tin.w + (double)ho * wo) * channels * 2.0;
-    if ((kernel == 3 || (kernel == 5 && relu != ACT_RELU6)) && (stride == 1 || stride == 2)) {
+    if (dilation == 2 && kernel == 5 && stride == 1 && relu != ACT_RELU6) {
+        op.dw_tma = &DW_TMA[DW_K5_S1_D2];
+    } else if (dilation == 1 && (kernel == 3 || (kernel == 5 && relu != ACT_RELU6)) && (stride == 1 || stride == 2)) {
         op.dw_tma = &DW_TMA[kernel == 3 ? (stride == 1 ? DW_K3_S1 : DW_K3_S2) : (stride == 1 ? DW_K5_S1 : DW_K5_S2)];
+    }
+    if (op.dw_tma) {
         rc = make_tmap_dw(&op.tmap_dw, tin.data + in_col_off, (uint64_t)C, (uint64_t)tin.w, (uint64_t)tin.h,
                           (uint64_t)net->max_batch, (uint64_t)tin.c, op.dw_tma->box_w, op.dw_tma->box_h);
         if (rc != PIFPAF_OK) return rc;
@@ -2814,7 +2841,7 @@ static int net_forward_impl(pifpaf_net_t* net, const float* images_dev, int32_t 
                     smem = smem_cf;
                 }
                 PIFPAF_CUDA_TRY(launch_k(pdl, v->kernel, dim3(grid), dim3(v->threads), smem, st, op.tmap_dw, a));
-            } else if (a.kernel == 5 && (a.stride == 1 || a.stride == 2)) {
+            } else if (a.kernel == 5 && op.dw_dil == 1 && (a.stride == 1 || a.stride == 2)) {
                 const long long total = (long long)batch * ((a.Hout + DW_OY - 1) / DW_OY) * DW_OY *
                                         ((a.Wout + DW_OX - 1) / DW_OX) * a.C8;
                 const int grid = (int)std::min<long long>((total + 255) / 256, (long long)n_sm * 64);
@@ -2823,7 +2850,7 @@ static int net_forward_impl(pifpaf_net_t* net, const float* images_dev, int32_t 
             } else {
                 const long long total = (long long)batch * a.Hout * a.Wout * a.C8;
                 const int grid = (int)std::min<long long>((total + 255) / 256, (long long)n_sm * 32);
-                k_dwconv<<<grid, 256, 0, st>>>(a);
+                k_dwconv<<<grid, 256, 0, st>>>(a, op.dw_dil);
             }
             PIFPAF_LAUNCH_CHECK();
         } else if (op.kind == OP_MAXPOOL) {

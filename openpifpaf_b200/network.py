@@ -253,33 +253,55 @@ def plan_from_shell(shell):
     if not all(hasattr(base, a) for a in ('input_block', 'stage2', 'stage3', 'stage4', 'conv5')):
         raise UnsupportedModel(f'unsupported base network {type(base).__name__}: expected ShuffleNetV2K, Resnet or '
                                'MobileNetV2')
-    if len(base.input_block) != 1:
-        raise UnsupportedModel('input_conv2 variants are not supported')
+    return _plan_from_shufflenetv2k(shell)
+
+
+def _shufflenetv2k_block(blk):
+    """one InvertedResidualK (basenetworks.py:186-242), folded; 'dilation' only where it is not 1
+    (--shufflenetv2k-stage4-dilation, which the reference pairs with stride 1)"""
+    b2 = blk.branch2
+    dw = b2[3]
+    entry = {'first': blk.branch1 is not None, 'stride': int(dw.stride[0]),
+             'kernel': int(dw.kernel_size[0]), 'pad': int(dw.padding[0])}
+    if dw.dilation[0] != 1:
+        if entry['stride'] != 1:
+            raise UnsupportedModel('dilated depthwise convolutions with a stride are not supported')
+        entry['dilation'] = int(dw.dilation[0])
+    entry['b2_pw1'] = _fold(b2[0], b2[1])
+    entry['b2_dw'] = _fold(b2[3], b2[4])
+    entry['b2_pw2'] = _fold(b2[5], b2[6])
+    if blk.branch1 is not None:
+        entry['b1_dw'] = _fold(blk.branch1[0], blk.branch1[1])
+        entry['b1_pw'] = _fold(blk.branch1[2], blk.branch1[3])
+    return entry
+
+
+def _plan_from_shufflenetv2k(shell):
+    """basenetworks.py:245-355: the stem (and the second 3x3 stride-2 conv of --shufflenetv2k-input-conv2-stride as
+    plan['input2']), stages 2-4 (stage 4 at stride 1 with dilated depthwise convs under
+    --shufflenetv2k-stage4-dilation) and conv5: a 1x1 conv (plan['conv5']) or, under --shufflenetv2k-conv5-as-stage,
+    two more InvertedResidualK blocks (plan['conv5_stage'])."""
+    base = shell.base_net
+    if len(base.input_block) not in (1, 2):
+        raise UnsupportedModel(f'unsupported ShuffleNetV2K input block of {len(base.input_block)} convolutions')
     conv, bn = base.input_block[0][0], base.input_block[0][1]
     w, b = _fold(conv, bn)
     plan = {'kind': 'shufflenetv2k',
             'input': {'w': w, 'b': b, 'stride': int(conv.stride[0]), 'pad': int(conv.padding[0])},
             'stages': [], 'heads': []}
+    if len(base.input_block) == 2:
+        conv, bn = base.input_block[1][0], base.input_block[1][1]
+        if _pair(conv.kernel_size) != (3, 3) or _pair(conv.stride) != (2, 2) or _pair(conv.padding) != (1, 1) or \
+                _pair(conv.dilation) != (1, 1) or conv.groups != 1:
+            raise UnsupportedModel(f'ShuffleNetV2K input_conv2: expected a 3x3 stride-2 conv, got {conv}')
+        w, b = _fold(conv, bn)
+        plan['input2'] = {'w': w, 'b': b, 'kernel': 3, 'stride': 2, 'pad': 1}
     for stage in (base.stage2, base.stage3, base.stage4):
-        blocks = []
-        for blk in stage:
-            b2 = blk.branch2
-            dw = b2[3]
-            if dw.dilation[0] != 1:
-                raise UnsupportedModel('dilated stages are not supported')
-            entry = {'first': blk.branch1 is not None, 'stride': int(dw.stride[0]),
-                     'kernel': int(dw.kernel_size[0]), 'pad': int(dw.padding[0])}
-            entry['b2_pw1'] = _fold(b2[0], b2[1])
-            entry['b2_dw'] = _fold(b2[3], b2[4])
-            entry['b2_pw2'] = _fold(b2[5], b2[6])
-            if blk.branch1 is not None:
-                entry['b1_dw'] = _fold(blk.branch1[0], blk.branch1[1])
-                entry['b1_pw'] = _fold(blk.branch1[2], blk.branch1[3])
-            blocks.append(entry)
-        plan['stages'].append(blocks)
-    if not isinstance(base.conv5[0], torch.nn.Conv2d):
-        raise UnsupportedModel('conv5_as_stage is not supported')
-    plan['conv5'] = _fold(base.conv5[0], base.conv5[1])
+        plan['stages'].append([_shufflenetv2k_block(blk) for blk in stage])
+    if isinstance(base.conv5[0], torch.nn.Conv2d):
+        plan['conv5'] = _fold(base.conv5[0], base.conv5[1])
+    else:
+        plan['conv5_stage'] = [_shufflenetv2k_block(blk) for blk in base.conv5]
     plan['heads'] = _heads_plan(shell, base)
     return plan
 
@@ -291,12 +313,16 @@ def heads_only_plan(plan, c_in=None):
     return {'kind': 'heads_only', 'c_in': c, 'heads': plan['heads']}
 
 
-def random_plan(base_name='shufflenetv2k16', heads=((17, 1, 1, 1), (19, 1, 2, 2)), seed=0, confidence_bias=-4.0):
+def random_plan(base_name='shufflenetv2k16', heads=((17, 1, 1, 1), (19, 1, 2, 2)), seed=0, confidence_bias=-4.0, *,
+                stage4_dilation=1, input_conv2_stride=0, input_conv2_outchannels=None, conv5_as_stage=False):
     """Random-init folded plan of the named architecture (no checkpoint can be downloaded here).
     heads: (n_fields, n_confidences, n_vectors, n_scales) per head; vector offsets all True.
     confidence_bias is added to the bias of the confidence channels so that a random-init head emits a
     sparse confidence map (sigmoid(-4) ~ 0.02) like a trained network's background; with a zero bias every
-    cell sits near 0.5 and passes every decoder threshold, which no trained model produces."""
+    cell sits near 0.5 and passes every decoder threshold, which no trained model produces.
+    The keyword options are the reference's --shufflenetv2k-stage4-dilation, --shufflenetv2k-input-conv2-stride,
+    --shufflenetv2k-input-conv2-outchannels and --shufflenetv2k-conv5-as-stage (basenetworks.py:245-334); the plan has
+    the layout `plan_from_shell` extracts from such a Shell."""
     repeats, ch = SHUFFLENETV2K_CONFIGS[base_name]
     rng = np.random.Generator(np.random.PCG64(seed))
 
@@ -306,32 +332,46 @@ def random_plan(base_name='shufflenetv2k16', heads=((17, 1, 1, 1), (19, 1, 2, 2)
         b = (rng.standard_normal(cout) * 0.05).astype(np.float32)
         return w, b
 
+    def block(cin, cout, first, stride, dil):
+        bf = cout // 2
+        e = {'first': first, 'stride': stride, 'kernel': 5, 'pad': 2 * dil}
+        if dil != 1:
+            e['dilation'] = dil
+        e['b2_pw1'] = conv(bf, cin if first else bf)
+        e['b2_dw'] = conv(bf, bf, 5, dw=True)
+        e['b2_pw2'] = conv(bf, bf)
+        if first:
+            e['b1_dw'] = conv(cin, cin, 5, dw=True)
+            e['b1_pw'] = conv(bf, cin)
+        return e
+
     w, b = conv(ch[0], 3, 3)
     plan = {'kind': 'shufflenetv2k', 'input': {'w': w, 'b': b, 'stride': 2, 'pad': 1}, 'stages': [], 'heads': []}
     cin = ch[0]
-    for rep, cout in zip(repeats, ch[1:4]):
-        bf = cout // 2
-        blocks = []
-        for i in range(rep):
-            first = i == 0
-            e = {'first': first, 'stride': 2 if first else 1, 'kernel': 5, 'pad': 2}
-            e['b2_pw1'] = conv(bf, cin if first else bf)
-            e['b2_dw'] = conv(bf, bf, 5, dw=True)
-            e['b2_pw2'] = conv(bf, bf)
-            if first:
-                e['b1_dw'] = conv(cin, cin, 5, dw=True)
-                e['b1_pw'] = conv(bf, cin)
-            blocks.append(e)
-        plan['stages'].append(blocks)
+    stride = 16                     # basenetworks.py:271-313
+    if input_conv2_stride:
+        c2 = input_conv2_outchannels or cin
+        w, b = conv(c2, cin, 3)
+        plan['input2'] = {'w': w, 'b': b, 'kernel': 3, 'stride': 2, 'pad': 1}
+        cin, stride = c2, stride * 2
+    for rep, cout, dil in zip(repeats, ch[1:4], (1, 1, stage4_dilation)):
+        if dil != 1:
+            stride //= 2
+        plan['stages'].append([block(cin if i == 0 else cout, cout, i == 0, 2 if i == 0 and dil == 1 else 1, dil)
+                               for i in range(rep)])
         cin = cout
-    plan['conv5'] = conv(ch[4], cin)
+    if conv5_as_stage:
+        plan['conv5_stage'] = [block(cin, ch[4], cin != ch[4], 1, stage4_dilation),
+                               block(ch[4], ch[4], False, 1, stage4_dilation)]
+    else:
+        plan['conv5'] = conv(ch[4], cin)
     for (nf, nconf, nvec, nsc) in heads:
         ncomp = 1 + nconf + 2 * nvec + nsc
         w = (rng.standard_normal((nf * ncomp, ch[4])) * np.sqrt(1.0 / ch[4])).astype(np.float32)
         b = (rng.standard_normal(nf * ncomp) * 0.1).astype(np.float32)
         b.reshape(nf, ncomp)[:, 1:1 + nconf] += np.float32(confidence_bias)
         plan['heads'].append({'w': w, 'b': b, 'n_fields': nf, 'n_comp': ncomp,
-                              'ops': head_ops(nconf, nvec, nsc, (True,) * nvec), 'stride': 16})
+                              'ops': head_ops(nconf, nvec, nsc, (True,) * nvec), 'stride': stride})
     return plan
 
 
@@ -658,15 +698,24 @@ def build_ops(plan, in_h, in_w, layout=None, fuse_dw=None):
                     'w': wp, 'b': bp, 'relu': int(relu), 'out': pieces[0][2],
                     'pieces': [tuple(int(v) for v in pc) for pc in pieces]})
 
-    def dwconv(tin, cols, width, wb, kernel, stride, pad, tout):
+    def dwconv(tin, cols, width, wb, e, tout):
+        """the depthwise conv of block entry e (its kernel, stride, pad and dilation)"""
+        kernel = e['kernel']
         w, b = wb
         w = w.reshape(w.shape[0], kernel * kernel)
         wp = np.zeros((width, kernel * kernel), dtype=np.float32)
         bp = np.zeros((width,), dtype=np.float32)
         wp[cols] = w
         bp[cols] = b
-        ops.append({'kind': 'dwconv', 'in': tin, 'in_off': 0, 'channels': width, 'kernel': kernel,
-                    'stride': stride, 'pad': pad, 'w': wp, 'b': bp, 'relu': 0, 'out': tout, 'out_off': 0})
+        op = {'kind': 'dwconv', 'in': tin, 'in_off': 0, 'channels': width, 'kernel': kernel,
+              'stride': e['stride'], 'pad': e['pad'], 'w': wp, 'b': bp, 'relu': 0, 'out': tout, 'out_off': 0}
+        if e.get('dilation', 1) != 1:
+            op['dilation'] = e['dilation']
+        ops.append(op)
+
+    def out_hw(h, w, e):
+        span = e.get('dilation', 1) * (e['kernel'] - 1) + 1
+        return (h + 2 * e['pad'] - span) // e['stride'] + 1, (w + 2 * e['pad'] - span) // e['stride'] + 1
 
     inp = plan['input']
     k = inp['w'].shape[-1]
@@ -676,15 +725,31 @@ def build_ops(plan, in_h, in_w, layout=None, fuse_dw=None):
     cur = tensor(h, w, pad16(c0))
     ops.append({'kind': 'input_conv', 'in_h': in_h, 'in_w': in_w, 'kernel': k, 'stride': inp['stride'],
                 'pad': inp['pad'], 'c_out': c0, 'w': _f32(inp['w']), 'b': _f32(inp['b']), 'relu': 1, 'out': cur})
+    if plan.get('input2') is not None:
+        # --shufflenetv2k-input-conv2-stride: 3x3 conv + BN + ReLU on the stem output (basenetworks.py:283-294), an
+        # implicit-GEMM conv op
+        e2 = plan['input2']
+        h, w = out_hw(h, w, e2)
+        c0 = e2['w'].shape[0]
+        t2 = tensor(h, w, pad16(c0))
+        ops.append({'kind': 'conv', 'in': cur, 'in_off': 0, 'c_in': e2['w'].shape[1], 'kernel': e2['kernel'],
+                    'stride': e2['stride'], 'pad': e2['pad'], 'dilation': 1, 'n_out': c0, 'w': _f32(e2['w']),
+                    'b': _f32(e2['b']), 'relu': 1, 'out': t2, 'out_off': 0, 'residual': -1, 'residual_off': 0})
+        cur = t2
     lay = _Layout(c0, split=False)
+    stages = list(plan['stages'])
+    if plan.get('conv5_stage') is not None:
+        # --shufflenetv2k-conv5-as-stage: without a branch1 (stage 4 as wide as conv5) the two blocks continue stage 4
+        # (same width, same dilation), otherwise they are one more stage whose first block has stride 1
+        c5s = plan['conv5_stage']
+        stages = stages[:-1] + [stages[-1] + c5s] if not c5s[0]['first'] else stages + [c5s]
     block_outputs = []
-    for blocks in plan['stages'] if layout == 'bins' else []:
+    for blocks in stages if layout == 'bins' else []:
         # ---- 'bins' layout: every channel is written once, into the buffer of the block that consumes it
         bf = blocks[0]['b2_pw2'][0].shape[0]
         hp = _branch_pitch(bf)
         e0 = blocks[0]
-        kk, st, pd = e0['kernel'], e0['stride'], e0['pad']
-        ho, wo = (h + 2 * pd - kk) // st + 1, (w + 2 * pd - kk) // st + 1
+        ho, wo = out_hw(h, w, e0)
         producers, bins, final = _plan_stage_bins(bf, len(blocks))
         t_bin = {t: tensor(ho, wo, pad16(bins[t]['width'])) for t in bins}
         t_bin['final'] = tensor(ho, wo, pad16(final['width']))
@@ -695,14 +760,14 @@ def build_ops(plan, in_h, in_w, layout=None, fuse_dw=None):
         cols = lay.cols()
         # block 0, branch1: dw (stride) -> 1x1; branch2: 1x1 -> dw (stride) -> 1x1   (basenetworks.py:200-226)
         t_a = tensor(ho, wo, lay.width)
-        dwconv(cur, cols, lay.width, e0['b1_dw'], kk, st, pd, t_a)
+        dwconv(cur, cols, lay.width, e0['b1_dw'], e0, t_a)
         conv1x1_scatter(t_a, cols, lay.width, e0['b1_pw'], True, producers[0]['order'], pieces_of(0))
         # the tensor in front of the STRIDE-2 depthwise conv gets 128-byte pixels (_dw_in_pitch).  Its producer leaves the padding
         # channels unwritten (rows with a 32-byte hole) and does not pay for writing them.
         t_c = tensor(h, w, _dw_in_pitch(bf))
         conv1x1(cur, 0, cols, lay.width, e0['b2_pw1'], True, t_c)
         t_d = tensor(ho, wo, hp)
-        dwconv(t_c, np.arange(bf), hp, e0['b2_dw'], kk, st, pd, t_d)
+        dwconv(t_c, np.arange(bf), hp, e0['b2_dw'], e0, t_d)
         conv1x1_scatter(t_d, np.arange(bf), hp, e0['b2_pw2'], True, producers[1]['order'], pieces_of(1))
         h, w = ho, wo
         for t, e in enumerate(blocks[1:], start=1):
@@ -715,37 +780,37 @@ def build_ops(plan, in_h, in_w, layout=None, fuse_dw=None):
             t_c = tensor(h, w, hp)          # stride-1 depthwise launches are issue bound: the padding buys nothing there
             conv1x1(t_bin[t], 0, in_cols, width, e['b2_pw1'], True, t_c)
             order = producers[t + 1]['order']
-            if fuse_dw and e['kernel'] == 5 and e['pad'] == 2 and len(order) <= 512:
+            # k_dw_gemm is built for the undilated 5x5, pad 2
+            if fuse_dw and e['kernel'] == 5 and e['pad'] == 2 and e.get('dilation', 1) == 1 and len(order) <= 512:
                 dw_conv1x1_scatter(t_c, hp, e['b2_dw'], 5, 1, 2, e['b2_pw2'], True, order, pieces_of(t + 1))
                 continue
             t_d = tensor(h, w, hp)
-            dwconv(t_c, np.arange(bf), hp, e['b2_dw'], e['kernel'], 1, e['pad'], t_d)
+            dwconv(t_c, np.arange(bf), hp, e['b2_dw'], e, t_d)
             conv1x1_scatter(t_d, np.arange(bf), hp, e['b2_pw2'], True, order, pieces_of(t + 1))
         logical = final['logical']
         phys = np.empty((2 * bf,), dtype=np.int64)
         phys[logical[logical >= 0]] = np.nonzero(logical >= 0)[0]
         cur, lay = t_bin['final'], _Layout(2 * bf, split=False, phys=phys, width=tensors[t_bin['final']][2])
         block_outputs.append((cur, lay))
-    for blocks in plan['stages'] if layout == 'shuffle' else []:
+    for blocks in stages if layout == 'shuffle' else []:
         for e in blocks:
             bf = e['b2_pw2'][0].shape[0]
             hp = pad16(bf)
-            kk, st, pd = e['kernel'], e['stride'], e['pad']
-            ho, wo = (h + 2 * pd - kk) // st + 1, (w + 2 * pd - kk) // st + 1
+            ho, wo = out_hw(h, w, e)
             out_lay = _Layout(2 * bf, split=True)
             t_out = tensor(ho, wo, out_lay.width)
             if e['first']:
                 cols = lay.cols()
                 # branch1: dw (stride) -> 1x1   (basenetworks.py:200-212)
                 t_a = tensor(ho, wo, lay.width)
-                dwconv(cur, cols, lay.width, e['b1_dw'], kk, st, pd, t_a)
+                dwconv(cur, cols, lay.width, e['b1_dw'], e, t_a)
                 t_b = tensor(ho, wo, hp)
                 conv1x1(t_a, 0, cols, lay.width, e['b1_pw'], True, t_b)
                 # branch2: 1x1 -> dw (stride) -> 1x1   (basenetworks.py:214-226)
                 t_c = tensor(h, w, hp)
                 conv1x1(cur, 0, cols, lay.width, e['b2_pw1'], True, t_c)
                 t_d = tensor(ho, wo, hp)
-                dwconv(t_c, np.arange(bf), hp, e['b2_dw'], kk, st, pd, t_d)
+                dwconv(t_c, np.arange(bf), hp, e['b2_dw'], e, t_d)
                 conv1x1(t_d, 0, np.arange(bf), hp, e['b2_pw2'], True, t_out, shuffle=(t_b, 0))
             else:
                 assert lay.split and lay.half == bf
@@ -757,10 +822,14 @@ def build_ops(plan, in_h, in_w, layout=None, fuse_dw=None):
                 t_c = tensor(h, w, hp)
                 conv1x1(cur, a0, lead + np.arange(bf), lead + bf, e['b2_pw1'], True, t_c)
                 t_d = tensor(ho, wo, hp)
-                dwconv(t_c, np.arange(bf), hp, e['b2_dw'], kk, st, pd, t_d)
+                dwconv(t_c, np.arange(bf), hp, e['b2_dw'], e, t_d)
                 conv1x1(t_d, 0, np.arange(bf), hp, e['b2_pw2'], True, t_out, shuffle=(cur, 0))
             cur, lay, h, w = t_out, out_lay, ho, wo
             block_outputs.append((cur, lay))
+    if plan.get('conv5_stage') is not None:
+        # the heads read the last stage output as it lies: lay.width columns in physical order
+        ops.append(_heads_op(plan['heads'], cur, lay.width, lay.cols()))
+        return tensors, ops, {'block_outputs': block_outputs, 'feature': (cur, lay)}
     w5, b5 = plan['conv5']
     c5 = w5.shape[0]
     t5 = tensor(h, w, pad16(c5))
@@ -769,11 +838,16 @@ def build_ops(plan, in_h, in_w, layout=None, fuse_dw=None):
     return tensors, ops, {'block_outputs': block_outputs, 'feature': (t5, _Layout(c5, split=False))}
 
 
-def _heads_op(heads, t_in, k_cols):
+def _heads_op(heads, t_in, k_cols, cols=None):
+    """cols: the physical column of each logical input channel (None: column c holds channel c)"""
+    w = _f32(np.concatenate([_f32(hd['w']) for hd in heads], axis=0))
+    if cols is not None:
+        wp = np.zeros((w.shape[0], k_cols), dtype=np.float32)
+        wp[:, cols] = w
+        w = wp
     return {'kind': 'heads', 'in': t_in, 'k_cols': k_cols, 'upsample': int(heads[0].get('upsample', 1)),
             'n_fields': [hd['n_fields'] for hd in heads], 'n_comp': [hd['n_comp'] for hd in heads],
-            'ops': [o for hd in heads for o in hd['ops']],
-            'w': _f32(np.concatenate([_f32(hd['w']) for hd in heads], axis=0)),
+            'ops': [o for hd in heads for o in hd['ops']], 'w': w,
             'b': _f32(np.concatenate([_f32(hd['b']) for hd in heads], axis=0))}
 
 
@@ -972,8 +1046,9 @@ class CompiledNet:
                 _lib.check(L.pifpaf_net_maxpool(H, o['in'], o['in_off'], o['channels'], o['stride'], o['out'],
                                                 o['out_off']))
             elif o['kind'] == 'dwconv':
-                _lib.check(L.pifpaf_net_dwconv(H, o['in'], o['in_off'], o['channels'], o['kernel'], o['stride'],
-                                               o['pad'], _ptr(o['w']), _ptr(o['b']), o['relu'], o['out'], o['out_off']))
+                _lib.check(L.pifpaf_net_dwconv_dilated(H, o['in'], o['in_off'], o['channels'], o['kernel'],
+                                                       o['stride'], o['pad'], _ptr(o['w']), _ptr(o['b']), o['relu'],
+                                                       o['out'], o['out_off'], o.get('dilation', 1)))
             elif o['kind'] == 'heads':
                 n = len(o['n_fields'])
                 nf = (ctypes.c_int32 * n)(*o['n_fields'])
