@@ -2053,9 +2053,16 @@ __global__ void __launch_bounds__(32) k_det_select(Dims d, GrowParams gp, int ma
     if (lane == 0) counts[b] = n_det;
 }
 
-// decoder/cifdet.py:55-64: torchvision.ops.batched_nms (coordinate trick: boxes shifted by category * (max + 1)) or
-// torchvision.ops.nms, then scores *= suppression except for the kept ones, kept flag = score > instance_threshold.
-// torchvision's CPU kernel restated: stable descending order, IoU = inter / (area_i + area_j - inter) > threshold.
+// decoder/cifdet.py:55-64: torchvision.ops.batched_nms or torchvision.ops.nms, then scores *= suppression except for
+// the kept ones, kept flag = score > instance_threshold.  torchvision's CPU kernel restated: stable descending order,
+// IoU = inter / (area_i + area_j - inter) > threshold.
+// batched_nms on CPU tensors dispatches on boxes.numel() > 4000 (torchvision/ops/boxes.py, batched_nms):
+//   n <= 1000: _batched_nms_coordinate_trick, one nms over boxes shifted by category * (max coordinate + 1).  The
+//              shift can overlap boxes of neighbouring categories (negative corners) and rounds shifted coordinates.
+//   n > 1000:  _batched_nms_vanilla, one nms per category on the unshifted boxes.  Restated here as one pass over the
+//              same stable order that compares only boxes of the same category: a category's subsequence of that
+//              order is the order its own nms sorts into, and suppression never crosses categories.
+constexpr int DET_NMS_VANILLA_MIN = 1001;
 constexpr int DET_NMS_NT = 128;
 __global__ void __launch_bounds__(DET_NMS_NT) k_det_nms(int max_det, float iou_threshold, int by_category,
                                                         float suppression, float instance_threshold,
@@ -2089,9 +2096,11 @@ __global__ void __launch_bounds__(DET_NMS_NT) k_det_nms(int max_det, float iou_t
     }
     __syncthreads();
     const float shift = s_max + 1.0f;                                  // max_coordinate + 1
+    const bool per_category = by_category && n >= DET_NMS_VANILLA_MIN;
+    const bool shifted = by_category && !per_category;
     for (int i = tid; i < n; i += DET_NMS_NT) {
         const float* r = rec + (size_t)i * DET_REC;
-        const float off = by_category ? r[0] * shift : 0.0f;          // idxs.to(boxes) * (max_coordinate + 1)
+        const float off = shifted ? r[0] * shift : 0.0f;              // idxs.to(boxes) * (max_coordinate + 1)
         const float4 bx = make_float4(r[2] + off, r[3] + off, r[4] + off, r[5] + off);
         box[i] = bx;
         area[i] = (bx.z - bx.x) * (bx.w - bx.y);
@@ -2108,9 +2117,11 @@ __global__ void __launch_bounds__(DET_NMS_NT) k_det_nms(int max_det, float iou_t
         if (!sup[i]) {
             const float4 bi = box[i];
             const float ai = area[i];
+            const float ci = per_category ? rec[(size_t)i * DET_REC] : 0.0f;
             for (int oj = oi + 1 + tid; oj < n; oj += DET_NMS_NT) {
                 const int j = order[oj];
                 if (sup[j]) continue;
+                if (per_category && rec[(size_t)j * DET_REC] != ci) continue;
                 const float4 bj = box[j];
                 const float xx1 = fmaxf(bi.x, bj.x), yy1 = fmaxf(bi.y, bj.y);
                 const float xx2 = fminf(bi.z, bj.z), yy2 = fminf(bi.w, bj.w);

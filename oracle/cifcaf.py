@@ -184,11 +184,43 @@ def grow_connection_blend(caf, x, y, s, filter_sigmas=1.0, only_max=False):
 
 _ref_loaded = False
 
-# statics of the reference classes we touch, with their defaults (csrc/src/*.cpp)
+# every static the reference extension exposes (csrc/src/module.cpp:26-32,58,76-117), keyed by the name of the
+# matching OracleParams field where there is one, with the reference's defaults (csrc/src/*.cpp)
 REF_DEFAULTS = {
-    'greedy': False, 'keypoint_threshold': 0.15, 'keypoint_threshold_rel': 0.5,
+    'block_joints': False, 'greedy': False, 'keypoint_threshold': 0.15, 'keypoint_threshold_rel': 0.5,
     'reverse_match': True, 'force_complete': False, 'force_complete_caf_th': 0.001,
+    'cifhr_neighbors': 16, 'cifhr_threshold': 0.3, 'cifhr_ablation_skip': False,
+    'seed_threshold': 0.2, 'seeds_ablation_nms': False, 'seeds_ablation_no_rescore': False,
+    'det_seed_threshold': 0.2, 'caf_score_th': 0.3, 'caf_ablation_no_rescore': False,
+    'nms_instance_threshold': 0.15, 'nms_keypoint_threshold': 0.15, 'nms_suppression': 0.00001,
+    'max_detections_before_nms': 120,
 }
+# name -> (torchscript class path, static) of REF_DEFAULTS
+_REF_STATICS = {
+    'block_joints': ('openpifpaf_decoder.CifCaf', 'block_joints'),
+    'greedy': ('openpifpaf_decoder.CifCaf', 'greedy'),
+    'keypoint_threshold': ('openpifpaf_decoder.CifCaf', 'keypoint_threshold'),
+    'keypoint_threshold_rel': ('openpifpaf_decoder.CifCaf', 'keypoint_threshold_rel'),
+    'reverse_match': ('openpifpaf_decoder.CifCaf', 'reverse_match'),
+    'force_complete': ('openpifpaf_decoder.CifCaf', 'force_complete'),
+    'force_complete_caf_th': ('openpifpaf_decoder.CifCaf', 'force_complete_caf_th'),
+    'cifhr_neighbors': ('openpifpaf_decoder_utils.CifHr', 'neighbors'),
+    'cifhr_threshold': ('openpifpaf_decoder_utils.CifHr', 'threshold'),
+    'cifhr_ablation_skip': ('openpifpaf_decoder_utils.CifHr', 'ablation_skip'),
+    'seed_threshold': ('openpifpaf_decoder_utils.CifSeeds', 'threshold'),
+    'seeds_ablation_nms': ('openpifpaf_decoder_utils.CifSeeds', 'ablation_nms'),
+    'seeds_ablation_no_rescore': ('openpifpaf_decoder_utils.CifSeeds', 'ablation_no_rescore'),
+    'det_seed_threshold': ('openpifpaf_decoder_utils.CifDetSeeds', 'threshold'),
+    'caf_score_th': ('openpifpaf_decoder_utils.CafScored', 'default_score_th'),
+    'caf_ablation_no_rescore': ('openpifpaf_decoder_utils.CafScored', 'ablation_no_rescore'),
+    'nms_instance_threshold': ('openpifpaf_decoder_utils.NMSKeypoints', 'instance_threshold'),
+    'nms_keypoint_threshold': ('openpifpaf_decoder_utils.NMSKeypoints', 'keypoint_threshold'),
+    'nms_suppression': ('openpifpaf_decoder_utils.NMSKeypoints', 'suppression'),
+    'max_detections_before_nms': ('openpifpaf_decoder.CifDet', 'max_detections_before_nms'),
+}
+# a reused reference CifCaf / CifDet runs its n-th call at CifHr revision n, until the call that would reach 10 001
+# zeroes the buffer and runs at 0 (src/cif_hr.cpp:115-120)
+REVISION_WRAP = 10000
 
 
 def ref_available():
@@ -210,26 +242,70 @@ def load_ref():
 
 
 def ref_configure(**kw):
-    """Set reference statics (module.cpp:26-32,76-117); unspecified -> defaults."""
+    """Set every reference static (module.cpp:26-32,58,76-117) to `kw` (keys of REF_DEFAULTS) or, when not given,
+    back to its default.  The statics are process-global: without the reset, one call's options would leak into
+    every later reference run of the process."""
     import torch
-    dec = load_ref()
-    cfg = dict(REF_DEFAULTS)
-    cfg.update({k: v for k, v in kw.items() if k in REF_DEFAULTS})
-    for k, v in cfg.items():
-        getattr(dec.CifCaf, 'set_' + k)(v)
-    u = torch.classes.openpifpaf_decoder_utils
-    u.CifHr.set_threshold(kw.get('cifhr_threshold', 0.3))
-    u.CifHr.set_neighbors(kw.get('cifhr_neighbors', 16))
-    u.CifSeeds.set_threshold(kw.get('seed_threshold', 0.2))
-    u.CafScored.set_default_score_th(kw.get('caf_score_th', 0.3))
-    u.NMSKeypoints.set_instance_threshold(kw.get('nms_instance_threshold', 0.15))
-    u.NMSKeypoints.set_keypoint_threshold(kw.get('nms_keypoint_threshold', 0.15))
-    u.NMSKeypoints.set_suppression(kw.get('nms_suppression', 0.00001))
+    load_ref()
+    unknown = set(kw) - set(REF_DEFAULTS)
+    assert not unknown, f'not a reference static: {sorted(unknown)}'
+    for k, default in REF_DEFAULTS.items():
+        path, static = _REF_STATICS[k]
+        ns, cls = path.split('.')
+        getattr(getattr(getattr(torch.classes, ns), cls), 'set_' + static)(type(default)(kw.get(k, default)))
+
+
+def ref_statics():
+    """the current value of every reference static, keyed like REF_DEFAULTS"""
+    import torch
+    load_ref()
+    out = {}
+    for k, (path, static) in _REF_STATICS.items():
+        ns, cls = path.split('.')
+        out[k] = getattr(getattr(getattr(torch.classes, ns), cls), 'get_' + static)()
+    return out
+
+
+def calls_before(revision):
+    """calls a reused reference instance makes before the call that runs at CifHr `revision`"""
+    assert revision == int(revision) and 0 <= revision <= REVISION_WRAP, revision
+    return REVISION_WRAP if revision == 0 else int(revision) - 1
+
+
+def _advance(revisions, zero_call):
+    """yield once before each call of an instance that runs at the next of `revisions`, after making the calls before it
+    on all-zero fields (calls_before).  With a CifHr threshold above 0 those write nothing, so the map stays as clean
+    as a fresh one: zeroed at the wrap to revision 0, where a never-written pixel reads 0 (src/cif_seeds.cpp:17-30),
+    and -1 at every other revision.  Pixels an earlier decode of the sequence wrote hold at most its revision + 1, so
+    they read -1 from two revisions on; a sequence may not decode at two consecutive revisions."""
+    import torch
+    calls, last = 0, None
+    for r in revisions:
+        n = calls_before(r)
+        assert n >= calls, f'revisions out of call order: {list(revisions)}'
+        assert last is None or r == 0 or r > last + 1, f'revision {r} right after {last} reads a dirty map'
+        if n > calls:
+            assert torch.classes.openpifpaf_decoder_utils.CifHr.get_threshold() > 0.0, \
+                'zero fields write the CifHr map at threshold 0'
+        for _ in range(n - calls):
+            zero_call()
+        yield r
+        calls, last = n + 1, r
 
 
 def ref_decode(cif, cif_stride, caf, caf_stride, skeleton, n_keypoints=None,
-               initial_annotations=None, initial_ids=None, taps=False):
-    """Run the unmodified reference on a FRESH CifCaf instance (revision 1.0)."""
+               initial_annotations=None, initial_ids=None, taps=False, revision=1):
+    """Run the unmodified reference on a CifCaf instance that decodes at CifHr `revision` (integer, 0 to
+    REVISION_WRAP; 1 = a FRESH instance).  See ref_decode_revisions."""
+    return ref_decode_revisions(cif, cif_stride, caf, caf_stride, skeleton, n_keypoints, initial_annotations,
+                                initial_ids, taps, revisions=(revision,))[0]
+
+
+def ref_decode_revisions(cif, cif_stride, caf, caf_stride, skeleton, n_keypoints=None,
+                         initial_annotations=None, initial_ids=None, taps=False, revisions=(1,)):
+    """The same decode on ONE reference CifCaf instance at each of `revisions` (in call order: 1, 2, ..., 10000,
+    then 0), the calls in between made on all-zero fields of the same shape (_advance).  Returns a list of what
+    ref_decode returns."""
     import torch
     dec = load_ref()
     cif_t = torch.from_numpy(np.ascontiguousarray(cif, dtype=np.float32))
@@ -237,6 +313,16 @@ def ref_decode(cif, cif_stride, caf, caf_stride, skeleton, n_keypoints=None,
     sk = torch.from_numpy(np.ascontiguousarray(skeleton, dtype=np.int64))
     K = int(n_keypoints if n_keypoints is not None else cif_t.shape[0])
     inst = dec.CifCaf(K, sk)
+    zc, zf = torch.zeros_like(cif_t), torch.zeros_like(caf_t)
+    out = []
+    for _ in _advance(revisions, lambda: inst.call(zc, cif_stride, zf, caf_stride)):
+        out.append(_ref_cifcaf_call(inst, cif_t, cif_stride, caf_t, caf_stride, sk, initial_annotations,
+                                    initial_ids, taps))
+    return out
+
+
+def _ref_cifcaf_call(inst, cif_t, cif_stride, caf_t, caf_stride, sk, initial_annotations, initial_ids, taps):
+    import torch
     ia = ii = None
     if initial_annotations is not None and len(initial_annotations):
         ia = torch.from_numpy(np.ascontiguousarray(initial_annotations, dtype=np.float32))
@@ -259,11 +345,22 @@ def ref_decode(cif, cif_stride, caf, caf_stride, skeleton, n_keypoints=None,
     return ann.numpy().copy(), ids.numpy().copy(), t
 
 
-def ref_decode_det(field, stride):
-    """Run the unmodified reference CifDet (csrc/src/cifdet.cpp) on a FRESH instance.  (CifDetHr is not exported
-    as a TorchScript class, module.cpp:76-102, so there are no stage taps on this side.)"""
+def ref_decode_det(field, stride, revision=1):
+    """Run the unmodified reference CifDet (csrc/src/cifdet.cpp) on an instance that decodes at CifHr `revision`
+    (1 = a FRESH instance; see ref_decode_det_revisions)."""
+    return ref_decode_det_revisions(field, stride, (revision,))[0]
+
+
+def ref_decode_det_revisions(field, stride, revisions=(1,)):
+    """ref_decode_revisions for CifDet.  (CifDetHr is not exported as a TorchScript class, module.cpp:76-102, so
+    there are no stage taps on this side.)"""
     import torch
     dec = load_ref()
     f_t = torch.from_numpy(np.ascontiguousarray(field, dtype=np.float32))
-    cats, scores, boxes = dec.CifDet().call(f_t, stride)
-    return cats.numpy().copy(), scores.numpy().copy(), boxes.numpy().copy().reshape(-1, 4)
+    inst = dec.CifDet()
+    zero = torch.zeros_like(f_t)
+    out = []
+    for _ in _advance(revisions, lambda: inst.call(zero, stride)):
+        cats, scores, boxes = inst.call(f_t, stride)
+        out.append((cats.numpy().copy(), scores.numpy().copy(), boxes.numpy().copy().reshape(-1, 4)))
+    return out

@@ -36,6 +36,45 @@ CASES = [
 ]
 
 
+# non-default decoder options (reference CLI flags of decoder/factory.py:52-82 and decoder/cifcaf.py:174-211, or the
+# statics of csrc/src/module.cpp), each run on the fields of OPTION_FIELDS: tests/golden/options_<option>__<field>.npz
+FORCE_COMPLETE = {'force_complete': True, 'keypoint_threshold': 0.0, 'keypoint_threshold_rel': 0.0,
+                  'nms_keypoint_threshold': 0.0, 'nms_instance_threshold': 0.0}     # what --force-complete-pose sets
+OPTION_CASES = [
+    # name, reference statics
+    ('cif_th_0.05', {'cifhr_threshold': 0.05}),                                  # --cif-th
+    ('cif_th_0.5', {'cifhr_threshold': 0.5}),
+    ('neighbors_1', {'cifhr_neighbors': 1}),                                     # CifHr.neighbors
+    ('neighbors_64', {'cifhr_neighbors': 64}),
+    ('seed_th_0.01', {'seed_threshold': 0.01, 'keypoint_threshold': 0.01}),     # --seed-threshold (lowers the
+    ('seed_th_0.5', {'seed_threshold': 0.5}),                                    # keypoint threshold with it)
+    ('caf_th_0.05', {'caf_score_th': 0.05}),                                     # --caf-th
+    ('caf_th_0.6', {'caf_score_th': 0.6}),
+    ('seeds_nms', {'seeds_ablation_nms': True}),                                 # --ablation-cifseeds-nms
+    ('seeds_no_rescore', {'seeds_ablation_no_rescore': True}),                   # --ablation-cifseeds-no-rescore
+    ('caf_no_rescore', {'caf_ablation_no_rescore': True}),                       # --ablation-caf-no-rescore
+    ('no_rescore_skip', {'seeds_ablation_no_rescore': True, 'caf_ablation_no_rescore': True,
+                         'cifhr_ablation_skip': True}),                          # both, which set CifHr.ablation_skip
+    ('block_joints', {'block_joints': True}),                                    # --cifcaf-block-joints
+    ('kp_rel_0', {'keypoint_threshold_rel': 0.0}),                               # --keypoint-threshold-rel
+    ('kp_rel_1', {'keypoint_threshold_rel': 1.0}),
+    ('instance_th_0', {'nms_instance_threshold': 0.0}),                          # --instance-threshold
+    ('instance_th_0.4', {'nms_instance_threshold': 0.4}),
+    ('suppression_0', {'nms_suppression': 0.0}),                                 # NMSKeypoints.suppression
+    ('suppression_1', {'nms_suppression': 1.0}),
+    ('force_complete', dict(FORCE_COMPLETE, force_complete_caf_th=-1.0)),        # --force-complete-caf-th -1: --caf-th
+    ('force_complete_caf_th_0.3', dict(FORCE_COMPLETE, force_complete_caf_th=0.3)),
+    ('force_complete_greedy', dict(FORCE_COMPLETE, greedy=True)),
+    # evaluation style: --force-complete-pose --seed-threshold 0.01 --cif-th 0.1 --caf-th 0.1 --no-reverse-match
+    ('eval', dict(FORCE_COMPLETE, seed_threshold=0.01, cifhr_threshold=0.1, caf_score_th=0.1, reverse_match=False)),
+]
+OPTION_FIELDS = ['coco41_poisson_s0', 'crowd30', 'wholebody_4p', 'coco51_5p_stride8']       # names of CASES
+
+
+def option_golden_name(option, field):
+    return f'options_{option}__{field}'
+
+
 DET_CASES = [
     # name, n_categories, h, w, n_objects, seed, n_distractors, stride
     ('det11_3cat_1', 3, 11, 11, 1, 2, 2, 16),
@@ -49,33 +88,45 @@ def sha(a):
     return hashlib.sha256(np.ascontiguousarray(a).tobytes()).hexdigest()
 
 
+def write_decoder_golden(path, workload, h, w, n_people, seed, n_dis, stride, statics, store_fields=False,
+                         seed_arrays=True):
+    """the reference's outputs under `statics` on a fresh instance, in the layout of tests/golden/decoder_*.npz.
+    seed_arrays=False stores the seeds as n_seeds and the sha256 of seeds_f / seeds_vxys (a crowd or WholeBody
+    input has thousands of seeds; the option goldens would otherwise take megabytes)."""
+    f = synth.make_fields(workload, h, w, n_people, seed, n_dis)
+    oc.ref_configure(**statics)
+    ann, ids, taps = oc.ref_decode(f['cif'], stride, f['caf'], stride, f['skeleton'], f['n_keypoints'], taps=True)
+    if seed_arrays:
+        seeds = dict(seeds_f=taps['seeds_f'], seeds_vxys=taps['seeds_vxys'])
+    else:
+        seeds = dict(n_seeds=len(taps['seeds_f']), seeds_f_sha256=sha(taps['seeds_f']),
+                     seeds_vxys_sha256=sha(taps['seeds_vxys']))
+    data = dict(
+        workload=workload, h=h, w=w, n_people=-1 if n_people is None else n_people, seed=seed,
+        n_distractors=n_dis, stride=stride,
+        statics_keys=np.array(list(statics.keys()), dtype='U64'),
+        statics_vals=np.array([float(v) for v in statics.values()], dtype=np.float64),
+        fields_sha256=synth.fields_digest(f['cif'], f['caf']),
+        annotations=ann, ids=ids,
+        **seeds,
+        n_fwd=np.array([len(x) for x in taps['fwd']], dtype=np.int64),
+        n_bwd=np.array([len(x) for x in taps['bwd']], dtype=np.int64),
+        fwd_sha256=sha(np.concatenate([x.reshape(-1, 7) for x in taps['fwd']])),
+        bwd_sha256=sha(np.concatenate([x.reshape(-1, 7) for x in taps['bwd']])),
+        cifhr_sha256=sha(taps['cifhr']), cifhr_sum=float(taps['cifhr'].astype(np.float64).sum()),
+    )
+    if store_fields:
+        data['cif'] = f['cif']
+        data['caf'] = f['caf']
+    np.savez_compressed(path, **data)
+    print(os.path.basename(path), 'N =', len(ann), 'seeds =', len(taps['seeds_f']), os.path.getsize(path), 'bytes')
+
+
 def main():
     out_dir = os.path.join(ROOT, 'tests', 'golden')
     os.makedirs(out_dir, exist_ok=True)
-    for name, workload, h, w, n_people, seed, n_dis, stride, statics in CASES:
-        f = synth.make_fields(workload, h, w, n_people, seed, n_dis)
-        oc.ref_configure(**statics)
-        ann, ids, taps = oc.ref_decode(f['cif'], stride, f['caf'], stride, f['skeleton'], f['n_keypoints'], taps=True)
-        data = dict(
-            workload=workload, h=h, w=w, n_people=-1 if n_people is None else n_people, seed=seed,
-            n_distractors=n_dis, stride=stride,
-            statics_keys=np.array(list(statics.keys()), dtype='U64'),
-            statics_vals=np.array([float(v) for v in statics.values()], dtype=np.float64),
-            fields_sha256=synth.fields_digest(f['cif'], f['caf']),
-            annotations=ann, ids=ids,
-            seeds_f=taps['seeds_f'], seeds_vxys=taps['seeds_vxys'],
-            n_fwd=np.array([len(x) for x in taps['fwd']], dtype=np.int64),
-            n_bwd=np.array([len(x) for x in taps['bwd']], dtype=np.int64),
-            fwd_sha256=sha(np.concatenate([x.reshape(-1, 7) for x in taps['fwd']])),
-            bwd_sha256=sha(np.concatenate([x.reshape(-1, 7) for x in taps['bwd']])),
-            cifhr_sha256=sha(taps['cifhr']), cifhr_sum=float(taps['cifhr'].astype(np.float64).sum()),
-        )
-        if name == 'coco11_1p':
-            data['cif'] = f['cif']
-            data['caf'] = f['caf']
-        path = os.path.join(out_dir, f'decoder_{name}.npz')
-        np.savez_compressed(path, **data)
-        print(name, 'N =', len(ann), 'seeds =', len(taps['seeds_f']), os.path.getsize(path), 'bytes')
+    for name, *args in CASES:
+        write_decoder_golden(os.path.join(out_dir, f'decoder_{name}.npz'), *args, store_fields=name == 'coco11_1p')
     oc.ref_configure()
     # CifDet (csrc/src/cifdet.cpp): raw output of a FRESH torch.classes.openpifpaf_decoder.CifDet instance
     for name, n_cat, h, w, n_obj, seed, n_dis, stride in DET_CASES:
@@ -242,6 +293,20 @@ def main_reference_outputs():
     print('reference_outputs', os.path.getsize(path), 'bytes')
 
 
+def main_options():
+    """tests/golden/options_*.npz: every OPTION_CASES entry on every OPTION_FIELDS input"""
+    out_dir = os.path.join(ROOT, 'tests', 'golden')
+    cases = {name: args for name, *args in CASES}
+    for option, statics in OPTION_CASES:
+        for field in OPTION_FIELDS:
+            args = cases[field][:-1]
+            assert not cases[field][-1]
+            write_decoder_golden(os.path.join(out_dir, option_golden_name(option, field) + '.npz'), *args, statics,
+                                 seed_arrays=False)
+    oc.ref_configure()
+
+
 if __name__ == '__main__':
     main()
+    main_options()
     main_reference_outputs()

@@ -17,6 +17,11 @@ def golden_cases():
     return sorted(glob.glob(os.path.join(GOLDEN_DIR, 'decoder_*.npz')))
 
 
+def golden_option_cases():
+    """tests/golden/options_*.npz: the reference under non-default decoder options (oracle/make_golden.py OPTION_CASES)"""
+    return sorted(glob.glob(os.path.join(GOLDEN_DIR, 'options_*.npz')))
+
+
 def golden_det_cases():
     return sorted(glob.glob(os.path.join(GOLDEN_DIR, 'cifdet_*.npz')))
 
@@ -40,12 +45,25 @@ def load_golden(path):
     return g, f, statics, digest_ok
 
 
+FLAG_STATICS = ('greedy', 'force_complete', 'reverse_match', 'block_joints', 'cifhr_ablation_skip', 'seeds_ablation_nms',
+                'seeds_ablation_no_rescore', 'caf_ablation_no_rescore', 'cifhr_neighbors')
+
+
 def statics_to_params(statics):
     """reference static names -> params-struct field values (ints for flags)."""
     out = {}
     for k, v in statics.items():
-        out[k] = int(v) if k in ('greedy', 'force_complete', 'reverse_match') else float(v)
+        out[k] = int(v) if k in FLAG_STATICS else float(v)
     return out
+
+
+def reset_native_statics():
+    """every static of the native decoder classes back to its default (the reference's)"""
+    from openpifpaf_b200 import decoder
+    for cls in (decoder.CifCaf, decoder.CifHr, decoder.CifSeeds, decoder.CafScored, decoder.NMSKeypoints,
+                decoder.CifDetSeeds, decoder.CifDet):
+        for name, default in cls.STATICS.items():
+            getattr(cls, 'set_' + name)(default)
 
 
 def assert_annotations_close(got, want, what=''):
