@@ -130,6 +130,26 @@ def _pair(v):
     return tuple(v) if isinstance(v, (tuple, list)) else (v, v)
 
 
+def _fold_stem(conv, bn):
+    """the stem conv + BN of a ShuffleNetV2K or Resnet input block, folded (its kernel size is the weight's)"""
+    w, b = _fold(conv, bn)
+    return {'w': w, 'b': b, 'stride': int(conv.stride[0]), 'pad': int(conv.padding[0])}
+
+
+def _conv_entry(c, n):
+    """a square conv + BN, folded, as an implicit-GEMM conv entry; 'dilation' only where it is not 1"""
+    if len(set(_pair(c.kernel_size))) != 1 or len(set(_pair(c.stride))) != 1 or \
+            len(set(_pair(c.padding))) != 1 or len(set(_pair(c.dilation))) != 1:
+        raise UnsupportedModel('only square ResNet convolutions are supported')
+    w, b = _fold(c, n)
+    e = {'w': w, 'b': b, 'kernel': int(c.kernel_size[0]), 'stride': int(c.stride[0]), 'pad': int(c.padding[0])}
+    if c.dilation[0] != 1:
+        if c.stride[0] != 1:
+            raise UnsupportedModel('dilated convolutions with a stride are not supported')
+        e['dilation'] = int(c.dilation[0])
+    return e
+
+
 def _plan_from_resnet(shell):
     """basenetworks.py:71-150: torchvision ResNet (input_block = conv1, bn1, relu, then the max pool under
     --resnet-pool0-stride or a 3x3 conv + BN + ReLU under --resnet-input-conv2-stride; block2..block5 = layer1..layer4
@@ -142,36 +162,19 @@ def _plan_from_resnet(shell):
     for m in base.modules():
         if isinstance(m, torch.nn.Conv2d) and m.groups != 1:
             raise UnsupportedModel('grouped convolutions (ResNeXt) are not supported')
-
-    def conv_entry(c, n):
-        if len(set(_pair(c.kernel_size))) != 1 or len(set(_pair(c.stride))) != 1 or \
-                len(set(_pair(c.padding))) != 1 or len(set(_pair(c.dilation))) != 1:
-            raise UnsupportedModel('only square ResNet convolutions are supported')
-        w_, b_ = _fold(c, n)
-        e = {'w': w_, 'b': b_, 'kernel': int(c.kernel_size[0]), 'stride': int(c.stride[0]), 'pad': int(c.padding[0])}
-        if c.dilation[0] != 1:
-            if c.stride[0] != 1:
-                raise UnsupportedModel('dilated convolutions with a stride are not supported')
-            e['dilation'] = int(c.dilation[0])
-        return e
-
     parts = _resnet_input_block(base.input_block)
-    conv, bn = parts[0][1]
-    w, b = _fold(conv, bn)
-    plan = {'kind': 'resnet',
-            'input': {'w': w, 'b': b, 'stride': int(conv.stride[0]), 'pad': int(conv.padding[0])},
-            'blocks': [], 'heads': _heads_plan(shell, base)}
+    plan = {'kind': 'resnet', 'input': _fold_stem(*parts[0][1]), 'blocks': [], 'heads': _heads_plan(shell, base)}
     if len(parts) == 2 and parts[1][0] == 'pool':
         plan['pool'] = {'stride': int(_pair(parts[1][1].stride)[0])}
     elif len(parts) == 2:
-        plan['input2'] = conv_entry(*parts[1][1])
+        plan['input2'] = _conv_entry(*parts[1][1])
 
     for stage in (base.block2, base.block3, base.block4, base.block5):
         for blk in stage:
-            e = {'convs': [conv_entry(blk.conv1, blk.bn1), conv_entry(blk.conv2, blk.bn2)]}
+            e = {'convs': [_conv_entry(blk.conv1, blk.bn1), _conv_entry(blk.conv2, blk.bn2)]}
             if hasattr(blk, 'conv3'):
-                e['convs'].append(conv_entry(blk.conv3, blk.bn3))
-            e['downsample'] = None if blk.downsample is None else conv_entry(blk.downsample[0], blk.downsample[1])
+                e['convs'].append(_conv_entry(blk.conv3, blk.bn3))
+            e['downsample'] = None if blk.downsample is None else _conv_entry(blk.downsample[0], blk.downsample[1])
             plan['blocks'].append(e)
     return plan
 
@@ -284,18 +287,14 @@ def _plan_from_shufflenetv2k(shell):
     base = shell.base_net
     if len(base.input_block) not in (1, 2):
         raise UnsupportedModel(f'unsupported ShuffleNetV2K input block of {len(base.input_block)} convolutions')
-    conv, bn = base.input_block[0][0], base.input_block[0][1]
-    w, b = _fold(conv, bn)
-    plan = {'kind': 'shufflenetv2k',
-            'input': {'w': w, 'b': b, 'stride': int(conv.stride[0]), 'pad': int(conv.padding[0])},
+    plan = {'kind': 'shufflenetv2k', 'input': _fold_stem(base.input_block[0][0], base.input_block[0][1]),
             'stages': [], 'heads': []}
     if len(base.input_block) == 2:
         conv, bn = base.input_block[1][0], base.input_block[1][1]
         if _pair(conv.kernel_size) != (3, 3) or _pair(conv.stride) != (2, 2) or _pair(conv.padding) != (1, 1) or \
                 _pair(conv.dilation) != (1, 1) or conv.groups != 1:
             raise UnsupportedModel(f'ShuffleNetV2K input_conv2: expected a 3x3 stride-2 conv, got {conv}')
-        w, b = _fold(conv, bn)
-        plan['input2'] = {'w': w, 'b': b, 'kernel': 3, 'stride': 2, 'pad': 1}
+        plan['input2'] = _conv_entry(conv, bn)
     for stage in (base.stage2, base.stage3, base.stage4):
         plan['stages'].append([_shufflenetv2k_block(blk) for blk in stage])
     if isinstance(base.conv5[0], torch.nn.Conv2d):
@@ -365,14 +364,30 @@ def random_plan(base_name='shufflenetv2k16', heads=((17, 1, 1, 1), (19, 1, 2, 2)
                                block(ch[4], ch[4], False, 1, stage4_dilation)]
     else:
         plan['conv5'] = conv(ch[4], cin)
-    for (nf, nconf, nvec, nsc) in heads:
-        ncomp = 1 + nconf + 2 * nvec + nsc
-        w = (rng.standard_normal((nf * ncomp, ch[4])) * np.sqrt(1.0 / ch[4])).astype(np.float32)
-        b = (rng.standard_normal(nf * ncomp) * 0.1).astype(np.float32)
-        b.reshape(nf, ncomp)[:, 1:1 + nconf] += np.float32(confidence_bias)
-        plan['heads'].append({'w': w, 'b': b, 'n_fields': nf, 'n_comp': ncomp,
-                              'ops': head_ops(nconf, nvec, nsc, (True,) * nvec), 'stride': stride})
+    plan['heads'] = _random_heads(rng, heads, ch[4], stride, confidence_bias)
     return plan
+
+
+def _random_heads(rng, heads, c_in, stride, confidence_bias, upsample=1):
+    """Random-init heads on c_in features at the given feature stride, drawn from rng (weights, then biases, head by
+    head).  A head spec is (n_fields, n_confidences, n_vectors, n_scales), optionally with the vector offsets as a
+    fifth entry (default: every vector has one).  upsample is the heads' upsample_stride."""
+    out = []
+    for spec in heads:
+        nf, nconf, nvec, nsc = spec[:4]
+        offsets = tuple(spec[4]) if len(spec) > 4 else (True,) * nvec
+        ncomp = 1 + nconf + 2 * nvec + nsc
+        nc = nf * ncomp * upsample * upsample
+        w = (rng.standard_normal((nc, c_in)) * np.sqrt(1.0 / c_in)).astype(np.float32)
+        b = (rng.standard_normal(nc) * 0.1).astype(np.float32)
+        # conv channel (field * n_comp + comp) * up^2 + sub (PixelShuffle order, heads.py:333-343)
+        b.reshape(nf, ncomp, upsample * upsample)[:, 1:1 + nconf] += np.float32(confidence_bias)
+        hd = {'w': w, 'b': b, 'n_fields': nf, 'n_comp': ncomp,
+              'ops': head_ops(nconf, nvec, nsc, offsets), 'stride': stride // upsample}
+        if upsample != 1:
+            hd['upsample'] = upsample
+        out.append(hd)
+    return out
 
 
 RESNET_CONFIGS = {      # torchvision.models.resnet: (block, layers); network/factory.py:57-58
@@ -431,20 +446,7 @@ def random_resnet_plan(base_name='resnet50', heads=((17, 1, 1, 1), (19, 1, 2, 2)
             down = conv(cout, cin, 1, stride, gain=1.0) if (stride != 1 or cin != cout) else None
             plan['blocks'].append({'convs': convs, 'downsample': down})
             cin = cout
-    for spec in heads:
-        nf, nconf, nvec, nsc = spec[:4]
-        offsets = tuple(spec[4]) if len(spec) > 4 else (True,) * nvec
-        ncomp = 1 + nconf + 2 * nvec + nsc
-        nc = nf * ncomp * upsample * upsample
-        w = (rng.standard_normal((nc, cin)) * np.sqrt(1.0 / cin)).astype(np.float32)
-        b = (rng.standard_normal(nc) * 0.1).astype(np.float32)
-        # conv channel (field * n_comp + comp) * up^2 + sub (PixelShuffle order, heads.py:333-343)
-        b.reshape(nf, ncomp, upsample * upsample)[:, 1:1 + nconf] += np.float32(confidence_bias)
-        hd = {'w': w, 'b': b, 'n_fields': nf, 'n_comp': ncomp,
-              'ops': head_ops(nconf, nvec, nsc, offsets), 'stride': base_stride // upsample}
-        if upsample != 1:
-            hd['upsample'] = upsample
-        plan['heads'].append(hd)
+    plan['heads'] = _random_heads(rng, heads, cin, base_stride, confidence_bias, upsample)
     return plan
 
 
@@ -622,121 +624,173 @@ def default_fuse_dw():
     return os.environ.get('PIFPAF_FUSE_DW', '0') == '1'
 
 
-def build_ops(plan, in_h, in_w, layout=None, fuse_dw=None):
-    """Lower a plan to the op list of libpifpaf_b200 (pure Python; no GPU needed).
+def _scatter_rows(wb, order, in_cols, k_cols):
+    """GEMM operands of a 1x1 conv (w [n, c_in, ...], b [n]): weights [len(order), k_cols] whose row j is output channel
+    order[j] (-1: a zero padding row) and whose column in_cols[i] holds input channel i, and the bias [len(order)]"""
+    w, b = wb
+    w = w.reshape(w.shape[0], -1)
+    assert len(in_cols) == w.shape[1]
+    real = order >= 0
+    wp = np.zeros((len(order), k_cols), dtype=np.float32)
+    wp[np.ix_(np.nonzero(real)[0], in_cols)] = w[order[real]]
+    bp = np.zeros((len(order),), dtype=np.float32)
+    bp[real] = b[order[real]]
+    return wp, bp
 
-    Returns (tensors, ops): tensors[i] = (h, w, c_phys); ops are dicts with a 'kind' in
+
+def _dw_rows(wb, kernel, width, cols=None):
+    """depthwise weights [width, kernel^2] and bias [width] with channel i of wb at row cols[i] (default: row i), zero
+    elsewhere"""
+    w, b = wb
+    c = w.shape[0]
+    cols = np.arange(c) if cols is None else cols
+    wp = np.zeros((width, kernel * kernel), dtype=np.float32)
+    bp = np.zeros((width,), dtype=np.float32)
+    wp[cols] = w.reshape(c, kernel * kernel)
+    bp[cols] = b
+    return wp, bp
+
+
+class _OpList:
+    """The tensors (tensors[i] = (h, w, c_phys)) and ops of one lowering.  Each op kind is written by one method here,
+    whose dict fields are the C ABI arguments (include/pifpaf_b200.h); the lowerings only wire them.  Methods without a
+    t_out argument add their output tensor and return it."""
+
+    def __init__(self):
+        self.tensors, self.ops = [], []
+
+    def tensor(self, h, w, c):
+        self.tensors.append((h, w, c))
+        return len(self.tensors) - 1
+
+    def out_hw(self, t_in, e):
+        """output size of the conv entry e (kernel, stride, pad, optional dilation) on tensor t_in"""
+        h, w, _ = self.tensors[t_in]
+        span = e.get('dilation', 1) * (e['kernel'] - 1) + 1
+        return (h + 2 * e['pad'] - span) // e['stride'] + 1, (w + 2 * e['pad'] - span) // e['stride'] + 1
+
+    def input_conv(self, inp, in_h, in_w, act):
+        """the stem on the [3, in_h, in_w] image"""
+        k, c = inp['w'].shape[-1], inp['w'].shape[0]
+        t = self.tensor((in_h + 2 * inp['pad'] - k) // inp['stride'] + 1,
+                        (in_w + 2 * inp['pad'] - k) // inp['stride'] + 1, pad16(c))
+        self.ops.append({'kind': 'input_conv', 'in_h': in_h, 'in_w': in_w, 'kernel': k, 'stride': inp['stride'],
+                         'pad': inp['pad'], 'c_out': c, 'w': _f32(inp['w']), 'b': _f32(inp['b']), 'relu': act,
+                         'out': t})
+        return t
+
+    def conv(self, t_in, e, act, residual=-1):
+        """implicit-GEMM conv of entry e; residual: a tensor added to the output before the activation"""
+        n = e['w'].shape[0]
+        t = self.tensor(*self.out_hw(t_in, e), pad16(n))
+        self.ops.append({'kind': 'conv', 'in': t_in, 'in_off': 0, 'c_in': e['w'].shape[1], 'kernel': e['kernel'],
+                         'stride': e['stride'], 'pad': e['pad'], 'dilation': e.get('dilation', 1), 'n_out': n,
+                         'w': _f32(e['w']), 'b': _f32(e['b']), 'relu': int(act), 'out': t, 'out_off': 0,
+                         'residual': residual, 'residual_off': 0})
+        return t
+
+    def dwconv(self, t_in, wb, e, act=0, cols=None, width=None):
+        """depthwise conv with the kernel, stride, pad and dilation of entry e.  cols: the channel of t_in each weight
+        row meets (default: in order); width: the channels the op covers and the output's pitch (default: the weights'
+        channels, the output padded to 16)"""
+        c = wb[0].shape[0]
+        t = self.tensor(*self.out_hw(t_in, e), pad16(c) if width is None else width)
+        w, b = _dw_rows(wb, e['kernel'], c if width is None else width, cols)
+        op = {'kind': 'dwconv', 'in': t_in, 'in_off': 0, 'channels': w.shape[0], 'kernel': e['kernel'],
+              'stride': e['stride'], 'pad': e['pad'], 'w': w, 'b': b, 'relu': act, 'out': t, 'out_off': 0}
+        if e.get('dilation', 1) != 1:
+            op['dilation'] = e['dilation']
+        self.ops.append(op)
+        return t
+
+    def conv1x1(self, t_in, in_off, in_cols, k_cols, wb, act, t_out, shuffle=None):
+        """1x1 conv GEMM over k_cols columns of t_in from in_off (input channel i at column in_cols[i]); shuffle =
+        (tensor, column): write the output interleaved with those pass-through channels (cat + channel_shuffle)"""
+        n = wb[0].shape[0]
+        w, b = _scatter_rows(wb, np.arange(n), in_cols, k_cols)
+        s_t, s_off = (-1, 0) if shuffle is None else shuffle
+        self.ops.append({'kind': 'conv1x1', 'in': t_in, 'in_off': in_off, 'k_cols': k_cols, 'n_out': n,
+                         'w': w, 'b': b, 'relu': int(act), 'out': t_out, 'out_off': 0,
+                         'shuffle_src': s_t, 'shuffle_off': s_off})
+
+    def conv1x1_scatter(self, t_in, in_cols, k_cols, wb, act, order, pieces):
+        """1x1 conv whose GEMM columns are the producer's output channels in `order` (-1: padding column, zero
+        weights) and whose column pieces (col0, count, tensor, tensor_col) go to different tensors"""
+        w, b = _scatter_rows(wb, order, in_cols, k_cols)
+        self.ops.append({'kind': 'conv1x1', 'in': t_in, 'in_off': 0, 'k_cols': k_cols, 'n_out': len(order),
+                         'w': w, 'b': b, 'relu': int(act), 'out': pieces[0][2], 'out_off': pieces[0][3],
+                         'shuffle_src': -1, 'shuffle_off': 0, 'pieces': [tuple(int(v) for v in pc) for pc in pieces]})
+
+    def dw_conv1x1_scatter(self, t_in, width, dw_wb, e, wb, act, order, pieces):
+        """the depthwise conv of entry e on the first len(dw) of `width` channels of t_in, then conv1x1_scatter on its
+        output -- one fused kernel, no intermediate tensor"""
+        dw_w, dw_b = _dw_rows(dw_wb, e['kernel'], width)
+        w, b = _scatter_rows(wb, order, np.arange(dw_wb[0].shape[0]), width)
+        self.ops.append({'kind': 'dw_conv1x1', 'in': t_in, 'in_off': 0, 'channels': width, 'kernel': e['kernel'],
+                         'stride': e['stride'], 'pad': e['pad'], 'dw_w': dw_w, 'dw_b': dw_b, 'dw_relu': 0,
+                         'n_out': len(order), 'w': w, 'b': b, 'relu': int(act), 'out': pieces[0][2],
+                         'pieces': [tuple(int(v) for v in pc) for pc in pieces]})
+
+    def maxpool(self, t_in, channels, stride):
+        """3x3 max pool, padding 1"""
+        h, w, _ = self.tensors[t_in]
+        t = self.tensor((h - 1) // stride + 1, (w - 1) // stride + 1, pad16(channels))
+        self.ops.append({'kind': 'maxpool', 'in': t_in, 'in_off': 0, 'channels': channels, 'stride': stride,
+                         'out': t, 'out_off': 0})
+        return t
+
+    def heads(self, heads, t_in, k_cols, cols=None):
+        """all heads as one GEMM with the CompositeField4 eval epilogue; cols: the physical column of each logical input
+        channel (None: column c holds channel c)"""
+        w = _f32(np.concatenate([_f32(hd['w']) for hd in heads], axis=0))
+        if cols is not None:
+            wp = np.zeros((w.shape[0], k_cols), dtype=np.float32)
+            wp[:, cols] = w
+            w = wp
+        self.ops.append({'kind': 'heads', 'in': t_in, 'k_cols': k_cols, 'upsample': int(heads[0].get('upsample', 1)),
+                         'n_fields': [hd['n_fields'] for hd in heads], 'n_comp': [hd['n_comp'] for hd in heads],
+                         'ops': [o for hd in heads for o in hd['ops']], 'w': w,
+                         'b': _f32(np.concatenate([_f32(hd['b']) for hd in heads], axis=0))})
+
+
+def build_ops(plan, in_h, in_w, layout=None, fuse_dw=None):
+    """Lower a plan to the op list of libpifpaf_b200 (pure Python; no GPU needed).  layout and fuse_dw apply to
+    ShuffleNetV2K plans (default_layout, default_fuse_dw) and are ignored for the others.
+
+    Returns (tensors, ops, info): tensors[i] = (h, w, c_phys); ops are dicts with a 'kind' in
     {'input_conv', 'conv1x1', 'dwconv', 'dw_conv1x1', 'conv', 'maxpool', 'heads'} whose fields are the C ABI
-    arguments."""
-    if plan.get('kind') == 'resnet':
-        return _build_ops_resnet(plan, in_h, in_w)
-    if plan.get('kind') == 'mobilenetv2':
-        return _build_ops_mobilenetv2(plan, in_h, in_w)
-    if plan.get('kind') == 'heads_only':
+    arguments (written by _OpList); info = {'block_outputs': [(tensor, _Layout)], 'feature': (tensor, _Layout)}."""
+    L = _OpList()
+    kind = plan.get('kind')
+    if kind == 'shufflenetv2k':
+        info = _lower_shufflenetv2k(L, plan, in_h, in_w, layout, fuse_dw)
+    elif kind == 'resnet':
+        info = _lower_resnet(L, plan, in_h, in_w)
+    elif kind == 'mobilenetv2':
+        info = _lower_mobilenetv2(L, plan, in_h, in_w)
+    elif kind == 'heads_only':
         # in_h x in_w is the FEATURE map here; the feature tensor is filled through CompiledNet.forward_features
         c_in = int(plan['c_in'])
-        return [(in_h, in_w, pad16(c_in))], [_heads_op(plan['heads'], 0, c_in)], \
-            {'block_outputs': [], 'feature': (0, _Layout(c_in, split=False))}
-    if plan.get('kind') != 'shufflenetv2k':
+        L.heads(plan['heads'], L.tensor(in_h, in_w, pad16(c_in)), c_in)
+        info = {'block_outputs': [], 'feature': (0, _Layout(c_in, split=False))}
+    else:
         raise RuntimeError('unsupported plan kind')
+    return L.tensors, L.ops, info
+
+
+def _lower_shufflenetv2k(L, plan, in_h, in_w, layout, fuse_dw):
     layout = default_layout() if layout is None else layout
     if layout not in ('bins', 'shuffle'):
         raise RuntimeError("layout must be 'bins' or 'shuffle'")
     fuse_dw = default_fuse_dw() if fuse_dw is None else bool(fuse_dw)
-    tensors, ops = [], []
-
-    def tensor(h, w, c):
-        tensors.append((h, w, c))
-        return len(tensors) - 1
-
-    def conv1x1(tin, in_off, in_cols, k_cols, wb, relu, tout, shuffle=None):
-        w, b = wb
-        w = w.reshape(w.shape[0], -1)
-        n, cin = w.shape
-        assert len(in_cols) == cin
-        wp = np.zeros((n, k_cols), dtype=np.float32)
-        wp[:, in_cols] = w
-        s_t, s_off = (-1, 0) if shuffle is None else shuffle
-        ops.append({'kind': 'conv1x1', 'in': tin, 'in_off': in_off, 'k_cols': k_cols, 'n_out': n,
-                    'w': wp, 'b': _f32(b), 'relu': int(relu), 'out': tout, 'out_off': 0,
-                    'shuffle_src': s_t, 'shuffle_off': s_off})
-
-    def conv1x1_scatter(tin, in_cols, k_cols, wb, relu, order, pieces):
-        """1x1 conv whose GEMM columns are the producer's output channels in `order` (-1: padding column, zero
-        weights) and whose column pieces (col0, count, tensor, tensor_col) go to different tensors."""
-        w, b = wb
-        w = w.reshape(w.shape[0], -1)
-        assert len(in_cols) == w.shape[1]
-        real = order >= 0
-        wp = np.zeros((len(order), k_cols), dtype=np.float32)
-        wp[np.ix_(np.nonzero(real)[0], in_cols)] = w[order[real]]
-        bp = np.zeros((len(order),), dtype=np.float32)
-        bp[real] = b[order[real]]
-        ops.append({'kind': 'conv1x1', 'in': tin, 'in_off': 0, 'k_cols': k_cols, 'n_out': len(order),
-                    'w': wp, 'b': bp, 'relu': int(relu), 'out': pieces[0][2], 'out_off': pieces[0][3],
-                    'shuffle_src': -1, 'shuffle_off': 0, 'pieces': [tuple(int(v) for v in pc) for pc in pieces]})
-
-    def dw_conv1x1_scatter(tin, width, dw_wb, kernel, stride, pad, wb, relu, order, pieces):
-        """depthwise kxk on the first len(dw) channels of tin, then the scatter 1x1 conv of conv1x1_scatter on its
-        output -- one fused kernel, no intermediate tensor"""
-        dw_w, dw_b = dw_wb
-        c = dw_w.shape[0]
-        dwp = np.zeros((width, kernel * kernel), dtype=np.float32)
-        dbp = np.zeros((width,), dtype=np.float32)
-        dwp[:c] = dw_w.reshape(c, kernel * kernel)
-        dbp[:c] = dw_b
-        w, b = wb
-        w = w.reshape(w.shape[0], -1)
-        assert w.shape[1] == c
-        real = order >= 0
-        wp = np.zeros((len(order), width), dtype=np.float32)
-        wp[np.ix_(np.nonzero(real)[0], np.arange(c))] = w[order[real]]
-        bp = np.zeros((len(order),), dtype=np.float32)
-        bp[real] = b[order[real]]
-        ops.append({'kind': 'dw_conv1x1', 'in': tin, 'in_off': 0, 'channels': width, 'kernel': kernel,
-                    'stride': stride, 'pad': pad, 'dw_w': dwp, 'dw_b': dbp, 'dw_relu': 0, 'n_out': len(order),
-                    'w': wp, 'b': bp, 'relu': int(relu), 'out': pieces[0][2],
-                    'pieces': [tuple(int(v) for v in pc) for pc in pieces]})
-
-    def dwconv(tin, cols, width, wb, e, tout):
-        """the depthwise conv of block entry e (its kernel, stride, pad and dilation)"""
-        kernel = e['kernel']
-        w, b = wb
-        w = w.reshape(w.shape[0], kernel * kernel)
-        wp = np.zeros((width, kernel * kernel), dtype=np.float32)
-        bp = np.zeros((width,), dtype=np.float32)
-        wp[cols] = w
-        bp[cols] = b
-        op = {'kind': 'dwconv', 'in': tin, 'in_off': 0, 'channels': width, 'kernel': kernel,
-              'stride': e['stride'], 'pad': e['pad'], 'w': wp, 'b': bp, 'relu': 0, 'out': tout, 'out_off': 0}
-        if e.get('dilation', 1) != 1:
-            op['dilation'] = e['dilation']
-        ops.append(op)
-
-    def out_hw(h, w, e):
-        span = e.get('dilation', 1) * (e['kernel'] - 1) + 1
-        return (h + 2 * e['pad'] - span) // e['stride'] + 1, (w + 2 * e['pad'] - span) // e['stride'] + 1
-
-    inp = plan['input']
-    k = inp['w'].shape[-1]
-    h = (in_h + 2 * inp['pad'] - k) // inp['stride'] + 1
-    w = (in_w + 2 * inp['pad'] - k) // inp['stride'] + 1
-    c0 = inp['w'].shape[0]
-    cur = tensor(h, w, pad16(c0))
-    ops.append({'kind': 'input_conv', 'in_h': in_h, 'in_w': in_w, 'kernel': k, 'stride': inp['stride'],
-                'pad': inp['pad'], 'c_out': c0, 'w': _f32(inp['w']), 'b': _f32(inp['b']), 'relu': 1, 'out': cur})
+    tensor = L.tensor
+    cur = L.input_conv(plan['input'], in_h, in_w, ACT_RELU)
     if plan.get('input2') is not None:
         # --shufflenetv2k-input-conv2-stride: 3x3 conv + BN + ReLU on the stem output (basenetworks.py:283-294), an
         # implicit-GEMM conv op
-        e2 = plan['input2']
-        h, w = out_hw(h, w, e2)
-        c0 = e2['w'].shape[0]
-        t2 = tensor(h, w, pad16(c0))
-        ops.append({'kind': 'conv', 'in': cur, 'in_off': 0, 'c_in': e2['w'].shape[1], 'kernel': e2['kernel'],
-                    'stride': e2['stride'], 'pad': e2['pad'], 'dilation': 1, 'n_out': c0, 'w': _f32(e2['w']),
-                    'b': _f32(e2['b']), 'relu': 1, 'out': t2, 'out_off': 0, 'residual': -1, 'residual_off': 0})
-        cur = t2
-    lay = _Layout(c0, split=False)
+        cur = L.conv(cur, plan['input2'], ACT_RELU)
+    h, w, _ = L.tensors[cur]
+    lay = _Layout((plan.get('input2') or plan['input'])['w'].shape[0], split=False)
     stages = list(plan['stages'])
     if plan.get('conv5_stage') is not None:
         # --shufflenetv2k-conv5-as-stage: without a branch1 (stage 4 as wide as conv5) the two blocks continue stage 4
@@ -749,7 +803,7 @@ def build_ops(plan, in_h, in_w, layout=None, fuse_dw=None):
         bf = blocks[0]['b2_pw2'][0].shape[0]
         hp = _branch_pitch(bf)
         e0 = blocks[0]
-        ho, wo = out_hw(h, w, e0)
+        ho, wo = L.out_hw(cur, e0)
         producers, bins, final = _plan_stage_bins(bf, len(blocks))
         t_bin = {t: tensor(ho, wo, pad16(bins[t]['width'])) for t in bins}
         t_bin['final'] = tensor(ho, wo, pad16(final['width']))
@@ -759,16 +813,14 @@ def build_ops(plan, in_h, in_w, layout=None, fuse_dw=None):
 
         cols = lay.cols()
         # block 0, branch1: dw (stride) -> 1x1; branch2: 1x1 -> dw (stride) -> 1x1   (basenetworks.py:200-226)
-        t_a = tensor(ho, wo, lay.width)
-        dwconv(cur, cols, lay.width, e0['b1_dw'], e0, t_a)
-        conv1x1_scatter(t_a, cols, lay.width, e0['b1_pw'], True, producers[0]['order'], pieces_of(0))
+        t_a = L.dwconv(cur, e0['b1_dw'], e0, cols=cols, width=lay.width)
+        L.conv1x1_scatter(t_a, cols, lay.width, e0['b1_pw'], True, producers[0]['order'], pieces_of(0))
         # the tensor in front of the STRIDE-2 depthwise conv gets 128-byte pixels (_dw_in_pitch).  Its producer leaves the padding
         # channels unwritten (rows with a 32-byte hole) and does not pay for writing them.
         t_c = tensor(h, w, _dw_in_pitch(bf))
-        conv1x1(cur, 0, cols, lay.width, e0['b2_pw1'], True, t_c)
-        t_d = tensor(ho, wo, hp)
-        dwconv(t_c, np.arange(bf), hp, e0['b2_dw'], e0, t_d)
-        conv1x1_scatter(t_d, np.arange(bf), hp, e0['b2_pw2'], True, producers[1]['order'], pieces_of(1))
+        L.conv1x1(cur, 0, cols, lay.width, e0['b2_pw1'], True, t_c)
+        t_d = L.dwconv(t_c, e0['b2_dw'], e0, width=hp)
+        L.conv1x1_scatter(t_d, np.arange(bf), hp, e0['b2_pw2'], True, producers[1]['order'], pieces_of(1))
         h, w = ho, wo
         for t, e in enumerate(blocks[1:], start=1):
             assert not e['first'] and e['stride'] == 1 and e['b2_pw2'][0].shape[0] == bf
@@ -776,42 +828,38 @@ def build_ops(plan, in_h, in_w, layout=None, fuse_dw=None):
             wcol = bins[t]['wcol']
             in_cols = np.empty((bf,), dtype=np.int64)
             in_cols[wcol[wcol >= 0]] = np.nonzero(wcol >= 0)[0]
-            width = tensors[t_bin[t]][2]
             t_c = tensor(h, w, hp)          # stride-1 depthwise launches are issue bound: the padding buys nothing there
-            conv1x1(t_bin[t], 0, in_cols, width, e['b2_pw1'], True, t_c)
+            L.conv1x1(t_bin[t], 0, in_cols, L.tensors[t_bin[t]][2], e['b2_pw1'], True, t_c)
             order = producers[t + 1]['order']
             # k_dw_gemm is built for the undilated 5x5, pad 2
             if fuse_dw and e['kernel'] == 5 and e['pad'] == 2 and e.get('dilation', 1) == 1 and len(order) <= 512:
-                dw_conv1x1_scatter(t_c, hp, e['b2_dw'], 5, 1, 2, e['b2_pw2'], True, order, pieces_of(t + 1))
+                L.dw_conv1x1_scatter(t_c, hp, e['b2_dw'], e, e['b2_pw2'], True, order, pieces_of(t + 1))
                 continue
-            t_d = tensor(h, w, hp)
-            dwconv(t_c, np.arange(bf), hp, e['b2_dw'], e, t_d)
-            conv1x1_scatter(t_d, np.arange(bf), hp, e['b2_pw2'], True, order, pieces_of(t + 1))
+            t_d = L.dwconv(t_c, e['b2_dw'], e, width=hp)
+            L.conv1x1_scatter(t_d, np.arange(bf), hp, e['b2_pw2'], True, order, pieces_of(t + 1))
         logical = final['logical']
         phys = np.empty((2 * bf,), dtype=np.int64)
         phys[logical[logical >= 0]] = np.nonzero(logical >= 0)[0]
-        cur, lay = t_bin['final'], _Layout(2 * bf, split=False, phys=phys, width=tensors[t_bin['final']][2])
+        cur, lay = t_bin['final'], _Layout(2 * bf, split=False, phys=phys, width=L.tensors[t_bin['final']][2])
         block_outputs.append((cur, lay))
     for blocks in stages if layout == 'shuffle' else []:
         for e in blocks:
             bf = e['b2_pw2'][0].shape[0]
             hp = pad16(bf)
-            ho, wo = out_hw(h, w, e)
+            ho, wo = L.out_hw(cur, e)
             out_lay = _Layout(2 * bf, split=True)
             t_out = tensor(ho, wo, out_lay.width)
             if e['first']:
                 cols = lay.cols()
                 # branch1: dw (stride) -> 1x1   (basenetworks.py:200-212)
-                t_a = tensor(ho, wo, lay.width)
-                dwconv(cur, cols, lay.width, e['b1_dw'], e, t_a)
+                t_a = L.dwconv(cur, e['b1_dw'], e, cols=cols, width=lay.width)
                 t_b = tensor(ho, wo, hp)
-                conv1x1(t_a, 0, cols, lay.width, e['b1_pw'], True, t_b)
+                L.conv1x1(t_a, 0, cols, lay.width, e['b1_pw'], True, t_b)
                 # branch2: 1x1 -> dw (stride) -> 1x1   (basenetworks.py:214-226)
                 t_c = tensor(h, w, hp)
-                conv1x1(cur, 0, cols, lay.width, e['b2_pw1'], True, t_c)
-                t_d = tensor(ho, wo, hp)
-                dwconv(t_c, np.arange(bf), hp, e['b2_dw'], e, t_d)
-                conv1x1(t_d, 0, np.arange(bf), hp, e['b2_pw2'], True, t_out, shuffle=(t_b, 0))
+                L.conv1x1(cur, 0, cols, lay.width, e['b2_pw1'], True, t_c)
+                t_d = L.dwconv(t_c, e['b2_dw'], e, width=hp)
+                L.conv1x1(t_d, 0, np.arange(bf), hp, e['b2_pw2'], True, t_out, shuffle=(t_b, 0))
             else:
                 assert lay.split and lay.half == bf
                 # x1, x2 = x.chunk(2): x2 is the column window [bf, 2*bf) (basenetworks.py:234-236).  TMA needs a
@@ -820,149 +868,58 @@ def build_ops(plan, in_h, in_w, layout=None, fuse_dw=None):
                 a0 = _view_start(bf)
                 lead = bf - a0
                 t_c = tensor(h, w, hp)
-                conv1x1(cur, a0, lead + np.arange(bf), lead + bf, e['b2_pw1'], True, t_c)
-                t_d = tensor(ho, wo, hp)
-                dwconv(t_c, np.arange(bf), hp, e['b2_dw'], e, t_d)
-                conv1x1(t_d, 0, np.arange(bf), hp, e['b2_pw2'], True, t_out, shuffle=(cur, 0))
+                L.conv1x1(cur, a0, lead + np.arange(bf), lead + bf, e['b2_pw1'], True, t_c)
+                t_d = L.dwconv(t_c, e['b2_dw'], e, width=hp)
+                L.conv1x1(t_d, 0, np.arange(bf), hp, e['b2_pw2'], True, t_out, shuffle=(cur, 0))
             cur, lay, h, w = t_out, out_lay, ho, wo
             block_outputs.append((cur, lay))
     if plan.get('conv5_stage') is not None:
         # the heads read the last stage output as it lies: lay.width columns in physical order
-        ops.append(_heads_op(plan['heads'], cur, lay.width, lay.cols()))
-        return tensors, ops, {'block_outputs': block_outputs, 'feature': (cur, lay)}
-    w5, b5 = plan['conv5']
-    c5 = w5.shape[0]
+        L.heads(plan['heads'], cur, lay.width, lay.cols())
+        return {'block_outputs': block_outputs, 'feature': (cur, lay)}
+    c5 = plan['conv5'][0].shape[0]
     t5 = tensor(h, w, pad16(c5))
-    conv1x1(cur, 0, lay.cols(), lay.width, (w5, b5), True, t5)
-    ops.append(_heads_op(plan['heads'], t5, c5))
-    return tensors, ops, {'block_outputs': block_outputs, 'feature': (t5, _Layout(c5, split=False))}
+    L.conv1x1(cur, 0, lay.cols(), lay.width, plan['conv5'], True, t5)
+    L.heads(plan['heads'], t5, c5)
+    return {'block_outputs': block_outputs, 'feature': (t5, _Layout(c5, split=False))}
 
 
-def _heads_op(heads, t_in, k_cols, cols=None):
-    """cols: the physical column of each logical input channel (None: column c holds channel c)"""
-    w = _f32(np.concatenate([_f32(hd['w']) for hd in heads], axis=0))
-    if cols is not None:
-        wp = np.zeros((w.shape[0], k_cols), dtype=np.float32)
-        wp[:, cols] = w
-        w = wp
-    return {'kind': 'heads', 'in': t_in, 'k_cols': k_cols, 'upsample': int(heads[0].get('upsample', 1)),
-            'n_fields': [hd['n_fields'] for hd in heads], 'n_comp': [hd['n_comp'] for hd in heads],
-            'ops': [o for hd in heads for o in hd['ops']], 'w': w,
-            'b': _f32(np.concatenate([_f32(hd['b']) for hd in heads], axis=0))}
-
-
-def _build_ops_resnet(plan, in_h, in_w):
+def _lower_resnet(L, plan, in_h, in_w):
     """torchvision BasicBlock / Bottleneck (eval): every conv+BN is one implicit-GEMM conv op; the residual
     add and the final ReLU of a block are fused into the epilogue of its last conv."""
-    tensors, ops = [], []
-
-    def tensor(h, w, c):
-        tensors.append((h, w, c))
-        return len(tensors) - 1
-
-    def conv(tin, e, relu, tout, residual=-1):
-        ops.append({'kind': 'conv', 'in': tin, 'in_off': 0, 'c_in': e['w'].shape[1], 'kernel': e['kernel'],
-                    'stride': e['stride'], 'pad': e['pad'], 'dilation': e.get('dilation', 1), 'n_out': e['w'].shape[0],
-                    'w': _f32(e['w']), 'b': _f32(e['b']), 'relu': int(relu), 'out': tout, 'out_off': 0,
-                    'residual': residual, 'residual_off': 0})
-
-    def out_hw(h, w, e):
-        span = e.get('dilation', 1) * (e['kernel'] - 1) + 1
-        return ((h + 2 * e['pad'] - span) // e['stride'] + 1, (w + 2 * e['pad'] - span) // e['stride'] + 1)
-
-    inp = plan['input']
-    k = inp['w'].shape[-1]
-    h = (in_h + 2 * inp['pad'] - k) // inp['stride'] + 1
-    w = (in_w + 2 * inp['pad'] - k) // inp['stride'] + 1
-    c0 = inp['w'].shape[0]
-    cur = tensor(h, w, pad16(c0))
-    ops.append({'kind': 'input_conv', 'in_h': in_h, 'in_w': in_w, 'kernel': k, 'stride': inp['stride'],
-                'pad': inp['pad'], 'c_out': c0, 'w': _f32(inp['w']), 'b': _f32(inp['b']), 'relu': 1, 'out': cur})
+    cur = L.input_conv(plan['input'], in_h, in_w, ACT_RELU)
     if plan.get('pool') is not None:
-        s = plan['pool']['stride']
-        h, w = (h - 1) // s + 1, (w - 1) // s + 1          # 3x3, padding 1
-        t_pool = tensor(h, w, pad16(c0))
-        ops.append({'kind': 'maxpool', 'in': cur, 'in_off': 0, 'channels': c0, 'stride': s, 'out': t_pool, 'out_off': 0})
-        cur = t_pool
+        cur = L.maxpool(cur, plan['input']['w'].shape[0], plan['pool']['stride'])
     if plan.get('input2') is not None:
-        e2 = plan['input2']
-        h, w = out_hw(h, w, e2)
-        t2 = tensor(h, w, pad16(e2['w'].shape[0]))
-        conv(cur, e2, True, t2)
-        cur, c0 = t2, e2['w'].shape[0]
-    c_cur = c0
+        cur = L.conv(cur, plan['input2'], ACT_RELU)
     block_outputs = []
     for e in plan['blocks']:
-        identity = cur
-        hh, ww = h, w
-        t_in = cur
-        if e['downsample'] is not None:
-            ds = e['downsample']
-            dh, dw_ = out_hw(h, w, ds)
-            identity = tensor(dh, dw_, pad16(ds['w'].shape[0]))
-            conv(cur, ds, False, identity)
-        n_convs = len(e['convs'])
-        for ci, ce in enumerate(e['convs']):
-            oh, ow = out_hw(hh, ww, ce)
-            t_out = tensor(oh, ow, pad16(ce['w'].shape[0]))
-            last = ci == n_convs - 1
-            conv(t_in, ce, True, t_out, residual=identity if last else -1)
-            t_in, hh, ww = t_out, oh, ow
-        cur, h, w, c_cur = t_in, hh, ww, e['convs'][-1]['w'].shape[0]
-        block_outputs.append((cur, _Layout(c_cur, split=False)))
-    ops.append(_heads_op(plan['heads'], cur, c_cur))
-    return tensors, ops, {'block_outputs': block_outputs, 'feature': (cur, _Layout(c_cur, split=False))}
+        identity = cur if e['downsample'] is None else L.conv(cur, e['downsample'], ACT_NONE)
+        for i, ce in enumerate(e['convs']):
+            cur = L.conv(cur, ce, ACT_RELU, residual=identity if i == len(e['convs']) - 1 else -1)
+        block_outputs.append((cur, _Layout(e['convs'][-1]['w'].shape[0], split=False)))
+    c = plan['blocks'][-1]['convs'][-1]['w'].shape[0]
+    L.heads(plan['heads'], cur, c)
+    return {'block_outputs': block_outputs, 'feature': (cur, _Layout(c, split=False))}
 
 
-def _build_ops_mobilenetv2(plan, in_h, in_w):
-    """torchvision InvertedResidual (eval): the expand 1x1 and the linear projection are pointwise conv ops (the
+def _lower_mobilenetv2(L, plan, in_h, in_w):
+    """torchvision InvertedResidual (eval): the expand 1x1 and the linear projection are implicit-GEMM conv ops (the
     projection adds the block input in its epilogue), the 3x3 depthwise conv a dwconv op; every activation is ReLU6.
     Tensors are padded to 16 channels (24 -> 32)."""
-    tensors, ops = [], []
-
-    def tensor(h, w, c):
-        tensors.append((h, w, c))
-        return len(tensors) - 1
-
-    def conv(tin, e, act, tout, residual=-1):
-        ops.append({'kind': 'conv', 'in': tin, 'in_off': 0, 'c_in': e['w'].shape[1], 'kernel': e['kernel'],
-                    'stride': e['stride'], 'pad': e['pad'], 'dilation': 1, 'n_out': e['w'].shape[0],
-                    'w': _f32(e['w']), 'b': _f32(e['b']), 'relu': act, 'out': tout, 'out_off': 0,
-                    'residual': residual, 'residual_off': 0})
-
-    inp = plan['input']
-    k, s, p = inp['kernel'], inp['stride'], inp['pad']
-    h, w = (in_h + 2 * p - k) // s + 1, (in_w + 2 * p - k) // s + 1
-    c = inp['w'].shape[0]
-    cur = tensor(h, w, pad16(c))
-    ops.append({'kind': 'input_conv', 'in_h': in_h, 'in_w': in_w, 'kernel': k, 'stride': s, 'pad': p, 'c_out': c,
-                'w': _f32(inp['w']), 'b': _f32(inp['b']), 'relu': ACT_RELU6, 'out': cur})
+    cur = L.input_conv(plan['input'], in_h, in_w, ACT_RELU6)
     block_outputs = []
     for e in plan['blocks']:
         x = cur
         if e['expand'] is not None:
-            c = e['expand']['w'].shape[0]
-            t_e = tensor(h, w, pad16(c))
-            conv(cur, e['expand'], ACT_RELU6, t_e)
-            cur = t_e
-        dw = e['dw']
-        st = dw['stride']
-        ho, wo = (h + 2 * dw['pad'] - 3) // st + 1, (w + 2 * dw['pad'] - 3) // st + 1
-        t_d = tensor(ho, wo, pad16(c))
-        ops.append({'kind': 'dwconv', 'in': cur, 'in_off': 0, 'channels': c, 'kernel': 3, 'stride': st,
-                    'pad': dw['pad'], 'w': _f32(dw['w'].reshape(c, 9)), 'b': _f32(dw['b']), 'relu': ACT_RELU6,
-                    'out': t_d, 'out_off': 0})
-        h, w = ho, wo
-        c = e['project']['w'].shape[0]
-        t_p = tensor(h, w, pad16(c))
-        conv(t_d, e['project'], ACT_NONE, t_p, residual=x if e['residual'] else -1)
-        cur = t_p
-        block_outputs.append((cur, _Layout(c, split=False)))
+            cur = L.conv(cur, e['expand'], ACT_RELU6)
+        cur = L.dwconv(cur, (e['dw']['w'], e['dw']['b']), e['dw'], ACT_RELU6)
+        cur = L.conv(cur, e['project'], ACT_NONE, residual=x if e['residual'] else -1)
+        block_outputs.append((cur, _Layout(e['project']['w'].shape[0], split=False)))
     c = plan['last']['w'].shape[0]
-    t_l = tensor(h, w, pad16(c))
-    conv(cur, plan['last'], ACT_RELU6, t_l)
-    ops.append(_heads_op(plan['heads'], t_l, c))
-    return tensors, ops, {'block_outputs': block_outputs, 'feature': (t_l, _Layout(c, split=False))}
+    cur = L.conv(cur, plan['last'], ACT_RELU6)
+    L.heads(plan['heads'], cur, c)
+    return {'block_outputs': block_outputs, 'feature': (cur, _Layout(c, split=False))}
 
 
 class CompiledNet:
@@ -973,10 +930,7 @@ class CompiledNet:
         self.device = int(device)
         self.max_batch = int(max_batch)
         self.in_h, self.in_w = int(in_h), int(in_w)
-        if plan.get('kind') == 'shufflenetv2k':
-            self.tensor_shapes, ops, self.info = build_ops(plan, self.in_h, self.in_w, layout=layout, fuse_dw=fuse_dw)
-        else:
-            self.tensor_shapes, ops, self.info = build_ops(plan, self.in_h, self.in_w)
+        self.tensor_shapes, ops, self.info = build_ops(plan, self.in_h, self.in_w, layout=layout, fuse_dw=fuse_dw)
         self.op_desc = [{k: v for k, v in o.items() if not isinstance(v, np.ndarray)} for o in ops]
         self.handle = ctypes.c_void_p()
         _lib.check(self.lib.pifpaf_net_create(ctypes.byref(self.handle), self.device, self.max_batch))

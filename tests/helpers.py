@@ -82,3 +82,17 @@ def assert_annotations_close(got, want, what=''):
 def reference_outputs():
     """tests/golden/reference_outputs.npz: what the unmodified reference computed for the cases of oracle/make_golden.py"""
     return np.load(os.path.join(GOLDEN_DIR, 'reference_outputs.npz'))
+
+
+def assert_taps_match_emulation(net, ops, emu_acts, batch, what=''):
+    """After a forward of `net`: every tensor an op of `ops` writes (the heads aside) against the activations of the bf16
+    emulation (ops_emulator.run_ops with bf16=True), to 3e-2 of the emulated tensor's largest magnitude."""
+    for o in ops:
+        if o['kind'] == 'heads':
+            continue
+        for t_id in sorted({pc[2] for pc in o['pieces']}) if 'pieces' in o else [o['out']]:
+            got = net.tap(t_id, batch)
+            ref = emu_acts[t_id].numpy()
+            scale = max(float(np.abs(ref).max()), 1e-6)
+            assert float(np.abs(got - ref).max()) / scale < 3e-2, \
+                (what, o['kind'], t_id, o.get('kernel'), o.get('stride'), o.get('dilation'))

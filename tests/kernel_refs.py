@@ -36,8 +36,8 @@ def out_hw(h, w, kernel, stride, pad):
     return (h + 2 * pad - kernel) // stride + 1, (w + 2 * pad - kernel) // stride + 1
 
 
-def conv_ref(x, w, b, stride, pad, groups=1):
-    """x [B, H, W, C] (NHWC), w [N, C / groups, k, k] (torch layout), b [N] or None
+def conv_ref(x, w, b, stride, pad, groups=1, dilation=1):
+    """x [B, H, W, C] (NHWC), w [N, C / groups, k, k] (torch layout), b [N] or None, taps `dilation` pixels apart
     -> (y, mag): y = conv + b in float64 [B, Ho, Wo, N], mag = sum |x w| + |b| (the scale of the accumulation error)."""
     x = np.asarray(x, dtype=np.float64)
     w = np.asarray(w, dtype=np.float64)
@@ -45,14 +45,15 @@ def conv_ref(x, w, b, stride, pad, groups=1):
     N, cg, k, _ = w.shape
     assert C == cg * groups and N % groups == 0
     ng = N // groups
-    Ho, Wo = out_hw(H, W, k, stride, pad)
+    Ho, Wo = out_hw(H, W, (k - 1) * dilation + 1, stride, pad)
     xp = np.zeros((B, H + 2 * pad, W + 2 * pad, C))
     xp[:, pad:pad + H, pad:pad + W] = x
     y = np.zeros((B, Ho, Wo, N))
     mag = np.zeros((B, Ho, Wo, N))
     for ky in range(k):
         for kx in range(k):
-            xs = xp[:, ky:ky + stride * (Ho - 1) + 1:stride, kx:kx + stride * (Wo - 1) + 1:stride]
+            y0, x0 = ky * dilation, kx * dilation
+            xs = xp[:, y0:y0 + stride * (Ho - 1) + 1:stride, x0:x0 + stride * (Wo - 1) + 1:stride]
             if groups == C and ng == 1:                  # depthwise: elementwise per channel
                 y += xs * w[:, 0, ky, kx]
                 mag += np.abs(xs) * np.abs(w[:, 0, ky, kx])
@@ -74,14 +75,18 @@ def bf16_bound(ref, mag, k_terms):
     return U_BF16 * np.abs(ref) + (k_terms + 2) * U_F32 * mag
 
 
-def epilogue(y, mag, relu, res=None):
-    """+ residual, then ReLU (the order of the torchvision block tail); ReLU is 1-Lipschitz, the bound carries over"""
+def epilogue(y, mag, code, res=None):
+    """+ residual, then the activation of code (0 none, 1 ReLU, 2 ReLU6; the order of the torchvision block tail); both
+    activations are 1-Lipschitz, the bound carries over"""
+    assert code in (0, 1, 2), code
     if res is not None:
         res = np.asarray(res, dtype=np.float64)
         y = y + res
         mag = mag + np.abs(res)
-    if relu:
+    if code >= 1:
         y = np.maximum(y, 0.0)
+    if code == 2:
+        y = np.minimum(y, 6.0)
     return y, mag
 
 
@@ -109,21 +114,30 @@ def normalise_u8(images_hwc, mean, std):
     return (x - np.asarray(mean, dtype=np.float32)) / np.asarray(std, dtype=np.float32)
 
 
-def heads_ref(a, w, b, n_fields, n_comp, comp_ops):
-    """CompositeField4 eval epilogue (upsample 1) on a [B, h, w, K] feature map with weights w [N, K]:
-    -> per head (ref, bound) arrays [B, F, comp, h, w] in float64.  The bound pushes the accumulation error through
+def heads_ref(a, w, b, n_fields, n_comp, comp_ops, upsample=1):
+    """CompositeField4 eval epilogue on a [B, h, w, K] feature map with weights w [N, K]: PixelShuffle(upsample) and the
+    crop of (up - 1) // 2 low and ceil((up - 1) / 2) high cells, then the component ops with the index adds on the output
+    grid -> per head (ref, bound) arrays [B, F, comp, h', w'] in float64.  The bound pushes the accumulation error through
     the activation (sigmoid: Lipschitz 1/4, softplus: 1) and adds a few f32 ulp for expf / log1pf / the index add."""
     a = np.asarray(a, dtype=np.float64)
     w = np.asarray(w, dtype=np.float64)
     B, h, wd, K = a.shape
+    up = upsample
+    lo, hi = (up - 1) // 2, up // 2
     y = a @ w.T + b
     acc = (K + 2) * U_F32 * (np.abs(a) @ np.abs(w).T + np.abs(b))
-    xs = np.arange(wd, dtype=np.float64).reshape(1, 1, wd)
-    ys = np.arange(h, dtype=np.float64).reshape(1, h, 1)
+
+    def fields(t, col, nf, nc):
+        """conv channels (field, comp, sub-row, sub-column) -> [B, F, comp, h up, w up] (PixelShuffle), cropped"""
+        t = t[..., col * up * up:(col + nf * nc) * up * up].reshape(B, h, wd, nf, nc, up, up)
+        t = t.transpose(0, 3, 4, 1, 5, 2, 6).reshape(B, nf, nc, h * up, wd * up)
+        return t[..., lo:h * up - hi, lo:wd * up - hi].copy()
+
     out, col, op_off = [], 0, 0
     for nf, nc in zip(n_fields, n_comp):
-        v = y[..., col:col + nf * nc].reshape(B, h, wd, nf, nc).transpose(0, 3, 4, 1, 2).copy()
-        e = acc[..., col:col + nf * nc].reshape(B, h, wd, nf, nc).transpose(0, 3, 4, 1, 2).copy()
+        v, e = fields(y, col, nf, nc), fields(acc, col, nf, nc)
+        xs = np.arange(v.shape[-1], dtype=np.float64).reshape(1, 1, -1)
+        ys = np.arange(v.shape[-2], dtype=np.float64).reshape(1, -1, 1)
         for c in range(nc):
             op = comp_ops[op_off + c]
             if op == OP_SIGMOID:
@@ -152,6 +166,77 @@ def worst_ratio(got, ref, bound):
     err = np.abs(got - ref)
     err[~np.isfinite(got)] = np.inf
     return float((err / np.maximum(bound, 1e-300)).max()) if err.size else 0.0
+
+
+def maxpool_ref(x, stride):
+    """3x3 max pool with padding 1 on x [B, H, W, C] (the values themselves: a max rounds nothing)"""
+    B, H, W, C = x.shape
+    Ho, Wo = out_hw(H, W, 3, stride, 1)
+    xp = np.full((B, H + 2, W + 2, C), -np.inf, dtype=x.dtype)
+    xp[:, 1:1 + H, 1:1 + W] = x
+    return np.max([xp[:, ky:ky + stride * (Ho - 1) + 1:stride, kx:kx + stride * (Wo - 1) + 1:stride]
+                   for ky in range(3) for kx in range(3)], axis=0)
+
+
+def op_ref(o, taps, heads, images, batch):
+    """float64 reference of one op of network.build_ops on the tensors the GPU fed it -> (kind, worst err / bound).
+    taps: tensor -> [>= batch, h, w, c_phys] after the forward, heads: the head outputs, images [B, 3, H, W] f32.
+    The max pool is compared exactly (ratio 0 or inf)."""
+    kind = o['kind']
+
+    def a_in(t, off, n):
+        return taps[t][:batch, ..., off:off + n]
+
+    def out(n, t=None, off=None):
+        t = o['out'] if t is None else t
+        off = o.get('out_off', 0) if off is None else off
+        return taps[t][:batch, ..., off:off + n]
+
+    if kind == 'heads':
+        refs = heads_ref(a_in(o['in'], 0, o['k_cols']), bf16_round(o['w']), o['b'], o['n_fields'], o['n_comp'],
+                         o['ops'], o['upsample'])
+        return 'heads', max(worst_ratio(hb[:batch], r, bd) for hb, (r, bd) in zip(heads, refs))
+    if kind == 'input_conv':
+        ref, mag = epilogue(*conv_ref(images[:batch].transpose(0, 2, 3, 1), o['w'], o['b'], o['stride'], o['pad']),
+                            o['relu'])
+        return kind, worst_ratio(out(o['c_out']), ref, bf16_bound(ref, mag, 3 * o['kernel'] ** 2))
+    if kind == 'maxpool':
+        C = o['channels']
+        return kind, 0.0 if np.array_equal(out(C), maxpool_ref(a_in(o['in'], o['in_off'], C), o['stride'])) else np.inf
+    if kind == 'dw_conv1x1':
+        C = o['channels']
+        ref, bound = dw_gemm_ref(a_in(o['in'], o['in_off'], C), o['dw_w'], o['dw_b'], o['dw_relu'], bf16_round(o['w']),
+                                 o['b'], o['relu'])
+        return 'dw_gemm', max(worst_ratio(out(cnt, t, col), ref[..., c0:c0 + cnt], bound[..., c0:c0 + cnt])
+                              for c0, cnt, t, col in o['pieces'])
+    if kind == 'dwconv':
+        C, k, d = o['channels'], o['kernel'], o.get('dilation', 1)
+        ref, mag = epilogue(*conv_ref(a_in(o['in'], o['in_off'], C), o['w'].reshape(C, 1, k, k), o['b'], o['stride'],
+                                      o['pad'], groups=C, dilation=d), o['relu'])
+        label = 'dwconv k%d s%d' % (k, o['stride']) + (' d%d' % d if d != 1 else '')
+        return label, worst_ratio(out(C), ref, bf16_bound(ref, mag, k * k))
+    if kind == 'conv':
+        k, d = o['kernel'], o['dilation']
+        ref, mag = conv_ref(a_in(o['in'], o['in_off'], o['c_in']), bf16_round(o['w']), o['b'], o['stride'], o['pad'],
+                            dilation=d)
+        res = None if o['residual'] < 0 else a_in(o['residual'], o['residual_off'], o['n_out'])
+        ref, mag = epilogue(ref, mag, o['relu'], res)
+        label = 'conv k%d' % k + (' d%d' % d if d != 1 else '')
+        return label, worst_ratio(out(o['n_out']), ref, bf16_bound(ref, mag, o['c_in'] * k * k))
+    assert kind == 'conv1x1', kind
+    K, N = o['k_cols'], o['n_out']
+    ref, mag = conv_ref(a_in(o['in'], o['in_off'], K), bf16_round(o['w'])[:, :, None, None], o['b'], 1, 0)
+    ref, mag = epilogue(ref, mag, o['relu'])
+    bound = bf16_bound(ref, mag, K)
+    if 'pieces' in o:
+        return 'gemm scatter', max(worst_ratio(out(cnt, t, col), ref[..., c0:c0 + cnt], bound[..., c0:c0 + cnt])
+                                   for c0, cnt, t, col in o['pieces'])
+    if o['shuffle_src'] >= 0:
+        o_all = out(2 * N, off=0)
+        assert np.array_equal(o_all[..., 0::2], a_in(o['shuffle_src'], o['shuffle_off'], N)), \
+            'pass-through channels of the fused shuffle'
+        return 'gemm shuffle', worst_ratio(o_all[..., 1::2], ref, bound)
+    return 'gemm plain', worst_ratio(out(N), ref, bound)
 
 
 def fused_rings(channels, n_out):

@@ -1,15 +1,11 @@
-"""Test infrastructure: fp32 PyTorch restatement of the reference's MobileNetV2 base network and a CPU interpreter of
-the op list openpifpaf_b200.network.build_ops emits for it (paths relative to the reference's src/openpifpaf/):
+"""Test infrastructure: fp32 PyTorch restatement of the reference's MobileNetV2 base network and counters of the op list
+openpifpaf_b200.network.build_ops emits for it (paths relative to the reference's src/openpifpaf/):
 
   MobileNetV2          network/basenetworks.py:407-417 (backbone = torchvision mobilenet_v2().features, stride 32)
 
 The module attribute names and state_dict keys equal the reference's, so its own module loads these weights
 unchanged (tests/test_mobilenetv2.py compares the two).  Torchvision is always asked for weights=None."""
-import math
-
-import numpy as np
 import torch
-import torch.nn.functional as F
 
 import det_models
 from openpifpaf_b200 import constants
@@ -79,77 +75,6 @@ def reference_features(x, oracle_base):
 
 def golden_input():
     return torch.randn(1, 3, 49, 65, generator=torch.Generator().manual_seed(23))
-
-
-def act(y, code):
-    """activation codes of include/pifpaf_b200.h: 0 none, 1 ReLU, 2 ReLU6"""
-    if code == 1:
-        return F.relu(y)
-    if code == 2:
-        return torch.clamp(y, 0.0, 6.0)
-    assert code == 0, code
-    return y
-
-
-def run_ops(tensors, ops, images, bf16=False):
-    """images [B,3,H,W] float32 -> (head outputs [B,F,comp,h,w], activations [B,h,w,c_phys]), executing the op kinds of
-    a MobileNetV2 plan (input_conv, conv, dwconv, heads) as include/pifpaf_b200.h documents them.  With ``bf16`` the
-    activations and the conv / head weights are rounded to bf16 where the kernels round them (stem and depthwise
-    weights stay f32)."""
-    B = images.shape[0]
-    acts = [torch.zeros((B, h, w, c), dtype=torch.float32) for (h, w, c) in tensors]
-
-    def q(x):
-        return x.to(torch.bfloat16).to(torch.float32) if bf16 else x
-
-    def nchw(o, c):
-        return acts[o['in']][..., o['in_off']:o['in_off'] + c].permute(0, 3, 1, 2)
-
-    heads_out = None
-    for o in ops:
-        kind = o['kind']
-        if kind == 'input_conv':
-            y = F.conv2d(images, torch.from_numpy(o['w']), torch.from_numpy(o['b']), o['stride'], o['pad'])
-            acts[o['out']][..., :o['c_out']] = q(act(y, o['relu']).permute(0, 2, 3, 1))
-        elif kind == 'conv':
-            y = F.conv2d(nchw(o, o['c_in']), q(torch.from_numpy(o['w'])), torch.from_numpy(o['b']), o['stride'],
-                         o['pad'], o['dilation']).permute(0, 2, 3, 1)
-            if o['residual'] >= 0:
-                y = y + acts[o['residual']][..., o['residual_off']:o['residual_off'] + o['n_out']]
-            acts[o['out']][..., o['out_off']:o['out_off'] + o['n_out']] = q(act(y, o['relu']))
-        elif kind == 'dwconv':
-            c, k = o['channels'], o['kernel']
-            w = torch.from_numpy(o['w']).reshape(c, 1, k, k)
-            y = F.conv2d(nchw(o, c), w, torch.from_numpy(o['b']), o['stride'], o['pad'], groups=c)
-            acts[o['out']][..., o['out_off']:o['out_off'] + c] = q(act(y, o['relu']).permute(0, 2, 3, 1))
-        elif kind == 'heads':
-            up = o['upsample']
-            y = acts[o['in']][..., :o['k_cols']] @ q(torch.from_numpy(o['w'])).t() + torch.from_numpy(o['b'])
-            heads_out, col, op_off = [], 0, 0
-            for nf, nc in zip(o['n_fields'], o['n_comp']):
-                t = y[..., col * up * up:(col + nf * nc) * up * up].permute(0, 3, 1, 2)
-                if up > 1:
-                    lo, hi = (up - 1) // 2, math.ceil((up - 1) / 2)
-                    t = F.pixel_shuffle(t, up)
-                    t = t[:, :, lo:t.shape[2] - hi, lo:t.shape[3] - hi]
-                _, _, h, w = t.shape
-                t = t.reshape(B, nf, nc, h, w).clone()
-                for c_i in range(nc):
-                    op = o['ops'][op_off + c_i]
-                    if op == 1:
-                        t[:, :, c_i] = torch.sigmoid(t[:, :, c_i])
-                    elif op == 2:
-                        t[:, :, c_i] += torch.arange(w, dtype=torch.float32)
-                    elif op == 3:
-                        t[:, :, c_i] += torch.arange(h, dtype=torch.float32).view(h, 1)
-                    elif op == 4:
-                        t[:, :, c_i] = F.softplus(t[:, :, c_i])
-                heads_out.append(t)
-                col += nf * nc
-                op_off += nc
-        else:
-            raise ValueError(kind)
-    return heads_out, acts
 
 
 def op_counts(ops):

@@ -8,12 +8,10 @@ constructor and CLI, next to oracle/net_oracle.py (paths relative to the referen
     --shufflenetv2k-conv5-as-stage             conv5 = two InvertedResidualK blocks instead of a 1x1 conv
 
 Module attribute names and state_dict keys equal the reference's, so its own modules load these weights unchanged
-(tests/test_shufflenetv2k_variants.py compares the two).  Also a CPU interpreter of the op list build_ops emits for
-these models: tests/ops_emulator.py with each dilated depthwise op restated as the equivalent undilated op."""
+(tests/test_shufflenetv2k_variants.py compares the two)."""
 import torch
 
 import det_models
-import ops_emulator
 from openpifpaf_b200 import constants
 from oracle import net_oracle
 
@@ -154,25 +152,3 @@ def reference_features(variant, x, oracle_base):
 
 def golden_input():
     return torch.randn(1, 3, 49, 65, generator=torch.Generator().manual_seed(23))
-
-
-def undilated_ops(ops):
-    """the op list with every dilated depthwise op replaced by the same op with its kernel spread out:
-    (k - 1) * d + 1 taps per side, zero between the real ones -- the same sums (zero terms added)"""
-    out = []
-    for o in ops:
-        d = o.get('dilation', 1)
-        if o['kind'] == 'dwconv' and d != 1:
-            k, c = o['kernel'], o['channels']
-            kd = (k - 1) * d + 1
-            w = torch.zeros((c, kd, kd), dtype=torch.float32)
-            w[:, ::d, ::d] = torch.from_numpy(o['w']).reshape(c, k, k)
-            o = dict(o, kernel=kd, w=w.reshape(c, kd * kd).numpy())
-            del o['dilation']
-        out.append(o)
-    return out
-
-
-def run_ops(tensors, ops, images, bf16=False):
-    """tests/ops_emulator.run_ops on ops that may hold dilated depthwise convs"""
-    return ops_emulator.run_ops(tensors, undilated_ops(ops), images, bf16=bf16)

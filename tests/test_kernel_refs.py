@@ -10,10 +10,10 @@ from openpifpaf_b200 import network
 from oracle import net_oracle
 
 
-def torch_conv(x_nhwc, w, b, stride, pad, groups=1):
+def torch_conv(x_nhwc, w, b, stride, pad, groups=1, dilation=1):
     x = torch.from_numpy(np.asarray(x_nhwc, dtype=np.float64)).permute(0, 3, 1, 2)
     y = F.conv2d(x, torch.from_numpy(np.asarray(w, dtype=np.float64)),
-                 None if b is None else torch.from_numpy(np.asarray(b, dtype=np.float64)), stride, pad, groups=groups)
+                 None if b is None else torch.from_numpy(np.asarray(b, dtype=np.float64)), stride, pad, dilation, groups)
     return y.permute(0, 2, 3, 1).numpy()
 
 
@@ -38,6 +38,51 @@ def test_conv_ref_matches_torch_float64(k, stride, pad, c_in, n_out, groups):
     np.testing.assert_allclose(y, want, rtol=1e-12, atol=1e-12)
     # mag is the same conv on absolute values
     np.testing.assert_allclose(mag, torch_conv(np.abs(x), np.abs(w), np.abs(b), stride, pad, groups), rtol=1e-12)
+
+
+@pytest.mark.parametrize('k,stride,pad,dilation,c_in,n_out,groups', [
+    (3, 1, 2, 2, 8, 6, 1),      # ResNet block 5 under --resnet-block5-dilation 2
+    (3, 1, 4, 4, 5, 7, 1),      # dilation 4: most taps in the padding
+    (3, 1, 0, 2, 6, 4, 1),      # no padding: the output shrinks by d (k - 1)
+    (5, 1, 4, 2, 12, 12, 12),   # depthwise 5x5, dilation 2 (--shufflenetv2k-stage4-dilation 2)
+    (5, 1, 6, 3, 9, 9, 9),      # depthwise, dilation 3
+    (3, 2, 2, 2, 4, 4, 4),      # strided (the kernels refuse it; the reference is still a conv)
+])
+def test_conv_ref_dilated_matches_torch_float64(k, stride, pad, dilation, c_in, n_out, groups):
+    rng = np.random.default_rng(k * 100 + c_in + dilation)
+    x = rng.standard_normal((2, 13, 11, c_in))
+    w = rng.standard_normal((n_out, c_in // groups, k, k))
+    b = rng.standard_normal(n_out)
+    y, mag = kr.conv_ref(x, w, b, stride, pad, groups=groups, dilation=dilation)
+    want = torch_conv(x, w, b, stride, pad, groups, dilation)
+    assert y.shape == want.shape
+    np.testing.assert_allclose(y, want, rtol=1e-12, atol=1e-12)
+    np.testing.assert_allclose(mag, torch_conv(np.abs(x), np.abs(w), np.abs(b), stride, pad, groups, dilation), rtol=1e-12)
+
+
+@pytest.mark.parametrize('code', [0, 1, 2])
+def test_epilogue_activation_codes(code):
+    """codes 0 / 1 / 2 of include/pifpaf_b200.h (none, ReLU, ReLU6) after the residual add"""
+    rng = np.random.default_rng(7)
+    y = rng.uniform(-4.0, 10.0, (2, 5, 6, 8))
+    res = rng.standard_normal((2, 5, 6, 8))
+    mag = np.abs(y)
+    got, got_mag = kr.epilogue(y, mag, code, res)
+    t = torch.from_numpy(y + res)
+    want = [t, F.relu(t), F.relu6(t)][code].numpy()
+    np.testing.assert_array_equal(got, want)
+    np.testing.assert_array_equal(got_mag, mag + np.abs(res))
+    if code == 2:
+        assert (got == 6).any() and (got == 0).any()
+
+
+def test_maxpool_ref_matches_torch():
+    rng = np.random.default_rng(8)
+    for stride in (1, 2):
+        for H, W in ((1, 1), (2, 3), (9, 8), (10, 7)):
+            x = rng.standard_normal((2, H, W, 5))
+            want = F.max_pool2d(torch.from_numpy(x).permute(0, 3, 1, 2), 3, stride, 1).permute(0, 2, 3, 1).numpy()
+            np.testing.assert_array_equal(kr.maxpool_ref(x, stride), want)
 
 
 def test_residual_epilogue_adds_before_relu():
@@ -69,20 +114,17 @@ def test_dw_gemm_ref_is_depthwise_then_pointwise():
     assert (bound >= kr.U_BF16 * (np.abs(d) @ np.abs(w).T) - 1e-12).all()
 
 
-def test_heads_ref_matches_torch_ops():
-    rng = np.random.default_rng(3)
-    B, h, w, K = 2, 5, 7, 24
-    n_fields, n_comp = [3, 2], [5, 9]
-    comp_ops = [1, 2, 3, 4, 0] + [1, 2, 3, 0, 0, 4, 4, 1, 0]
-    N = sum(f * c for f, c in zip(n_fields, n_comp))
-    a = rng.standard_normal((B, h, w, K))
-    wt = rng.standard_normal((N, K)) * 3
-    bias = rng.standard_normal(N)
-    got = kr.heads_ref(a, wt, bias, n_fields, n_comp, comp_ops)
-    y = torch.from_numpy(a) @ torch.from_numpy(wt).T + torch.from_numpy(bias)
-    col, off = 0, 0
-    for (v, e), nf, nc in zip(got, n_fields, n_comp):
-        t = y[..., col:col + nf * nc].reshape(B, h, w, nf, nc).permute(0, 3, 4, 1, 2).clone()
+def torch_heads(a, wt, bias, n_fields, n_comp, comp_ops, up):
+    """the heads epilogue in torch float64: conv as a matmul, PixelShuffle(up), the reference's crop, the component ops"""
+    B = a.shape[0]
+    y = (torch.from_numpy(a) @ torch.from_numpy(wt).T + torch.from_numpy(bias)).permute(0, 3, 1, 2)
+    out, col, off = [], 0, 0
+    for nf, nc in zip(n_fields, n_comp):
+        t = torch.nn.PixelShuffle(up)(y[:, col * up * up:(col + nf * nc) * up * up])
+        lo, hi = (up - 1) // 2, int(np.ceil((up - 1) / 2.0))
+        t = t[:, :, lo:t.shape[2] - hi, lo:t.shape[3] - hi]
+        h, w = t.shape[2:]
+        t = t.reshape(B, nf, nc, h, w).clone()
         for c in range(nc):
             op = comp_ops[off + c]
             if op == 1:
@@ -93,11 +135,37 @@ def test_heads_ref_matches_torch_ops():
                 t[:, :, c] += torch.arange(h, dtype=torch.float64).view(1, h, 1)
             elif op == 4:
                 t[:, :, c] = F.softplus(t[:, :, c])
-        # torch's softplus returns x above 20 (threshold): log1p(exp(-20)) = 2e-9 from the exact value
-        np.testing.assert_allclose(v, t.numpy(), rtol=1e-12, atol=3e-9)
-        assert (e > 0).all()
+        out.append(t.numpy())
         col += nf * nc
         off += nc
+    return out
+
+
+def check_heads_ref(up):
+    rng = np.random.default_rng(3)
+    B, h, w, K = 2, 5, 7, 24
+    n_fields, n_comp = [3, 2], [5, 9]
+    comp_ops = [1, 2, 3, 4, 0] + [1, 2, 3, 0, 0, 4, 4, 1, 0]
+    N = sum(f * c for f, c in zip(n_fields, n_comp)) * up * up
+    a = rng.standard_normal((B, h, w, K))
+    wt = rng.standard_normal((N, K)) * 3
+    bias = rng.standard_normal(N)
+    got = kr.heads_ref(a, wt, bias, n_fields, n_comp, comp_ops, up)
+    for (v, e), want in zip(got, torch_heads(a, wt, bias, n_fields, n_comp, comp_ops, up)):
+        assert v.shape == want.shape == (B, v.shape[1], v.shape[2], h * up - (up - 1), w * up - (up - 1))
+        # torch's softplus returns x above 20 (threshold): log1p(exp(-20)) = 2e-9 from the exact value
+        np.testing.assert_allclose(v, want, rtol=1e-12, atol=3e-9)
+        assert (e > 0).all()
+
+
+def test_heads_ref_matches_torch_ops():
+    check_heads_ref(1)
+
+
+@pytest.mark.parametrize('up', [2, 3])
+def test_heads_ref_upsampled_matches_torch_ops(up):
+    """upsample_stride > 1 (heads.py:307-343): PixelShuffle, the crop, and the index adds on the output grid"""
+    check_heads_ref(up)
 
 
 def test_bf16_round_is_torch_round_to_nearest_even():
@@ -198,3 +266,34 @@ def test_fused_ring_plan_mirror_matches_net_cu():
     ]:
         assert line in flat, line
     assert kr.fused_rings(176, 176) == (3, 2) and kr.fused_rings(1024, 192) == (1, 1)
+
+
+def _emulation_plan(name):
+    import det_models
+    import mobilenetv2_models as mm
+    import shufflenetv2k_models as sm
+    if name == 'mobilenetv2':
+        return network.plan_from_shell(mm.make_pose_shell(seed=0))
+    if name in det_models.VARIANTS:
+        return network.plan_from_shell(det_models.make_variant_shell(name, seed=0))
+    return network.plan_from_shell(sm.make_pose_shell(name, 'tiny', seed=0))
+
+
+@pytest.mark.parametrize('name,layout,fuse', [
+    ('dil2_conv5stage', 'bins', True), ('conv2_dil2', 'shuffle', False), ('cocodet', None, None), ('pool2', None, None),
+    ('dil4', None, None), ('mobilenetv2', None, None)])
+def test_op_ref_bounds_hold_for_the_bf16_emulation(name, layout, fuse):
+    """kernel_refs.op_ref on every op kind (dilated convs, max pool, upsampled heads, scatter, shuffle, fused depthwise
+    -> 1x1): ops_emulator.run_ops with bf16 rounds where the kernels round, so its tensors must meet every bound"""
+    import ops_emulator
+    kw = {} if layout is None else {'layout': layout, 'fuse_dw': fuse}
+    tensors, ops, _ = network.build_ops(_emulation_plan(name), 49, 65, **kw)
+    images = np.random.default_rng(1).standard_normal((2, 3, 49, 65)).astype(np.float32)
+    heads, acts = ops_emulator.run_ops(tensors, ops, torch.from_numpy(images), bf16=True)
+    taps = {t: a.numpy() for t, a in enumerate(acts)}
+    kinds = set()
+    for i, o in enumerate(ops):
+        kind, r = kr.op_ref(o, taps, [h.numpy() for h in heads], images, 2)
+        assert r <= 1.0, (i, kind, r)
+        kinds.add(kind)
+    print(name, sorted(kinds))

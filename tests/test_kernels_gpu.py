@@ -731,61 +731,22 @@ def test_overlapped_predictor_equals_sequential(k16_plan, max_batch, reserve, mo
 
 
 # ---------------------------------------------------------------------------------------------------- teacher-forced networks
-def op_check(o, taps, heads, images, batch, t_shapes):
-    """float64 reference of one op of network.build_ops from the tensors the GPU fed it -> (kind, worst ratio)"""
-    kind = o['kind']
-
-    def a_in(t, off, n):
-        return taps[t][:batch, ..., off:off + n]
-
-    if kind == 'heads':
-        w = kr.bf16_round(o['w'])
-        refs = kr.heads_ref(a_in(o['in'], 0, o['k_cols']), w, o['b'], o['n_fields'], o['n_comp'], o['ops'])
-        return 'heads', max(kr.worst_ratio(hb[:batch], r, bd) for hb, (r, bd) in zip(heads, refs))
-    if kind == 'input_conv':
-        x = images[:batch].transpose(0, 2, 3, 1)
-        ref, mag = kr.conv_ref(x, o['w'], o['b'], o['stride'], o['pad'])
-        ref, mag = kr.epilogue(ref, mag, o['relu'])
-        return kind, kr.worst_ratio(taps[o['out']][:batch, ..., :o['c_out']], ref,
-                                    kr.bf16_bound(ref, mag, 3 * o['kernel'] ** 2))
-    if kind == 'dw_conv1x1':
-        C = o['channels']
-        ref, bound = kr.dw_gemm_ref(a_in(o['in'], o['in_off'], C), o['dw_w'], o['dw_b'], o['dw_relu'],
-                                    kr.bf16_round(o['w']), o['b'], o['relu'])
-        worst = 0.0
-        for c0, cnt, t, col in o['pieces']:
-            worst = max(worst, kr.worst_ratio(taps[t][:batch, ..., col:col + cnt], ref[..., c0:c0 + cnt],
-                                              bound[..., c0:c0 + cnt]))
-        return 'dw_gemm', worst
-    if kind == 'dwconv':
-        C, k = o['channels'], o['kernel']
-        ref, mag = kr.conv_ref(a_in(o['in'], o['in_off'], C), o['w'].reshape(C, 1, k, k), o['b'], o['stride'],
-                               o['pad'], groups=C)
-        ref, mag = kr.epilogue(ref, mag, o['relu'])
-        return 'dwconv k%d s%d' % (k, o['stride']), kr.worst_ratio(
-            taps[o['out']][:batch, ..., o['out_off']:o['out_off'] + C], ref, kr.bf16_bound(ref, mag, k * k))
-    if kind == 'conv':
-        k = o['kernel']
-        ref, mag = kr.conv_ref(a_in(o['in'], o['in_off'], o['c_in']), kr.bf16_round(o['w']), o['b'], o['stride'],
-                               o['pad'])
-        res = None if o['residual'] < 0 else a_in(o['residual'], o['residual_off'], o['n_out'])
-        ref, mag = kr.epilogue(ref, mag, o['relu'], res)
-        return 'conv k%d' % k, kr.worst_ratio(taps[o['out']][:batch, ..., o['out_off']:o['out_off'] + o['n_out']],
-                                              ref, kr.bf16_bound(ref, mag, o['c_in'] * k * k))
-    assert kind == 'conv1x1'
-    K, N = o['k_cols'], o['n_out']
-    ref, mag = kr.conv_ref(a_in(o['in'], o['in_off'], K), kr.bf16_round(o['w'])[:, :, None, None], o['b'], 1, 0)
-    ref, mag = kr.epilogue(ref, mag, o['relu'])
-    bound = kr.bf16_bound(ref, mag, K)
-    out = taps[o['out']][:batch]
-    if 'pieces' in o:
-        return 'gemm scatter', max(kr.worst_ratio(taps[t][:batch, ..., col:col + cnt], ref[..., c0:c0 + cnt],
-                                                  bound[..., c0:c0 + cnt]) for c0, cnt, t, col in o['pieces'])
-    if o['shuffle_src'] >= 0:
-        src = a_in(o['shuffle_src'], o['shuffle_off'], N)
-        assert np.array_equal(out[..., 0:2 * N:2], src), 'pass-through channels of the fused shuffle'
-        return 'gemm shuffle', kr.worst_ratio(out[..., 1:2 * N:2], ref, bound)
-    return 'gemm plain', kr.worst_ratio(out[..., o['out_off']:o['out_off'] + N], ref, bound)
+def check_ops_teacher_forced(net, ops, images, label, what=''):
+    """one forward of images [B, 3, H, W] (float32 numpy) through net, then every op of `ops` (build_ops of net's plan)
+    against kernel_refs.op_ref on the tensors the GPU actually fed it (each (tensor, column) has one producer:
+    test_kernel_refs.py::test_every_tensor_column_is_written_by_one_op); every ratio is recorded under
+    '<kind> (<label>)'.  -> ({kind: worst err / bound}, the head outputs of the forward as CUDA tensors)"""
+    B = images.shape[0]
+    fields = [t.clone() for t in net.forward(torch.from_numpy(images).cuda())]
+    torch.cuda.synchronize()
+    taps = {t: net.tap(t, B) for t in range(len(net.tensor_shapes))}
+    heads = [t.cpu().numpy() for t in fields]
+    worst = {}
+    for i, o in enumerate(ops):
+        kind, r = kr.op_ref(o, taps, heads, images, B)
+        worst[kind] = max(worst.get(kind, 0.0), r)
+        record(f'{kind} ({label})', r, f'{what} op {i}')
+    return worst, fields
 
 
 NETWORKS = [
@@ -801,24 +762,16 @@ NETWORKS = [
 @pytest.mark.parametrize('name,layout,fuse,H,W,B', NETWORKS,
                          ids=['%s-%s-fuse%s' % (n[0], n[1], n[2]) for n in NETWORKS])
 def test_teacher_forced_ops_of_real_networks(name, layout, fuse, H, W, B):
-    """one forward, then every op against the float64 reference of the tensors the GPU actually fed it (each
-    (tensor, column) has one producer: test_kernel_refs.py::test_every_tensor_column_is_written_by_one_op)"""
+    """one forward, then every op against the float64 reference of the tensors the GPU actually fed it"""
     if name == 'shufflenetv2k30-wholebody':
         shell = net_oracle.make_shell('shufflenetv2k30', n_keypoints=133, n_connections=160, seed=3)
     else:
         shell = net_oracle.make_shell(name, seed=4)
     plan = network.plan_from_shell(shell)
     kw = {} if layout is None else {'layout': layout, 'fuse_dw': fuse}
-    tensors, ops, _ = network.build_ops(plan, H, W, **kw)
+    _, ops, _ = network.build_ops(plan, H, W, **kw)
     net = network.CompiledNet(plan, H, W, B, **kw)
     images = np.random.default_rng(9).standard_normal((B, 3, H, W)).astype(np.float32)
-    heads = [t.cpu().numpy() for t in net.forward(torch.from_numpy(images).cuda())]
-    torch.cuda.synchronize()
-    taps = {t: net.tap(t, B) for t in range(len(tensors))}
+    worst, _ = check_ops_teacher_forced(net, ops, images, 'network', name)
     net.close()
-    worst = {}
-    for i, o in enumerate(ops):
-        kind, r = op_check(o, taps, heads, images, B, tensors)
-        worst[kind] = max(worst.get(kind, 0.0), r)
-        record(kind + ' (network)', r, f'{name} op {i}')
     print(name, layout, fuse, {k: round(v, 3) for k, v in worst.items()})

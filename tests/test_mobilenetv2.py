@@ -11,6 +11,7 @@ import torch
 
 import helpers
 import mobilenetv2_models as mm
+import ops_emulator
 from openpifpaf_b200 import network
 from oracle import build_ref, net_oracle
 
@@ -45,8 +46,8 @@ def test_lowering_reproduces_fp32_and_bf16_emulation(h, w):
         want = shell(x)
     plan = network.plan_from_shell(shell)
     tensors, ops, _ = network.build_ops(plan, h, w)
-    got, _ = mm.run_ops(tensors, ops, x)
-    emu, _ = mm.run_ops(tensors, ops, x, bf16=True)
+    got, _ = ops_emulator.run_ops(tensors, ops, x)
+    emu, _ = ops_emulator.run_ops(tensors, ops, x, bf16=True)
     assert len(got) == len(want) == 2
     for g, e, wt in zip(got, emu, want):
         assert g.shape == e.shape == wt.shape

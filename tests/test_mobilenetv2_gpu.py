@@ -19,19 +19,14 @@ import torch
 import det_models
 import kernel_refs as kr
 import mobilenetv2_models as mm
+import ops_emulator
 from openpifpaf_b200 import _lib, decoder, network, predictor
-from test_kernels_gpu import Case, Check, n_sm, pad8, pad16, ptr, record
+from test_kernels_gpu import Case, Check, check_ops_teacher_forced, n_sm, pad8, pad16, ptr
 
 pytestmark = pytest.mark.gpu
 
 FIELD_TOL_REL = 3e-2        # tests/test_network_gpu.py
 RELU6 = network.ACT_RELU6
-
-
-def epilogue(y, mag, code, res=None):
-    """+ residual, then the activation of code (0 none, 1 ReLU, 2 ReLU6); both are 1-Lipschitz, the bound carries over"""
-    y, mag = kr.epilogue(y, mag, code >= 1, res)
-    return (np.minimum(y, 6.0) if code == 2 else y), mag
 
 
 def straddling_bias(rng, n):
@@ -63,7 +58,7 @@ def test_input_conv_relu6(u8):
     def emit(L, net):
         _lib.check(L.pifpaf_net_input_conv(net, H, W, 3, 2, 1, C, ptr(w), ptr(b), RELU6, 0))
 
-    ref, mag = epilogue(*kr.conv_ref(x, w, b, 2, 1), RELU6)
+    ref, mag = kr.epilogue(*kr.conv_ref(x, w, b, 2, 1), RELU6)
     assert_straddles(ref)
     chk = Check('relu6 input_conv', batch)
     chk.own(0, 0, pad8(C))
@@ -108,7 +103,7 @@ def conv6_case(H, W, c_in, k, stride, N, in_off, res_col, out_off, batch, mb, se
 
     ref, mag = kr.conv_ref(case.data[0][:batch, ..., in_off:in_off + c_in], w, b, stride, pad)
     res = None if res_col is None else case.data[2][:batch, ..., res_col:res_col + N]
-    ref, mag = epilogue(ref, mag, RELU6, res)
+    ref, mag = kr.epilogue(ref, mag, RELU6, res)
     assert_straddles(ref)
     chk = Check('relu6 conv k%d%s' % (k, '' if res_col is None else ' residual'), batch)
     chk.own(1, out_off, out_off + pad8(N))
@@ -144,7 +139,7 @@ def test_conv1x1_plain_relu6():
         assert L.pifpaf_net_conv1x1(net, 0, 0, K, N, ptr(wt), ptr(b), 3, 1, 0, -1, 0) == _lib.E_BADARG
         assert L.pifpaf_net_num_ops(net) == 1
 
-    ref, mag = epilogue(*kr.conv_ref(case.data[0][:batch, ..., :K], wt[:, :, None, None], b, 1, 0), RELU6)
+    ref, mag = kr.epilogue(*kr.conv_ref(case.data[0][:batch, ..., :K], wt[:, :, None, None], b, 1, 0), RELU6)
     assert_straddles(ref)
     chk = Check('relu6 gemm plain', batch)
     chk.own(1, 0, N)
@@ -218,7 +213,7 @@ def dw_case(H, W, C, k, stride, pad, in_off, out_off, relu, batch, mb, seed=0):
         _lib.check(L.pifpaf_net_dwconv(net, 0, in_off, C, k, stride, pad, ptr(w), ptr(b), relu, 1, out_off))
 
     x = case.data[0][:batch, ..., in_off:in_off + C]
-    ref, mag = epilogue(*kr.conv_ref(x, w.reshape(C, 1, k, k), b, stride, pad, groups=C), relu)
+    ref, mag = kr.epilogue(*kr.conv_ref(x, w.reshape(C, 1, k, k), b, stride, pad, groups=C), relu)
     if relu == 2 and ref.size > 1000:
         assert_straddles(ref)
     chk = Check('relu6 dwconv k%d s%d' % (k, stride) if relu == 2 else 'dwconv k%d s%d' % (k, stride), batch)
@@ -258,52 +253,15 @@ def test_dwconv3_tma_schedules_are_bitwise_invariant(c, monkeypatch):
 
 
 # ---------------------------------------------------------------------------------------------------- network
-def op_check(o, taps, heads, images, batch):
-    """float64 reference of one MobileNetV2 op from the tensors the GPU fed it -> (kind, worst err / bound)"""
-    kind = o['kind']
-
-    def a_in(t, off, n):
-        return taps[t][:batch, ..., off:off + n]
-
-    if kind == 'heads':
-        refs = kr.heads_ref(a_in(o['in'], 0, o['k_cols']), kr.bf16_round(o['w']), o['b'], o['n_fields'], o['n_comp'],
-                            o['ops'])
-        return 'heads', max(kr.worst_ratio(hb[:batch], r, bd) for hb, (r, bd) in zip(heads, refs))
-    if kind == 'input_conv':
-        ref, mag = epilogue(*kr.conv_ref(images[:batch].transpose(0, 2, 3, 1), o['w'], o['b'], o['stride'], o['pad']),
-                            o['relu'])
-        return kind, kr.worst_ratio(taps[o['out']][:batch, ..., :o['c_out']], ref, kr.bf16_bound(ref, mag, 27))
-    if kind == 'dwconv':
-        C, k = o['channels'], o['kernel']
-        ref, mag = epilogue(*kr.conv_ref(a_in(o['in'], o['in_off'], C), o['w'].reshape(C, 1, k, k), o['b'],
-                                         o['stride'], o['pad'], groups=C), o['relu'])
-        return 'dwconv s%d' % o['stride'], kr.worst_ratio(taps[o['out']][:batch, ..., :C], ref,
-                                                          kr.bf16_bound(ref, mag, k * k))
-    assert kind == 'conv'
-    ref, mag = kr.conv_ref(a_in(o['in'], 0, o['c_in']), kr.bf16_round(o['w']), o['b'], o['stride'], o['pad'])
-    res = None if o['residual'] < 0 else a_in(o['residual'], 0, o['n_out'])
-    ref, mag = epilogue(ref, mag, o['relu'], res)
-    return ('conv residual' if res is not None else 'conv'), kr.worst_ratio(
-        taps[o['out']][:batch, ..., :o['n_out']], ref, kr.bf16_bound(ref, mag, o['c_in']))
-
-
 @pytest.mark.parametrize('H,W,B', [(641, 641, 2), (353, 481, 3)])
 def test_network_teacher_forced_and_against_fp32(H, W, B):
     shell = mm.make_pose_shell(seed=4)
     plan = network.plan_from_shell(shell)
-    tensors, ops, _ = network.build_ops(plan, H, W)
+    _, ops, _ = network.build_ops(plan, H, W)
     net = network.CompiledNet(plan, H, W, B)
     images = np.random.default_rng(9).standard_normal((B, 3, H, W)).astype(np.float32)
     x = torch.from_numpy(images).cuda()
-    got = [t.clone() for t in net.forward(x)]
-    torch.cuda.synchronize()
-    taps = {t: net.tap(t, B) for t in range(len(tensors))}
-    heads = [t.cpu().numpy() for t in got]
-    worst = {}
-    for i, o in enumerate(ops):
-        kind, r = op_check(o, taps, heads, images, B)
-        worst[kind] = max(worst.get(kind, 0.0), r)
-        record(kind + ' (mobilenetv2)', r, f'op {i}')
+    worst, got = check_ops_teacher_forced(net, ops, images, 'mobilenetv2')
     print(H, W, {k: round(v, 3) for k, v in worst.items()})
     # no 1x1 -> depthwise pair is fused: every depthwise op is its own launch (kind 2), nothing runs as kind 3
     _, kind, _, _ = net.forward_timed(x)
@@ -327,7 +285,7 @@ def test_gemm_impl_1_matches_emulation():
     size, batch = 97, 2
     x = torch.randn(batch, 3, size, size, generator=torch.Generator().manual_seed(6))
     tensors, ops, _ = network.build_ops(plan, size, size)
-    emu_heads, _ = mm.run_ops(tensors, ops, x, bf16=True)
+    emu_heads, _ = ops_emulator.run_ops(tensors, ops, x, bf16=True)
     net = network.CompiledNet(plan, size, size, batch)
     fields = {}
     for impl in (0, 1):

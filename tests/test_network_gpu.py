@@ -38,14 +38,7 @@ def test_every_op_matches_bf16_emulation(small, layout, fuse):
     for impl in ((0,) if fuse else (1, 0)):
         heads = net.forward(x.cuda(), gemm_impl=impl)
         torch.cuda.synchronize()
-        for o in ops:
-            if o['kind'] == 'heads':
-                continue
-            for t_id in sorted({pc[2] for pc in o['pieces']}) if 'pieces' in o else [o['out']]:
-                got = net.tap(t_id, B)
-                ref = emu_acts[t_id].numpy()
-                scale = max(float(np.abs(ref).max()), 1e-6)
-                assert float(np.abs(got - ref).max()) / scale < 3e-2, (impl, o['kind'], t_id)
+        helpers.assert_taps_match_emulation(net, ops, emu_acts, B, f'impl {impl}')
         for hg, he in zip(heads, emu_heads):
             assert float((hg.cpu() - he).abs().max()) < 5e-2
 
@@ -150,15 +143,9 @@ def test_resnet_implicit_gemm_matches_emulation_and_fp32(name, size, batch):
     emu_heads, emu_acts = ops_emulator.run_ops(tensors, ops, x, bf16=True)
     net = network.CompiledNet(plan, size, size, batch)
     for impl in (1, 0):
-        heads = net.forward(x.cuda(), gemm_impl=impl)
+        net.forward(x.cuda(), gemm_impl=impl)
         torch.cuda.synchronize()
-        for o in ops:
-            if o['kind'] == 'heads':
-                continue
-            got = net.tap(o['out'], batch)
-            ref = emu_acts[o['out']].numpy()
-            scale = max(float(np.abs(ref).max()), 1e-6)
-            assert float(np.abs(got - ref).max()) / scale < 3e-2, (impl, o['kind'], o['out'], o.get('kernel'), o.get('stride'))
+        helpers.assert_taps_match_emulation(net, ops, emu_acts, batch, f'{name} impl {impl}')
     with torch.no_grad():
         want = shell(x)
     # vs fp32 PyTorch: bf16 rounding through 21 / 54 layers (resnet50 with randomised BN statistics needs the wider
@@ -184,13 +171,7 @@ def test_k30_wholebody_network_and_decode():
     net = network.CompiledNet(plan, h, w, B)
     heads = net.forward(x.cuda())
     torch.cuda.synchronize()
-    for o in ops:
-        if o['kind'] == 'heads':
-            continue
-        got = net.tap(o['out'], B)
-        ref = emu_acts[o['out']].numpy()
-        scale = max(float(np.abs(ref).max()), 1e-6)
-        assert float(np.abs(got - ref).max()) / scale < 3e-2, (o['kind'], o['out'])
+    helpers.assert_taps_match_emulation(net, ops, emu_acts, B, 'k30 wholebody')
     with torch.no_grad():
         want = shell(x)
     for hg, hw_ in zip(heads, want):

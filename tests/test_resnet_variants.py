@@ -11,7 +11,7 @@ import torch
 
 import det_models
 import helpers
-import resnet_ops_emulator
+import ops_emulator
 from openpifpaf_b200 import network
 from oracle import build_ref, net_oracle
 
@@ -51,7 +51,7 @@ def test_variant_lowering_reproduces_oracle(variant, base_name):
         want = shell(x)
     plan = network.plan_from_shell(shell)
     tensors, ops, _ = network.build_ops(plan, h, w)
-    got, _ = resnet_ops_emulator.run_ops(tensors, ops, x)
+    got, _ = ops_emulator.run_ops(tensors, ops, x)
     assert len(got) == len(want)
     for g, wt in zip(got, want):
         assert g.shape == wt.shape

@@ -1,28 +1,22 @@
 """GPU: the kernels behind the Resnet variants of tests/test_resnet_variants.py -- dilated implicit-GEMM convs
 (--resnet-block5-dilation) against float64 with the bound, sentinels and column windows of tests/test_kernels_gpu.py;
 k_maxpool (--resnet-pool0-stride) bit for bit against torch.max_pool2d; whole resnet18 variants and the
-resnet18-cocodet recipe against fp32 PyTorch and op by op against the bf16 emulation."""
+resnet18-cocodet recipe against fp32 PyTorch, op by op against the bf16 emulation and against the float64 reference of
+what the GPU fed each op."""
 import numpy as np
 import pytest
 import torch
 
 import det_models
+import helpers
 import kernel_refs as kr
-import resnet_ops_emulator
+import ops_emulator
 from openpifpaf_b200 import _lib, network
-from test_kernels_gpu import Case, Check, n_sm, pad8, pad16, ptr
+from test_kernels_gpu import Case, Check, check_ops_teacher_forced, n_sm, pad8, pad16, ptr
 
 pytestmark = pytest.mark.gpu
 
 FIELD_TOL_REL = 3e-2        # tests/test_network_gpu.py
-
-
-def dilate(w, d):
-    """a k x k kernel with dilation d as the equivalent (d (k - 1) + 1)^2 kernel with zero taps"""
-    n, c, k, _ = w.shape
-    out = np.zeros((n, c, d * (k - 1) + 1, d * (k - 1) + 1), dtype=w.dtype)
-    out[:, :, ::d, ::d] = w
-    return out
 
 
 # (H, W, c_in, dilation, pad, n_out, in_off, residual col (None: no residual), relu, out_off, batch, max_batch)
@@ -61,7 +55,7 @@ def dil_case(H, W, c_in, d, pad, N, in_off, res_col, relu, out_off, batch, mb, s
         _lib.check(L.pifpaf_net_conv_dilated(net, 0, in_off, c_in, k, 1, pad, N, ptr(w), ptr(b), relu, 1, out_off,
                                              -1 if res_col is None else 2, 0 if res_col is None else res_col, d))
 
-    ref, mag = kr.conv_ref(case.data[0][:batch, ..., in_off:in_off + c_in], dilate(w, d), b, 1, pad)
+    ref, mag = kr.conv_ref(case.data[0][:batch, ..., in_off:in_off + c_in], w, b, 1, pad, dilation=d)
     res = None if res_col is None else case.data[2][:batch, ..., res_col:res_col + N]
     ref, mag = kr.epilogue(ref, mag, relu, res)
     chk = Check('conv k3 dilated', batch)
@@ -167,21 +161,18 @@ def test_resnet18_variant_matches_emulation_and_fp32(variant):
     size, batch = 161, 2
     x = torch.randn(batch, 3, size, size, generator=torch.Generator().manual_seed(6))
     tensors, ops, _ = network.build_ops(plan, size, size)
-    emu_heads, emu_acts = resnet_ops_emulator.run_ops(tensors, ops, x, bf16=True)
+    emu_heads, emu_acts = ops_emulator.run_ops(tensors, ops, x, bf16=True)
     net = network.CompiledNet(plan, size, size, batch)
     for impl in (1, 0):
         heads = net.forward(x.cuda(), gemm_impl=impl)
         torch.cuda.synchronize()
-        for o in ops:
-            if o['kind'] == 'heads':
-                continue
-            got = net.tap(o['out'], batch)
-            ref = emu_acts[o['out']].numpy()
-            scale = max(float(np.abs(ref).max()), 1e-6)
-            assert float(np.abs(got - ref).max()) / scale < 3e-2, (impl, o['kind'], o['out'], o.get('dilation'))
+        helpers.assert_taps_match_emulation(net, ops, emu_acts, batch, f'{variant} impl {impl}')
         for hg, he in zip(heads, emu_heads):
             assert hg.shape == he.shape
             assert float((hg.cpu() - he).abs().max()) < 5e-2 * max(float(he.abs().max()), 1.0)
+    # every op against float64 on the tensors the GPU fed it: the dilated convs, the max pool, the upsampled heads
+    worst, _ = check_ops_teacher_forced(net, ops, x.numpy(), 'resnet variants', variant)
+    print(variant, {k: round(v, 3) for k, v in worst.items()})
     with torch.no_grad():
         want = shell(x)
     for hg, hw_ in zip(net.forward(x.cuda()), want):

@@ -11,6 +11,7 @@ import pytest
 import torch
 
 import helpers
+import ops_emulator
 import shufflenetv2k_models as sm
 from openpifpaf_b200 import network
 from oracle import build_ref, net_oracle
@@ -68,7 +69,7 @@ def test_variant_lowering_reproduces_mirror(variant, config, layout):
         want = shell(x)
     plan = network.plan_from_shell(shell)
     tensors, ops, info = network.build_ops(plan, h, w, layout=layout)
-    got, acts = sm.run_ops(tensors, ops, x)
+    got, acts = ops_emulator.run_ops(tensors, ops, x)
     assert len(got) == len(want)
     for g, wt in zip(got, want):
         assert g.shape == wt.shape

@@ -19,19 +19,11 @@ import kernel_refs as kr
 import mobilenetv2_models as mm
 import shufflenetv2k_models as sm
 from openpifpaf_b200 import _lib, decoder, network, predictor
-from test_kernels_gpu import Case, Check, n_sm, op_check, pad8, pad16, ptr, record
+from test_kernels_gpu import Case, Check, check_ops_teacher_forced, n_sm, pad8, pad16, ptr
 
 pytestmark = pytest.mark.gpu
 
 FIELD_TOL_REL = 3e-2        # tests/test_network_gpu.py
-
-
-def spread(w, d):
-    """[C, k, k] taps d pixels apart as the equivalent [C, 1, kd, kd] kernel, kd = (k - 1) d + 1, zero in between"""
-    c, k, _ = w.shape
-    out = np.zeros((c, 1, (k - 1) * d + 1, (k - 1) * d + 1), dtype=w.dtype)
-    out[:, 0, ::d, ::d] = w
-    return out
 
 
 # (H, W, channels, kernel, dilation, pad, in_off, out_off, relu, batch, max_batch)
@@ -70,10 +62,7 @@ def dwd_case(H, W, C, k, d, pad, in_off, out_off, relu, batch, mb, seed=0):
         _lib.check(L.pifpaf_net_dwconv_dilated(net, 0, in_off, C, k, 1, pad, ptr(w), ptr(b), relu, 1, out_off, d))
 
     x = case.data[0][:batch, ..., in_off:in_off + C]
-    ref, mag = kr.conv_ref(x, spread(w, d), b, 1, pad, groups=C)
-    ref, mag = kr.epilogue(ref, mag, relu >= 1)
-    if relu == 2:
-        ref = np.minimum(ref, 6.0)
+    ref, mag = kr.epilogue(*kr.conv_ref(x, w.reshape(C, 1, k, k), b, 1, pad, groups=C, dilation=d), relu)
     chk = Check('dwconv k%d dilated' % k, batch)
     chk.own(1, out_off, out_off + pad8(C))
     chk.compare(1, out_off, ref, kr.bf16_bound(ref, mag, k * k))
@@ -143,19 +132,11 @@ def test_variant_teacher_forced_and_against_fp32(variant, layout):
     shell = k16_variant_shell(variant, seed=4)
     plan = network.plan_from_shell(shell)
     H, W, B = 129, 97, 2
-    tensors, ops, _ = network.build_ops(plan, H, W, layout=layout)
+    _, ops, _ = network.build_ops(plan, H, W, layout=layout)
     net = network.CompiledNet(plan, H, W, B, layout=layout)
     images = np.random.default_rng(9).standard_normal((B, 3, H, W)).astype(np.float32)
     x = torch.from_numpy(images).cuda()
-    got = [t.clone() for t in net.forward(x)]
-    torch.cuda.synchronize()
-    taps = {t: net.tap(t, B) for t in range(len(tensors))}
-    heads = [t.cpu().numpy() for t in got]
-    worst = {}
-    for i, o in enumerate(sm.undilated_ops(ops)):
-        kind, r = op_check(o, taps, heads, images, B, tensors)
-        worst[kind] = max(worst.get(kind, 0.0), r)
-        record(kind + ' (shufflenetv2k variants)', r, f'{variant} {layout} op {i}')
+    worst, got = check_ops_teacher_forced(net, ops, images, 'shufflenetv2k variants', f'{variant} {layout}')
     print(variant, layout, {k: round(v, 3) for k, v in worst.items()})
     torch.backends.cudnn.allow_tf32 = False
     torch.backends.cuda.matmul.allow_tf32 = False
