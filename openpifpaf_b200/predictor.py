@@ -21,6 +21,16 @@ from . import network as _network
 from . import preprocess as _preprocess
 
 
+def raw_image_chunks(images, max_batch, fill):
+    """Split the images of `Predictor.raw_images` into batches of at most max_batch; yields (images, fill) per batch.
+    A per-image fill list (`preprocess.pad_fills`) must have one entry per image and is sliced with the images; any
+    other fill applies to every batch as it is."""
+    if isinstance(fill, list) and len(fill) != len(images):
+        raise RuntimeError(f'fill has {len(fill)} colours for {len(images)} images')
+    for i in range(0, len(images), max_batch):
+        yield images[i:i + max_batch], fill[i:i + max_batch] if isinstance(fill, list) else fill
+
+
 class Predictor:
     """:param net: `network.CompiledNet`
     :param n_keypoints: number of keypoints of the CIF head
@@ -150,17 +160,17 @@ class Predictor:
         images with everything after the JPEG decode on the GPU: RescaleAbsolute(long edge = the compiled input size)
         + CenterPad (`preprocess.GpuPreprocess`, bit-identical to the reference's Pillow path), ToTensor + Normalize in
         the stem, forward, decode; then `Annotation.inverse_transform` (and `json_data`) for all annotations of an
-        image at once.  Returns per image (data [N, K, 3] (x, y, v) in original-image pixels, joint_scales [N, K], meta)
-        or, with json_data, (list of dicts, meta)."""
+        image at once.  fill: the pad colour as for `GpuPreprocess` (a list has one colour per image of `images`).
+        Returns per image (data [N, K, 3] (x, y, v) in original-image pixels, joint_scales [N, K], meta) or, with
+        json_data, (list of dicts, meta)."""
         if self.net.in_h != self.net.in_w:
             raise RuntimeError('raw_images needs a net compiled for a square input (CenterPad(long_edge))')
         if getattr(self, '_gpu_preprocess', None) is None:
             self._gpu_preprocess = _preprocess.GpuPreprocess(self.net.in_w, batched=True, device=self.device.index)
         out = []
-        for i in range(0, len(images), self.net.max_batch):
-            chunk = images[i:i + self.net.max_batch]
+        for chunk, chunk_fill in raw_image_chunks(images, self.net.max_batch, fill):
             with torch.cuda.stream(self.stream):
-                canvas, metas = self._gpu_preprocess(chunk, fill=fill, stream=self.stream)
+                canvas, metas = self._gpu_preprocess(chunk, fill=chunk_fill, stream=self.stream)
                 self.batch_device(canvas)
                 result = self.decoder.fetch(stream=self.result_stream())
                 self.join()

@@ -17,6 +17,7 @@ annotations of an image at once (same float32 / float64 roundings as the referen
 """
 import ctypes
 import math
+import numbers
 
 import numpy as np
 import torch
@@ -96,13 +97,15 @@ def center_pad_ltrb(w, h, target_w, target_h):
     return left, top, right, bottom
 
 
-def reference_meta(w, h, target_w, target_h, ltrb):
+def reference_meta(w, h, target_w, target_h, ltrb, rescaled=True):
     """The meta dict after NormalizeAnnotations -> _scale -> CenterPad (transforms/annotations.py:52-77,
-    transforms/scale.py:73-96, transforms/pad.py:26-33), float64 numpy like the reference."""
+    transforms/scale.py:73-96, transforms/pad.py:26-33), float64 numpy like the reference.
+    rescaled: RescaleAbsolute is part of the pipeline (a long edge is set).  Its _scale runs even when the size does not
+    change, and divides by zero on a 1-pixel-wide or -high image like the reference; without it no factor applies."""
     meta = {'offset': np.array((0.0, 0.0)), 'scale': np.array((1.0, 1.0)),
             'rotation': {'angle': 0.0, 'width': None, 'height': None},
             'valid_area': np.array((0.0, 0.0, w - 1, h - 1)), 'hflip': False, 'width_height': np.array((w, h))}
-    if (target_w, target_h) != (w, h) or True:
+    if rescaled:
         x_scale = (target_w - 1) / (w - 1)
         y_scale = (target_h - 1) / (h - 1)
         sf = np.array((x_scale, y_scale))
@@ -113,6 +116,40 @@ def reference_meta(w, h, target_w, target_h, ltrb):
     meta['offset'] -= ltrb[:2]
     meta['valid_area'][:2] += ltrb[:2]
     return meta
+
+
+def pad_fills(fill, n_images, batched):
+    """The `fill` argument of GpuPreprocess -> one (r, g, b) per image.  An int (grey) or a tuple (r, g, b) is one
+    colour for every image; a list holds one int or (r, g, b) per image and has exactly n_images entries.  None draws
+    like the reference: CenterPad a random grey per image with torch.randint(0, 255) (transforms/pad.py:52),
+    CenterPadTight (124, 116, 104) (pad.py:100-101)."""
+    if fill is None:
+        fill = [int(torch.randint(0, 255, (1,)).item()) if batched else TIGHT_PAD_FILL for _ in range(n_images)]
+    elif isinstance(fill, list):
+        if len(fill) != n_images:
+            raise RuntimeError(f'fill has {len(fill)} colours for {n_images} images')
+    else:
+        fill = [fill] * n_images
+    out = []
+    for f in fill:
+        c = (int(f),) * 3 if isinstance(f, numbers.Integral) else tuple(int(v) for v in f)
+        if len(c) != 3:
+            raise RuntimeError(f'a pad colour is an int or an (r, g, b) triple, not {f!r}')
+        out.append(c)
+    return out
+
+
+def resize_path(w, h, target_w, target_h, dst_pitch_bytes):
+    """The launch sequence pifpaf_image_resize_bilinear_u8 takes for a [h, w] image resized to [target_h, target_w]
+    into a destination with the given row pitch: 'hv' (horizontal pass into tmp, vertical pass into the destination),
+    'h_dense' (horizontal pass straight into a dense destination), 'h_pitched' (horizontal pass into tmp, then a row
+    copy), 'v' (vertical pass from the source) or 'copy'."""
+    need_h, need_v = target_w != w, target_h != h
+    if need_h and need_v:
+        return 'hv'
+    if need_h:
+        return 'h_dense' if dst_pitch_bytes == target_w * 3 else 'h_pitched'
+    return 'v' if need_v else 'copy'
 
 
 class GpuPreprocess:
@@ -153,9 +190,8 @@ class GpuPreprocess:
         return out, canvases.pop()
 
     def __call__(self, images, fill=None, stream=None):
-        """images: list of uint8 [h, w, 3] arrays / tensors (host).  fill: pad colour -- an int (grey) or an (r, g, b)
-        triple, or a list of those per image.  Default like the reference: CenterPad draws a random grey per image
-        with torch.randint(0, 255) (transforms/pad.py:52), CenterPadTight uses (124, 116, 104) (pad.py:100-101).
+        """images: list of uint8 [h, w, 3] arrays / tensors (host or CUDA).  fill: pad colour -- an int (grey) or an
+        (r, g, b) tuple for every image, or a list of those per image (`pad_fills`; default like the reference).
         Returns (canvas uint8 CUDA [B, H, W, 3], metas)."""
         imgs = [torch.as_tensor(np.ascontiguousarray(im)) if not isinstance(im, torch.Tensor) else im.contiguous()
                 for im in images]
@@ -165,12 +201,10 @@ class GpuPreprocess:
         sizes = [(int(im.shape[1]), int(im.shape[0])) for im in imgs]
         plans, (cw, ch) = self.plan(sizes)
         B = len(imgs)
-        if fill is None:
-            fill = [int(torch.randint(0, 255, (1,)).item()) if self.batched else TIGHT_PAD_FILL for _ in range(B)]
-        elif isinstance(fill, int) or (isinstance(fill, tuple) and len(fill) == 3 and B != 3):
-            fill = [fill] * B
-        fill = [(f, f, f) if isinstance(f, int) else tuple(int(c) for c in f) for f in fill]
+        fill = pad_fills(fill, B, self.batched)
         st = stream if stream is not None else torch.cuda.current_stream(self.device)
+        if any(im.is_cuda for im in imgs):
+            st.wait_stream(torch.cuda.current_stream(self.device))     # CUDA inputs (and .contiguous()) are written there
         L = _lib.lib()
         sp = ctypes.c_void_p(st.cuda_stream)
         with torch.cuda.stream(st):
@@ -193,7 +227,7 @@ class GpuPreprocess:
                     yb.data_ptr() if yb is not None else None, yk.data_ptr() if yk is not None else None, yks,
                     tmp.data_ptr(), sp))
                 keep.append((src, tmp))
-                metas.append(reference_meta(w, h, tw, th, np.asarray(ltrb)))
+                metas.append(reference_meta(w, h, tw, th, np.asarray(ltrb), rescaled=self.long_edge is not None))
             self._keepalive = keep
         return canvas, metas
 

@@ -30,6 +30,86 @@ def test_pillow_bilinear_restatement_is_bit_exact(h, w, tw, th):
     np.testing.assert_array_equal(pp.resize_bilinear_reference(img, tw, th), want)
 
 
+def sweep_sizes(n=300, seed=0):
+    """n random (h, w, target_w, target_h) in 1..900 -- up, down, mixed and unchanged directions -- followed by the
+    edges: 1-pixel rows and columns, 200x reductions (401 taps), a phone photo and a panorama to 641"""
+    rng = np.random.default_rng(seed)
+    out = [tuple(int(v) for v in rng.integers(1, 901, 4)) for _ in range(n)]
+    out += [(h, w, w, th) for (h, w, th) in rng.integers(1, 901, (4, 3)).tolist()]        # vertical only
+    out += [(h, w, tw, h) for (h, w, tw) in rng.integers(1, 901, (4, 3)).tolist()]        # horizontal only
+    return out + [(1, 1, 1, 1), (1, 1, 13, 11), (1, 37, 5, 1), (1, 37, 37, 9), (29, 1, 1, 7), (40, 30, 1, 1),
+                  (1, 900, 1, 900), (900, 1, 900, 1), (3, 25600, 128, 3), (20000, 5, 5, 97), (3024, 4032, 641, 480),
+                  (600, 8192, 641, 46)]
+
+
+def test_pillow_bilinear_restatement_random_sweep():
+    """the numpy restatement == PIL.Image.resize(BILINEAR) byte for byte on every size of `sweep_sizes`"""
+    PIL = pytest.importorskip('PIL.Image')
+    rng = np.random.default_rng(17)
+    bad = []
+    for (h, w, tw, th) in sweep_sizes():
+        img = rng.integers(0, 256, (h, w, 3), dtype=np.uint8)
+        want = np.asarray(PIL.fromarray(img).resize((tw, th), PIL.BILINEAR))
+        got = pp.resize_bilinear_reference(img, tw, th)
+        if got.shape != want.shape or not np.array_equal(got, want):
+            bad.append((h, w, tw, th))
+    assert not bad, f'{len(bad)} sizes differ from Pillow, first: {bad[:5]}'
+
+
+def test_pad_fills_tuple_is_one_colour_list_is_per_image():
+    assert pp.pad_fills((1, 2, 3), 3, True) == [(1, 2, 3)] * 3            # not three greys at B = 3
+    assert pp.pad_fills((1, 2, 3), 2, True) == [(1, 2, 3)] * 2
+    assert pp.pad_fills(7, 3, True) == [(7, 7, 7)] * 3
+    assert pp.pad_fills(np.uint8(9), 1, True) == [(9, 9, 9)]
+    assert pp.pad_fills([5, (1, 2, 3), np.array([4, 5, 6])], 3, True) == [(5, 5, 5), (1, 2, 3), (4, 5, 6)]
+    assert pp.pad_fills([(1, 2, 3)], 1, True) == [(1, 2, 3)]
+    for fill, n in (([1, 2], 3), ([1, 2, 3], 2), ([(1, 2, 3)], 3), ([], 1)):
+        with pytest.raises(RuntimeError, match='colours for'):
+            pp.pad_fills(fill, n, True)
+    for fill in ((1, 2), [(1, 2, 3, 4)]):
+        with pytest.raises(RuntimeError, match='triple'):
+            pp.pad_fills(fill, 1, True)
+    # default: CenterPad draws one torch.randint(0, 255) grey per image in order, CenterPadTight a fixed colour
+    torch.manual_seed(4)
+    greys = [int(torch.randint(0, 255, (1,)).item()) for _ in range(3)]
+    torch.manual_seed(4)
+    assert pp.pad_fills(None, 3, True) == [(g, g, g) for g in greys]
+    assert pp.pad_fills(None, 2, False) == [pp.TIGHT_PAD_FILL] * 2
+
+
+def test_raw_image_chunks_slice_per_image_fills():
+    """Predictor.raw_images pads image i with fill[i] in every batch of max_batch images, not fill[i % max_batch]"""
+    from openpifpaf_b200 import predictor
+    images = [f'image{i}' for i in range(7)]
+    fills = [(i, 2 * i, 3 * i) for i in range(7)]
+    chunks = list(predictor.raw_image_chunks(images, 3, fills))
+    assert [c for c, _ in chunks] == [images[0:3], images[3:6], images[6:7]]
+    assert [f for _, f in chunks] == [fills[0:3], fills[3:6], fills[6:7]]
+    for fill in (None, 5, (1, 2, 3)):
+        assert [f for _, f in predictor.raw_image_chunks(images, 3, fill)] == [fill] * 3
+    assert [c for c, _ in predictor.raw_image_chunks(images, 7, None)] == [images]
+    with pytest.raises(RuntimeError, match='colours for'):
+        list(predictor.raw_image_chunks(images, 3, fills[:3]))
+
+
+def test_reference_meta_without_rescale_on_one_pixel_images():
+    """no long edge: RescaleAbsolute is not in the pipeline, so a 1-pixel-wide or -high image has no scale factor
+    (the reference never divides by w - 1); with a long edge the reference's _scale divides by zero, and so does this"""
+    for (w, h) in ((1, 37), (50, 1), (1, 1)):
+        g = pp.GpuPreprocess.__new__(pp.GpuPreprocess)
+        g.long_edge, g.batched, g.multiple = None, False, 16
+        (tw, th, ltrb, _), = g.plan([(w, h)])[0]
+        meta = pp.reference_meta(w, h, tw, th, np.asarray(ltrb), rescaled=False)
+        assert np.array_equal(meta['scale'], (1.0, 1.0)) and np.array_equal(meta['offset'], (-ltrb[0], -ltrb[1]))
+        assert np.array_equal(meta['valid_area'], (ltrb[0], ltrb[1], w - 1, h - 1))
+        with pytest.raises(ZeroDivisionError):
+            pp.reference_meta(w, h, *pp.rescale_target(w, h, 161), np.asarray(ltrb))
+    # two-pixel images keep their factors, and a size the rescale leaves unchanged has factors of exactly 1
+    meta = pp.reference_meta(2, 3, 5, 7, np.zeros(4), rescaled=True)
+    assert np.array_equal(meta['scale'], (4.0, 3.0))
+    assert np.array_equal(pp.reference_meta(300, 641, 300, 641, np.zeros(4))['scale'], (1.0, 1.0))
+
+
 def test_coefficient_tables_are_normalised():
     for n_in, n_out in ((640, 641), (1280, 321), (37, 161)):
         bounds, kk = pp.pil_bilinear_coeffs(n_in, n_out)
@@ -72,13 +152,25 @@ def test_meta_and_annotations_equal_reference_transforms(tmp_path):
         from openpifpaf_b200 import preprocess as pp
         from openpifpaf.plugins.coco.constants import COCO_KEYPOINTS, COCO_PERSON_SKELETON, COCO_PERSON_SCORE_WEIGHTS
         rng = np.random.default_rng(0)
-        for (h, w, long_edge, batched) in ((427, 640, 641, True), (480, 360, 321, True), (333, 500, 385, False), (200, 300, None, False)):
+        for (h, w, long_edge, batched) in ((427, 640, 641, True), (480, 360, 321, True), (333, 500, 385, False),
+                                           (200, 300, None, False), (37, 1, None, False), (1, 50, None, False),
+                                           (1, 1, None, False), (37, 1, 161, True), (1, 50, 161, False)):
             img = rng.integers(0, 256, (h, w, 3), dtype=np.uint8)
             pre = [transforms.NormalizeAnnotations()]
             if long_edge:
                 pre.append(transforms.RescaleAbsolute(long_edge, fast=True))
             pre.append(transforms.CenterPad(long_edge) if batched else transforms.CenterPadTight(16))
             torch.manual_seed(3)
+            if long_edge and min(h, w) == 1:
+                # _scale divides by w - 1 or h - 1: the reference and reference_meta both refuse the image
+                for fn in (lambda: transforms.Compose(pre)(PIL.Image.fromarray(img), [], None),
+                           lambda: pp.reference_meta(w, h, *pp.rescale_target(w, h, long_edge), np.zeros(4))):
+                    try:
+                        fn()
+                        raise AssertionError(('no ZeroDivisionError', h, w))
+                    except ZeroDivisionError:
+                        pass
+                continue
             image, anns, meta = transforms.Compose(pre)(PIL.Image.fromarray(img), [], None)
             torch.manual_seed(3)
             fill = int(torch.randint(0, 255, (1,)).item())
@@ -90,7 +182,7 @@ def test_meta_and_annotations_equal_reference_transforms(tmp_path):
             canvas[:] = (fill, fill, fill) if batched else pp.TIGHT_PAD_FILL
             canvas[ltrb[1]:ltrb[1] + th, ltrb[0]:ltrb[0] + tw] = pp.resize_bilinear_reference(img, tw, th)
             assert np.array_equal(np.asarray(image), canvas), 'resized + padded image differs'
-            mine = pp.reference_meta(w, h, tw, th, np.asarray(ltrb))
+            mine = pp.reference_meta(w, h, tw, th, np.asarray(ltrb), rescaled=long_edge is not None)
             for k in ('offset', 'scale', 'valid_area', 'width_height'):
                 assert np.array_equal(np.asarray(meta[k], dtype=np.float64), np.asarray(mine[k], dtype=np.float64)), (k, meta[k], mine[k])
             # annotations: inverse_transform + json_data
