@@ -1955,15 +1955,10 @@ namespace {
 
 template <typename T>
 int net_alloc(pifpaf_net* net, T** p, size_t n, bool zero) {
-    cudaError_t e = cudaMalloc(reinterpret_cast<void**>(p), sizeof(T) * (n ? n : 1));
-    if (e != cudaSuccess) {
-        pifpaf::set_error("cudaMalloc of %zu bytes failed: %s", sizeof(T) * n, cudaGetErrorString(e));
-        return e == cudaErrorMemoryAllocation ? PIFPAF_E_NOMEM : PIFPAF_E_CUDA;
-    }
-    net->owned.push_back(*p);
+    PIFPAF_TRY(pifpaf::dev_alloc(p, n, net->owned));
     net->setup_synced = false;
     if (zero) {
-        e = cudaMemset(*p, 0, sizeof(T) * (n ? n : 1));
+        const cudaError_t e = cudaMemset(*p, 0, sizeof(T) * (n ? n : 1));
         if (e != cudaSuccess) { pifpaf::set_error("cudaMemset failed: %s", cudaGetErrorString(e)); return PIFPAF_E_CUDA; }
     }
     return PIFPAF_OK;
