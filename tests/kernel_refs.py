@@ -239,29 +239,6 @@ def op_ref(o, taps, heads, images, batch):
     return 'gemm plain', worst_ratio(out(N), ref, bound)
 
 
-def fused_rings(channels, n_out):
-    """(window ring, B ring) depths that pifpaf_net_dw_conv1x1_scatter picks for a fused depthwise -> 1x1 op.
-    Mirrors fused_smem_bytes, the candidate list {3,2},{2,2},{2,1},{1,1} and GEMM_SMEM_BUDGET of
-    openpifpaf_b200/csrc/net.cu; test_kernel_refs.py::test_fused_ring_plan_mirror_matches_net_cu fails when those
-    change, so the cases of test_kernels_gpu.py keep reaching every ring depth."""
-    def pad8(v):
-        return (v + 7) // 8 * 8
-
-    def pad16(v):
-        return (v + 15) // 16 * 16
-    C = pad8(channels)
-    nb = (n_out + 191) // 192                    # FD_MAX_BLOCK_N = 3 x 64 columns per CTA
-    bn = pad16((n_out + nb - 1) // nb)
-    window = 12 * 20 * 64 * 2                    # DwTile<1, 8, 16, 4, 1>::BYTES: (8+4) x (16+4) pixels x 64 channels
-    stg = 8 * 16 * 33 * 4                        # STG_BYTES
-    for ws, bs in ((3, 2), (2, 2), (2, 1), (1, 1)):
-        size = (1024 + 128 * 64 * 2 + bs * bn * 64 * 2 + ws * window + bn * nb * 5 + C * 26 * 4 + stg
-                + 2 * (ws + bs) * 8 + 64)
-        if size <= 222 * 1024:
-            return ws, bs
-    return None
-
-
 def written_columns(op, tensors):
     """(tensor, first column, end column) windows one op of network.build_ops writes ('heads' writes none of the
     activation tensors).  Plain outputs cover pad8(n) columns: the kernels store whole 8-channel vectors."""

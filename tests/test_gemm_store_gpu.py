@@ -53,6 +53,14 @@ PLAIN_CASES = [
     (41, 41, 1392, 240, 0, 32, False, 0, 1, 2),     # streaming weights
     (64, 64, 32, 174, 0, 0, False, 1, 3, 4),        # K = 32 (one half-filled K block), many tiles per CTA
     (41, 41, 704, 696, 0, 0, False, 1, 2, 3),       # 3 column blocks, tensor-bound stage-4 shape
+    # the plain plans of the shipped networks' 1x1s (tests/test_net_plan.py lists them)
+    (9, 11, 512, 128, 0, 0, False, 1, 2, 3),        # 2 x 64, resident 4
+    (9, 11, 256, 128, 0, 16, False, 0, 2, 3),       # 2 x 64, resident 8
+    (9, 11, 576, 160, 0, 0, False, 0, 2, 3),        # 3 x 64 - 32, streaming 5
+    (9, 11, 400, 348, 0, 0, False, 1, 2, 3),        # 176 x 2, resident 3
+    (9, 11, 208, 174, 0, 0, False, 1, 2, 3),        # 176, resident 7
+    (9, 11, 272, 256, 0, 0, False, 1, 2, 3),        # 256, streaming 4
+    (9, 11, 32, 256, 0, 0, False, 1, 2, 3),         # 256, resident 8
 ]
 
 
@@ -82,6 +90,21 @@ SCATTER_CASES = [
     # 9 destination tensors: more than the store maps, the per-lane epilogue
     (33, 35, 352, 144, [(16, i, 0) for i in range(9)], [16] * 9, 0, 3, 4),
     (33, 35, 352, 192, [(192, 0, 0)], [208], 1, 3, 4),
+    # 9 destination tensors in a 4-group tile (block_n = 256)
+    (13, 9, 176, 256, [(16, i, 16 * ((i + 1) % 2)) for i in range(8)] + [(128, 8, 0)], [32, 16] * 4 + [128], 1, 2, 3),
+] + [
+    # every instantiation (block_n = N = 16 .. 256): a 16-column piece at a column offset, the rest in another tensor
+    (9, 11, 72, n, [(16, 0, 16)] + ([(n - 16, 1, 0)] if n > 16 else []), [48, n + 16], n // 16 % 2, 2, 3)
+    for n in range(16, 257, 16)
+] + [
+    # the scatter plans of the shipped ShuffleNetV2K stage GEMMs (tests/test_net_plan.py lists them)
+    (9, 11, 256, 304, [(32, i, 0) for i in range(7)] + [(80, 7, 16)], [32] * 7 + [96], 1, 2, 3),   # 3 x 64 + 32, resident 7
+    (9, 11, 512, 528, [(64, i, 16) for i in range(6)] + [(144, 6, 0)], [80] * 6 + [144], 0, 2, 3),  # 176 x 3, streaming 5
+    (9, 11, 352, 400, [(48, i, 0) for i in range(6)] + [(112, 6, 16)], [48] * 6 + [128], 1, 2, 3),  # 208 x 2, streaming 4
+    (9, 11, 176, 208, [(48, 0, 0), (48, 1, 16), (64, 2, 0), (48, 3, 32)], [48, 64, 64, 80], 1, 2, 3),   # resident 7
+    (9, 11, 704, 704, [(224, 0, 0), (240, 1, 16), (240, 2, 0)], [224, 256, 240], 1, 2, 3),  # 240 x 3, streaming 4
+    (9, 11, 512, 512, [(256, 0, 0), (256, 1, 16)], [256, 272], 0, 2, 3),                   # 256 x 2, streaming 4
+    (9, 11, 256, 256, [(128, 0, 0), (128, 1, 0)], [128, 144], 1, 2, 3),                    # 256, resident 4
 ]
 
 
@@ -104,6 +127,9 @@ SCHEDULE_CASES = {
     'plain streaming': lambda: gemm_case(41, 41, 1392, 240, 0, 32, False, 0, 2, 3),
     'scatter resident': lambda: scatter_case(*SCATTER_CASES[6]),
     'scatter 8 maps': lambda: scatter_case(*SCATTER_CASES[4]),
+    'scatter 4 groups streaming': lambda: scatter_case(41, 43, 704, 704, [(224, 0, 0), (240, 1, 16), (240, 2, 0)],
+                                                       [224, 256, 240], 1, 2, 3),
+    'plain 3 groups resident 7': lambda: gemm_case(64, 64, 208, 174, 0, 0, False, 1, 3, 4),
 }
 
 

@@ -237,37 +237,6 @@ def test_every_tensor_column_is_written_by_one_op(base, layout, fuse):
             assert (owner[t][c0:c0 + n] < i).all(), (i, o['kind'], t)
 
 
-def test_fused_ring_plan_mirror_matches_net_cu():
-    """kernel_refs.fused_rings copies the shared-memory plan of the fused depthwise -> 1x1 op; the lines it copies
-    are still those of net.cu (change both together)"""
-    import os
-    import re
-    src = open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))),
-                            'openpifpaf_b200', 'csrc', 'net.cu')).read()
-    flat = re.sub(r'\s+', ' ', src)
-    for line in [
-        'size_t fused_smem_bytes(int ws, int bs, int block_n, int n_pad, int c_dw) { return 1024 + (size_t)BM * BK * 2 + '
-        '(size_t)bs * block_n * BK * 2 + (size_t)ws * DwTile<1, PH, PW, 4, 1>::BYTES + (size_t)n_pad * 5 + '
-        '(size_t)c_dw * 26 * 4 + STG_BYTES + (size_t)(2 * (ws + bs)) * 8 + 64; }',
-        'const int cand[][2] = {{3, 2}, {2, 2}, {2, 1}, {1, 1}};',
-        'if (fused_smem_bytes(c[0], c[1], block_n, n_pad, C) <= GEMM_SMEM_BUDGET)',
-        'const int n_blocks = (n_out + FD_MAX_BLOCK_N - 1) / FD_MAX_BLOCK_N;',
-        'const int block_n = pad16((n_out + n_blocks - 1) / n_blocks);',
-        'constexpr int FD_MAX_BLOCK_N = 3 * NGROUP;',
-        'constexpr size_t GEMM_SMEM_BUDGET = 222 * 1024;',
-        'constexpr int PH = 8, PW = 16;',
-        'static constexpr int IH = (TH - 1) * S + 5, IW = (TW - 1) * S + 5;',
-        'static constexpr int BYTES = IH * IW * 64 * 2;',
-        'constexpr int STG_LD = 33;',
-        'constexpr int STG_BYTES = CONSUMER_WARPS * 16 * STG_LD * 4;',
-        'constexpr int CONSUMER_WARPS = 8;',
-        'constexpr int BM = 128;',
-        'constexpr int BK = 64;',
-    ]:
-        assert line in flat, line
-    assert kr.fused_rings(176, 176) == (3, 2) and kr.fused_rings(1024, 192) == (1, 1)
-
-
 def _emulation_plan(name):
     import det_models
     import mobilenetv2_models as mm

@@ -17,6 +17,7 @@ import pytest
 import torch
 
 import kernel_refs as kr
+import net_plan
 from openpifpaf_b200 import _lib, constants, decoder, network, predictor
 from oracle import net_oracle
 
@@ -170,17 +171,27 @@ DW5_CASES = [
     (161, 161, 176, 5, 1, 2, 0, 0, 0, 2, 3),      # many items per CTA: the slot ring wraps many times
     (161, 161, 348, 5, 2, 2, 0, 0, 1, 5, 6),
 ]
-DWK_CASES = [                                      # k_dwconv: any other kernel
+# the other depthwise kernels: 3x3 runs DW_TMA[DW_K3_*], k_dwconv takes 7x7, dilations other than 2 and every
+# kernel but the 5x5 under gemm_impl = 1.  Optional trailing fields: (dilation, gemm_impl)
+DWK_CASES = [
     (13, 11, 20, 3, 1, 1, 0, 0, 1, 2, 3),
     (13, 11, 36, 3, 2, 1, 8, 16, 0, 1, 2),
     (17, 19, 44, 7, 1, 3, 0, 0, 0, 2, 3),
     (17, 19, 12, 7, 2, 3, 0, 8, 1, 3, 4),
     (6, 5, 72, 3, 2, 0, 0, 0, 1, 1, 2),
+    (13, 11, 24, 3, 1, 1, 8, 0, 2, 2, 3),              # ReLU6
+    (21, 19, 20, 3, 1, 3, 0, 8, 1, 2, 3, 3, 0),         # dilation 3
+    (23, 21, 36, 5, 1, 6, 0, 0, 0, 1, 2, 3, 0),         # 5x5, dilation 3
+    (17, 15, 44, 5, 1, 8, 8, 0, 1, 2, 3, 4, 0),         # 5x5, dilation 4
+    (12, 14, 24, 5, 2, 2, 0, 0, 2, 2, 3),               # 5x5 with ReLU6: k_dwconv5
+    (13, 11, 20, 3, 1, 1, 0, 16, 1, 2, 3, 1, 1),        # 3x3 under gemm_impl = 1: k_dwconv, stride 1
+    (13, 11, 36, 3, 2, 1, 8, 0, 2, 1, 2, 1, 1),         # ... stride 2
+    (29, 27, 72, 7, 2, 3, 0, 0, 1, 2, 3, 1, 1),
 ]
 
 
-def dw_case(H, W, C, k, stride, pad, in_off, out_off, relu, batch, mb, seed=0):
-    Ho, Wo = kr.out_hw(H, W, k, stride, pad)
+def dw_case(H, W, C, k, stride, pad, in_off, out_off, relu, batch, mb, dil=1, impl=0, seed=0):
+    Ho, Wo = kr.out_hw(H, W, (k - 1) * dil + 1, stride, pad)
     cin = pad16(in_off + pad8(C) + 8)
     cout = pad16(out_off + pad8(C) + 16)
     case = Case(mb, [(H, W, cin), (Ho, Wo, cout)], inputs={0}, seed=seed)
@@ -189,12 +200,13 @@ def dw_case(H, W, C, k, stride, pad, in_off, out_off, relu, batch, mb, seed=0):
     b = rng.standard_normal(C).astype(np.float32)
 
     def emit(L, net):
-        _lib.check(L.pifpaf_net_dwconv(net, 0, in_off, C, k, stride, pad, ptr(w), ptr(b), relu, 1, out_off))
+        _lib.check(L.pifpaf_net_dwconv_dilated(net, 0, in_off, C, k, stride, pad, ptr(w), ptr(b), relu, 1, out_off,
+                                               dil))
 
     x = case.data[0][:batch, ..., in_off:in_off + C]
-    ref, mag = kr.conv_ref(x, w.reshape(C, 1, k, k), b, stride, pad, groups=C)
+    ref, mag = kr.conv_ref(x, w.reshape(C, 1, k, k), b, stride, pad, groups=C, dilation=dil)
     ref, mag = kr.epilogue(ref, mag, relu)
-    chk = Check('dwconv k%d s%d' % (k, stride), batch)
+    chk = Check(dw_label(C, k, stride, relu, dil, impl), batch)
     chk.own(1, out_off, out_off + pad8(C))
     chk.compare(1, out_off, ref, kr.bf16_bound(ref, mag, k * k))
     if pad8(C) > C:       # padding channels: zero weight and bias
@@ -202,23 +214,28 @@ def dw_case(H, W, C, k, stride, pad, in_off, out_off, relu, batch, mb, seed=0):
     return case, emit, chk
 
 
+def dw_label(C, k, stride, relu, dil=1, impl=0):
+    """op kind of a depthwise case: its geometry and the kernel net.cu launches for it"""
+    return 'dwconv k%d s%d%s %s' % (k, stride, ' d%d' % dil if dil > 1 else '',
+                                    net_plan.dw_kernel(C, k, stride, relu, dil, gemm_impl=impl))
+
+
 def dw_id(c):
-    return 'H%dW%d-C%d-k%ds%dp%d-in%d-out%d-relu%d-B%dof%d' % c
+    return 'H%dW%d-C%d-k%ds%dp%d-in%d-out%d-relu%d-B%dof%d' % c[:11] + ('-d%d-impl%d' % c[11:] if len(c) > 11 else '')
 
 
 @pytest.mark.parametrize('impl', [0, 1], ids=['tma', 'simt'])
 @pytest.mark.parametrize('c', DW5_CASES, ids=dw_id)
 def test_dwconv5_matches_float64(c, impl):
-    case, emit, chk = dw_case(*c)
+    case, emit, chk = dw_case(*c, impl=impl)
     taps, _ = case.run(emit, c[9], impl=impl)
-    chk.kind += ' tma' if impl == 0 else ' simt'
     print(dw_id(c), impl, '%.3f' % chk.verify(taps, dw_id(c)))
 
 
 @pytest.mark.parametrize('c', DWK_CASES, ids=dw_id)
 def test_dwconv_generic_matches_float64(c):
     case, emit, chk = dw_case(*c)
-    taps, _ = case.run(emit, c[9])
+    taps, _ = case.run(emit, c[9], impl=c[12] if len(c) > 12 else 0)
     print(dw_id(c), '%.3f' % chk.verify(taps, dw_id(c)))
 
 
@@ -238,7 +255,7 @@ def test_dwconv5_stride2_channel_block_fastest(C, monkeypatch):
 
 
 # ---------------------------------------------------------------------------------------------------- fused dw -> 1x1
-fused_rings = kr.fused_rings
+fused_rings = net_plan.fused_rings
 
 
 # (H, W, channels, n_out, pieces [(count, dest, col)], dest widths, dw_relu, relu, batch, max_batch)
@@ -298,6 +315,10 @@ def test_fused_dw_gemm_matches_float64(c):
 
 # ---------------------------------------------------------------------------------------------------- dense conv
 # (H, W, c_in, kernel, stride, pad, n_out, in_off, residual col (None: no residual), relu, out_off, batch, max_batch)
+# n_out whose tiles are 16, 32, ..., 256 columns wide: every (column groups, last group width) instantiation of
+# k_gemm_wg, in order (1 x 16 ... 4 x 64); N = bn - 10 leaves a partial last 16-column group
+TILE_WIDTHS = [16, 22, 44, 64, 70, 92, 108, 124, 140, 150, 174, 188, 208, 214, 236, 256]
+
 CONV_CASES = [
     (9, 11, 64, 1, 2, 0, 32, 0, None, 0, 0, 1, 2),        # 1x1 stride 2 (ResNet downsample)
     (17, 19, 64, 3, 1, 1, 64, 0, 16, 1, 0, 2, 3),         # residual at a column offset
@@ -311,6 +332,26 @@ CONV_CASES = [
     (57, 61, 64, 3, 1, 1, 128, 0, 0, 1, 0, 2, 3),         # 40 patches per image
     (11, 13, 136, 1, 1, 0, 120, 8, 24, 1, 0, 2, 3),       # 1x1 stride 1 with residual: the pointwise GEMM route
     (11, 13, 136, 1, 1, 0, 120, 8, 24, 0, 16, 2, 3),
+    (15, 17, 128, 1, 2, 0, 96, 0, None, 1, 0, 2, 3),      # 2 K blocks: a 4-deep ring
+    (17, 19, 64, 1, 2, 0, 128, 0, None, 1, 0, 2, 3),      # 1 K block: a 2-deep ring (ResNet's 128-wide downsample)
+    # the pointwise plans of the shipped MobileNetV2 and ResNet-50 (tests/test_net_plan.py lists them)
+    (9, 11, 160, 1, 1, 0, 960, 0, None, 2, 0, 2, 3),      # ReLU6, 4 x 240, resident 6
+    (7, 9, 320, 1, 1, 0, 1280, 0, None, 2, 0, 2, 3),      # ReLU6, 5 x 256, streaming 4
+    (9, 11, 576, 1, 1, 0, 96, 0, 0, 0, 0, 2, 3),          # residual, 96, resident 5
+    (9, 11, 960, 1, 1, 0, 160, 0, 0, 0, 0, 2, 3),         # residual, 160, streaming 5
+    (7, 9, 512, 1, 1, 0, 2048, 0, 0, 1, 0, 2, 3),         # residual, 8 x 256, streaming 4
+    (9, 11, 256, 1, 1, 0, 1024, 0, 0, 1, 0, 2, 3),        # residual, 4 x 256, resident 4
+    (9, 11, 64, 1, 1, 0, 256, 0, 0, 1, 0, 2, 3),          # residual, 256, resident 8
+] + [
+    # every instantiation of the pointwise route with the per-lane residual epilogue (activation codes 0 / 1 / 2)
+    (11, 13, 136, 1, 1, 0, n, 8, 16, i % 3, 0, 2, 3) for i, n in enumerate(TILE_WIDTHS)
+] + [
+    # every instantiation of the implicit GEMM, 3x3 at stride 1 and 2: plain, ReLU6, residual (codes 0 / 1 / 2)
+    (11, 13, 72, 3, 1 + i % 2, 1, n, 8, None, 1, 16, 2, 3) for i, n in enumerate(TILE_WIDTHS)
+] + [
+    (12, 10, 64, 3, 2 - i % 2, 1, n, 0, None, 2, 0, 1, 2) for i, n in enumerate(TILE_WIDTHS)
+] + [
+    (10, 13, 64, 3, 1 + i % 2, 1, n, 0, 8, i % 3, 0, 2, 3) for i, n in enumerate(TILE_WIDTHS)
 ]
 
 
@@ -327,7 +368,7 @@ def conv_case(H, W, c_in, k, stride, pad, N, in_off, res_col, relu, out_off, bat
         inputs.add(2)
     case = Case(mb, tensors, inputs=inputs, seed=seed)
     rng = np.random.default_rng(seed + 3)
-    w = kr.random_bf16(rng, (N, c_in, k, k), 1 / np.sqrt(c_in * k * k))
+    w = kr.random_bf16(rng, (N, c_in, k, k), (4 if relu == 2 else 1) / np.sqrt(c_in * k * k))     # ReLU6: past 6
     b = rng.standard_normal(N).astype(np.float32)
 
     def emit(L, net):
@@ -337,7 +378,7 @@ def conv_case(H, W, c_in, k, stride, pad, N, in_off, res_col, relu, out_off, bat
     ref, mag = kr.conv_ref(case.data[0][:batch, ..., in_off:in_off + c_in], w, b, stride, pad)
     res = None if res_col is None else case.data[2][:batch, ..., res_col:res_col + N]
     ref, mag = kr.epilogue(ref, mag, relu, res)
-    chk = Check('conv k%d' % k, batch)
+    chk = Check('conv k%d' % k + (' relu6' if relu == 2 else ''), batch)
     chk.own(1, out_off, out_off + pad8(N))
     chk.compare(1, out_off, ref, kr.bf16_bound(ref, mag, c_in * k * k))
     if res_col is None and pad8(N) > N:
@@ -436,6 +477,24 @@ GEMM_CASES = [
     (41, 41, 1392, 240, 0, 32, False, 0, 1, 2),        # streaming weights
     (64, 64, 352, 176, 0, 0, False, 0, 3, 4),
     (161, 161, 176, 174, 0, 0, True, 1, 1, 2),         # pass-through double buffer wraps
+    # streaming weights (K = 1392) at ring depths 8 / 7 / 6, and 2 (a 224-column shuffle tile and its pass-through buffer)
+    (17, 19, 1392, 64, 0, 0, False, 0, 1, 2),
+    (17, 19, 1392, 96, 0, 16, False, 1, 2, 3),
+    (17, 19, 1392, 128, 0, 0, False, 0, 1, 2),
+    (17, 19, 1392, 224, 0, 0, True, 1, 1, 2),
+    # shuffle with the pass-through tile read per lane: 240 / 256-column tiles, and 4 blocks of 224 columns whose bias
+    # and scatter tables leave no room for the double buffer
+    (13, 11, 176, 236, 0, 0, True, 0, 2, 3),
+    (13, 11, 176, 256, 0, 0, True, 1, 2, 3),
+    (9, 11, 96, 896, 0, 0, True, 1, 2, 3),
+    # the shuffle plans of the shipped k16 / k30 stage GEMMs without src_tma (tests/test_net_plan.py lists them)
+    (9, 11, 704, 696, 0, 0, True, 1, 2, 3),            # 240 x 3, streaming 4
+    (9, 11, 512, 512, 0, 0, True, 1, 2, 3),            # 256 x 2, streaming 4
+    (9, 11, 256, 256, 0, 0, True, 0, 2, 3),            # 256, resident 4
+] + [
+    (9, 11, 72, n, 0, 0, True, i % 2, 2, 3) for i, n in enumerate(TILE_WIDTHS[:14])     # shuffle, src_tma
+] + [
+    (9, 11, 72, n, 0, 16 * (i % 2), False, 2, 2, 3) for i, n in enumerate(TILE_WIDTHS)  # ReLU6: per-lane epilogue
 ]
 
 
@@ -451,7 +510,7 @@ def gemm_case(h, w, K, N, in_off, out_off, shuffle, relu, batch, mb, seed=0):
         inputs.add(2)
     case = Case(mb, tensors, inputs=inputs, seed=seed)
     rng = np.random.default_rng(seed + 5)
-    wt = kr.random_bf16(rng, (N, K), 1 / np.sqrt(K))
+    wt = kr.random_bf16(rng, (N, K), (4 if relu == 2 else 1) / np.sqrt(K))      # ReLU6: outputs past 6
     b = rng.standard_normal(N).astype(np.float32)
 
     def emit(L, net):
@@ -461,7 +520,7 @@ def gemm_case(h, w, K, N, in_off, out_off, shuffle, relu, batch, mb, seed=0):
     ref, mag = kr.conv_ref(case.data[0][:batch, ..., in_off:in_off + K], wt[:, :, None, None], b, 1, 0)
     ref, mag = kr.epilogue(ref, mag, relu)
     bound = kr.bf16_bound(ref, mag, K)
-    chk = Check('gemm ' + ('shuffle' if shuffle else 'plain'), batch)
+    chk = Check('gemm ' + ('shuffle' if shuffle else 'plain') + (' relu6' if relu == 2 else ''), batch)
     if shuffle:
         chk.own(1, 0, 2 * N)
         chk.compare(1, 1, ref, bound, step=2)
@@ -545,21 +604,35 @@ def test_gemm_res_stages_retiling(c, monkeypatch):
 
 # ---------------------------------------------------------------------------------------------------- heads
 WHOLEBODY = ((133, 1, 1, 1), (160, 1, 2, 2))       # 133 x 5 + 160 x 8 = 1945 columns
-# (h, w, K, heads [(n_fields, n_conf, n_vec, n_scales)] or 'all' (one head with every comp op), batch, max_batch)
+# (h, w, K, heads [(n_fields, n_conf, n_vec, n_scales)] or 'all' (one head with every comp op), batch, max_batch,
+# optional upsample stride); a head has 1 + n_conf + 2 n_vec + n_scales components, each of up^2 conv columns
 HEADS_CASES = [
     (9, 13, 136, ((17, 1, 1, 1), (19, 1, 2, 2)), 2, 3),     # N = 237; 117 pixels per image: tiles span two images
     (9, 11, 200, WHOLEBODY, 2, 3),
     (5, 7, 72, 'all', 3, 4),
     (16, 8, 64, ((3, 1, 1, 1),), 1, 2),                      # N = 15, exactly one 128-row tile per image
+    (7, 9, 256, ((3, 1, 1, 1),), 2, 3),                      # K = 256: an 8-deep ring
+    (7, 9, 256, ((19, 1, 1, 1),), 2, 3),                     # 96-column tile: 7 deep
+    (7, 9, 256, ((25, 1, 1, 1),), 2, 3),                     # 128: 6 deep
+    (7, 9, 256, ((35, 1, 1, 1),), 2, 3),                     # 176: 5 deep
+    # several n blocks, a 5-component field straddling each block boundary (up = 1, 2), and a 3 x 3 sub-pixel group
+    # straddling it (up = 3: 45 columns per field, 160-column blocks)
+    (6, 7, 72, ((37, 1, 1, 1),), 2, 3, 2),
+    (5, 6, 72, ((7, 1, 1, 1),), 2, 3, 3),
+    (5, 6, 136, ((17, 1, 1, 1), (19, 1, 2, 2)), 1, 2, 3),
+] + [
+    (7, 5, 72, (((bn - 3) // 5, 1, 1, 1),), 2, 3) for bn in range(16, 257, 16)     # every instantiation
+] + [
+    (5, 4, 72, ((bn // 8, 1, 0, 0),), 2, 3, 2) for bn in range(16, 257, 16)        # upsampled, every instantiation
 ]
 
 
 def heads_id(c):
     return 'hw%dx%d-K%d-%s-B%dof%d' % (c[0], c[1], c[2], 'all' if c[3] == 'all' else 'x'.join(str(h[0]) for h in c[3]),
-                                       c[4], c[5])
+                                       c[4], c[5]) + ('-up%d' % c[6] if len(c) > 6 else '')
 
 
-def heads_case(h, w, K, spec, batch, mb, seed=0):
+def heads_case(h, w, K, spec, batch, mb, up=1, seed=0):
     if spec == 'all':
         n_fields, n_comp, ops = [3], [6], [0, 1, 2, 3, 4, 1]
     else:
@@ -567,7 +640,7 @@ def heads_case(h, w, K, spec, batch, mb, seed=0):
         ops_h = [network.head_ops(s[1], s[2], s[3], (True,) * s[2]) for s in spec]
         n_comp = [len(o) for o in ops_h]
         ops = [o for oh in ops_h for o in oh]
-    N = sum(f * c for f, c in zip(n_fields, n_comp))
+    N = sum(f * c for f, c in zip(n_fields, n_comp)) * up * up
     case = Case(mb, [(h, w, pad16(K + 8))], inputs={0}, seed=seed)
     rng = np.random.default_rng(seed + 7)
     wt = kr.random_bf16(rng, (N, K), 2 / np.sqrt(K))
@@ -575,21 +648,21 @@ def heads_case(h, w, K, spec, batch, mb, seed=0):
 
     def emit(L, net):
         n = len(n_fields)
-        _lib.check(L.pifpaf_net_heads(net, 0, K, n, i32(n_fields).ctypes.data_as(ctypes.c_void_p),
-                                      i32(n_comp).ctypes.data_as(ctypes.c_void_p),
-                                      i32(ops).ctypes.data_as(ctypes.c_void_p), ptr(wt), ptr(b)))
+        _lib.check(L.pifpaf_net_heads_upsampled(net, 0, K, n, i32(n_fields).ctypes.data_as(ctypes.c_void_p),
+                                                i32(n_comp).ctypes.data_as(ctypes.c_void_p),
+                                                i32(ops).ctypes.data_as(ctypes.c_void_p), up, ptr(wt), ptr(b)))
         return n
 
-    refs = kr.heads_ref(case.data[0][:batch, ..., :K], wt, b, n_fields, n_comp, ops)
+    refs = kr.heads_ref(case.data[0][:batch, ..., :K], wt, b, n_fields, n_comp, ops, up)
     return case, emit, refs
 
 
-def verify_heads(heads, refs, batch, what=''):
+def verify_heads(heads, refs, batch, what='', kind='heads'):
     worst = 0.0
     for hb, (ref, bound) in zip(heads, refs):
         assert (hb[batch:] == kr.SENTINEL).all(), f'heads {what}: wrote image >= batch'
         worst = max(worst, kr.worst_ratio(hb[:batch], ref, bound))
-    record('heads', worst, what)
+    record(kind, worst, what)
     return worst
 
 
@@ -598,7 +671,8 @@ def verify_heads(heads, refs, batch, what=''):
 def test_heads_match_float64(c, impl):
     case, emit, refs = heads_case(*c)
     _, heads = case.run(emit, c[4], impl=impl)
-    print(heads_id(c), impl, '%.3f' % verify_heads(heads, refs, c[4], heads_id(c)))
+    kind = 'heads upsampled' if len(c) > 6 else 'heads'
+    print(heads_id(c), impl, '%.3f' % verify_heads(heads, refs, c[4], heads_id(c), kind))
 
 
 # ---------------------------------------------------------------------------------------------------- schedules
@@ -608,16 +682,24 @@ SCHEDULE_CASES = {           # name -> (case factory, gemm_impl)
     'dw_gemm 1 block': (lambda: fused_case(*FUSED_CASES[-1]), 0),
     'dw_gemm 3 blocks': (lambda: fused_case(*FUSED_CASES[6]), 0),
     'conv 3x3': (lambda: conv_case(*CONV_CASES[9]), 0),
-    'gemm shuffle': (lambda: gemm_case(*GEMM_CASES[-1]), 0),
+    'gemm shuffle': (lambda: gemm_case(*GEMM_CASES[6]), 0),
     'gemm plain': (lambda: gemm_case(*GEMM_CASES[5]), 0),
     'gemm scatter resident': (lambda: scatter_case(*SCATTER_CASES[5]), 0),
     'gemm scatter streaming': (lambda: scatter_case(*SCATTER_CASES[2]), 0),
     'heads': (lambda: heads_case(41, 41, 136, ((17, 1, 1, 1), (19, 1, 2, 2)), 3, 3), 0),
+    'heads upsampled': (lambda: heads_case(21, 23, 72, ((7, 1, 1, 1),), 3, 3, 3), 0),
+    'conv 3x3 4 groups residual relu6': (lambda: conv_case(41, 43, 64, 3, 2, 1, 236, 0, 8, 2, 0, 2, 3), 0),
+    'conv 1x1 residual': (lambda: conv_case(57, 61, 136, 1, 1, 0, 188, 8, 16, 1, 0, 2, 3), 0),
+    'gemm relu6': (lambda: gemm_case(64, 64, 352, 214, 0, 16, False, 2, 3, 4), 0),
+    'gemm shuffle lane src': (lambda: gemm_case(61, 67, 176, 256, 0, 0, True, 1, 2, 3), 0),
+    'gemm streaming 8 stages': (lambda: gemm_case(41, 41, 1392, 64, 0, 0, False, 0, 2, 3), 0),
     'input_conv': (lambda: stem_case(161, 161, 3, 2, 1, 24, False, 3, 3), 0),
     # grid-stride kernels whose grids also follow the SM count: k_dwconv5, k_dwconv, k_gemm_simt
-    'dwconv5 s1 simt': (lambda: dw_case(61, 67, 176, 5, 1, 2, 0, 0, 0, 2, 3), 1),
-    'dwconv5 s2 simt': (lambda: dw_case(61, 67, 348, 5, 2, 2, 0, 0, 1, 2, 3), 1),
-    'dwconv k3 generic': (lambda: dw_case(61, 67, 72, 3, 2, 1, 0, 0, 1, 2, 3), 0),
+    'dwconv5 s1 simt': (lambda: dw_case(61, 67, 176, 5, 1, 2, 0, 0, 0, 2, 3, impl=1), 1),
+    'dwconv5 s2 simt': (lambda: dw_case(61, 67, 348, 5, 2, 2, 0, 0, 1, 2, 3, impl=1), 1),
+    'dwconv k3 s2 tma': (lambda: dw_case(61, 67, 72, 3, 2, 1, 0, 0, 1, 2, 3), 0),
+    'dwconv k7 generic': (lambda: dw_case(61, 67, 72, 7, 2, 3, 0, 0, 1, 2, 3), 0),
+    'dwconv k3 d3 generic': (lambda: dw_case(61, 67, 40, 3, 1, 3, 0, 0, 1, 2, 3, 3), 0),
     'conv 3x3 simt': (lambda: conv_case(*CONV_CASES[9]), 1),
     'gemm plain simt': (lambda: gemm_case(*GEMM_CASES[5]), 1),
     'gemm scatter simt': (lambda: scatter_case(*SCATTER_CASES[1]), 1),
