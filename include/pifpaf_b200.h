@@ -234,6 +234,43 @@ int pifpaf_image_fill_rgb(uint8_t* dst_dev, int64_t n_pixels, int32_t r, int32_t
 
 
 /* ------------------------------------------------------------------------ */
+/* Baseline JPEG decode, bit-identical to PIL.Image.open(f).convert('RGB') (datasets/image_list.py:18; Pillow's
+ * libjpeg-turbo: islow IDCT, fancy upsampling, fixed-point YCbCr->RGB).  The GPU decodes Huffman-coded sequential
+ * frames (SOF0 / SOF1) with 8-bit samples in one scan: grayscale, or YCbCr (JFIF, Adobe transform 1 or no colour
+ * marker) sampled 4:4:4, 4:2:2 or 4:2:0, components in frame order, with any DQT / DHT (every table the scan
+ * selects defined) and restart intervals.  Every other stream is routed to
+ * Pillow (PIFPAF_JPEG_PILLOW) and left to the caller.  Capacities are fixed at create; decode allocates nothing, is
+ * stream-ordered and not re-entrant. */
+typedef struct pifpaf_jpeg pifpaf_jpeg_t;
+
+#define PIFPAF_JPEG_GPU 0
+#define PIFPAF_JPEG_PILLOW 1
+
+/* max_images per decode, max_bytes of entropy-coded scan data per decode, max_pixels (w * h) per image, max_blocks
+ * 8x8 blocks per decode (summed over its GPU-route images: MCUs x blocks per MCU, the MCU grid covering the image;
+ * the coefficient and sample planes are sized by it). */
+int pifpaf_jpeg_create(pifpaf_jpeg_t** out, int32_t device, int32_t max_images, int64_t max_bytes, int64_t max_pixels,
+                       int64_t max_blocks);
+void pifpaf_jpeg_destroy(pifpaf_jpeg_t* jpeg);
+
+/* Decode n HOST streams data[i] of sizes[i] bytes, enqueued on `stream`.  GPU-route image i is written as uint8
+ * [h][w][3] at out_dev + out_offsets[i] (out_bytes: capacity of out_dev); routes[i] = PIFPAF_JPEG_GPU or
+ * PIFPAF_JPEG_PILLOW; hw[2i], hw[2i+1] = height, width (0 for the Pillow route, whose out_offsets[i] is -1).
+ * max_rounds caps the self-synchronising Huffman decode's rounds (-1: default; 0: every subsequence decoded
+ * serially); any cap gives the same image.  Every stream is parsed and validated first: a malformed or truncated
+ * stream, or a batch over the capacities, returns PIFPAF_E_BADARG with a message naming the stream and launches and
+ * writes nothing on the device.  The host buffers may be reused when the call returns. */
+int pifpaf_jpeg_decode(pifpaf_jpeg_t* jpeg, int32_t n, const uint8_t* const* data, const int64_t* sizes,
+                       uint8_t* out_dev, int64_t out_bytes, int32_t max_rounds,
+                       int32_t* routes, int32_t* hw, int64_t* out_offsets, void* stream);
+
+/* Counters of the last decode (synchronises its stream): stats[0] images decoded on the GPU, [1] images routed to
+ * Pillow, [2] subsequence slots, [3] self-synchronisation rounds that decoded something, [4] serial fallback decodes
+ * (subsequences still unsettled after the last round). */
+int pifpaf_jpeg_last_stats(pifpaf_jpeg_t* jpeg, int64_t* stats, int32_t n_stats);
+
+
+/* ------------------------------------------------------------------------ */
 /* Network forward: backbone + CompositeField4 heads (network/nets.py:35-48,
  * network/basenetworks.py:186-355, network/heads.py:272-378), as a list of fused
  * ops over NHWC bf16 activation tensors.  The host mirror of the reference

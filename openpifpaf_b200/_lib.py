@@ -73,6 +73,11 @@ SYMBOLS = {
     'pifpaf_image_resize_bilinear_u8': (ctypes.c_int, [VP, c_i32, c_i32, VP, c_i64, c_i32, c_i32, VP, VP, c_i32,
                                                         VP, VP, c_i32, VP, VP]),
     'pifpaf_image_fill_rgb': (ctypes.c_int, [VP, c_i64, c_i32, c_i32, c_i32, VP]),
+    'pifpaf_jpeg_create': (ctypes.c_int, [P(VP), c_i32, c_i32, c_i64, c_i64, c_i64]),
+    'pifpaf_jpeg_destroy': (None, [VP]),
+    'pifpaf_jpeg_decode': (ctypes.c_int, [VP, c_i32, P(VP), P(c_i64), VP, c_i64, c_i32, P(c_i32), P(c_i32), P(c_i64),
+                                          VP]),
+    'pifpaf_jpeg_last_stats': (ctypes.c_int, [VP, P(c_i64), c_i32]),
     'pifpaf_net_create': (ctypes.c_int, [P(VP), c_i32, c_i32]),
     'pifpaf_net_destroy': (None, [VP]),
     'pifpaf_net_tensor': (ctypes.c_int, [VP, c_i32, c_i32, c_i32, P(c_i32)]),

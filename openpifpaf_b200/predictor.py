@@ -83,6 +83,9 @@ class Predictor:
         torch.cuda.synchronize(self.device)
         self.decoder._free()
         self.net.close()
+        if getattr(self, '_jpeg', None) is not None:
+            self._jpeg.close()
+            self._jpeg = None
 
     def fields_batch(self, image_batch):
         """decoder/decoder.py:76-112 without the .cpu(): returns device-resident head tensors."""
@@ -182,6 +185,40 @@ class Predictor:
                     out.append((data, scales, meta))
         return out
 
+    def jpeg_images(self, files_or_bytes, *, json_data=False, fill=None, score_weights=None):
+        """`raw_images` of the JPEG files (paths or bytes) decoded like the reference's Predictor.images
+        (PIL.Image.open(f).convert('RGB'), datasets/image_list.py:18), but on the GPU (`preprocess.GpuJpegDecoder`;
+        streams it does not decode are decoded by Pillow).  Chunked by max_batch; each chunk's decode is enqueued on
+        the predictor's stream ahead of its resize.  Returns what raw_images returns, per file."""
+        files = list(files_or_bytes)
+        if isinstance(fill, list) and len(fill) != len(files):
+            raise RuntimeError(f'fill has {len(fill)} colours for {len(files)} images')
+        out = []
+        for chunk, chunk_fill in raw_image_chunks(files, self.net.max_batch, fill):
+            datas = [_preprocess.read_stream(f) for f in chunk]
+            dec = self._jpeg_decoder(datas)
+            images, _ = dec(datas, stream=self.stream, host_pillow=True)
+            out.extend(self.raw_images(images, json_data=json_data, fill=chunk_fill, score_weights=score_weights))
+        return out
+
+    def _jpeg_decoder(self, datas):
+        """the JPEG decoder, sized from the chunk's frame headers; re-created (after the work in flight) when a chunk
+        does not fit, at the larger of the old capacities and the chunk's needs"""
+        fp = [_preprocess.jpeg_footprint(d) for d in datas]
+        need = (len(datas), sum(len(d) for d in datas), max(p for p, _ in fp), sum(b for _, b in fp),
+                sum(p for p, _ in fp))
+        dec = getattr(self, '_jpeg', None)
+        if dec is None or not dec.fits(*need):
+            old = (0, 0, 0, 0)
+            if dec is not None:
+                torch.cuda.synchronize(self.device)
+                dec.close()
+                old = (dec.max_bytes, dec.max_pixels, dec.max_blocks, dec.out_pixels)
+            self._jpeg = _preprocess.GpuJpegDecoder(
+                self.net.max_batch, max(need[1], old[0]), max(need[2], old[1], 1), max_blocks=max(need[3], old[2], 1),
+                out_pixels=max(need[4], old[3], 1), device=self.device.index)
+        return self._jpeg
+
     def batches(self, host_batches):
         """Pipelined variant of `batch` over an iterable of host image batches (what Predictor.dataloader /
         enumerated_dataloader does in the reference, predictor.py:118-153): the H2D copy of batch i+1 runs on a
@@ -244,6 +281,10 @@ class DetPredictor(Predictor):
 
     def raw_images(self, images, **kwargs):
         raise RuntimeError('raw_images() is not implemented for detection (no inverse transform of boxes); '
+                           'preprocess on the host and call batch()')
+
+    def jpeg_images(self, files_or_bytes, **kwargs):
+        raise RuntimeError('jpeg_images() is not implemented for detection (no inverse transform of boxes); '
                            'preprocess on the host and call batch()')
 
 

@@ -12,10 +12,13 @@ Reference (paths relative to the reference's src/openpifpaf/):
 (pifpaf_image_resize_bilinear_u8; Pillow's ImagingResample restated, this module builds its coefficient tables) straight
 into the centre of a padded uint8 canvas, and returns the canvas -- the input of `CompiledNet.forward_uint8`, whose stem
 applies ToTensor + Normalize -- together with the per-image `meta` dicts the reference's transforms would have produced.
+`GpuJpegDecoder` decodes baseline JPEG files on the GPU bit-identically to PIL.Image.open(f).convert('RGB')
+(datasets/image_list.py:18), the step before them; streams the GPU does not decode are decoded by Pillow.
 `inverse_transform_batch` / `json_data_batch` are the array forms of `Annotation.inverse_transform` / `json_data` for all
 annotations of an image at once (same float32 / float64 roundings as the reference under numpy 2).
 """
 import ctypes
+import io
 import math
 import numbers
 
@@ -230,6 +233,124 @@ class GpuPreprocess:
                 metas.append(reference_meta(w, h, tw, th, np.asarray(ltrb), rescaled=self.long_edge is not None))
             self._keepalive = keep
         return canvas, metas
+
+
+# ----------------------------------------------------------------------------------------------------- JPEG decode
+def read_stream(f):
+    """a path or a bytes-like JPEG stream -> bytes"""
+    if isinstance(f, (bytes, bytearray, memoryview)):
+        return bytes(f)
+    with open(f, 'rb') as fh:
+        return fh.read()
+
+
+def pillow_rgb(data):
+    """the reference's decode (datasets/image_list.py:18): uint8 [h, w, 3]"""
+    from PIL import Image
+    with Image.open(io.BytesIO(data)) as im:
+        return np.asarray(im.convert('RGB'))
+
+
+def jpeg_footprint(data):
+    """(w * h, 8x8 blocks of the MCU grid) of a JPEG stream as pifpaf_jpeg_decode lays it out, from its frame header
+    (Pillow's parse; (0, 0) if Pillow cannot open it -- the decoder then reports why).  Sizes `GpuJpegDecoder` for a
+    batch exactly."""
+    from PIL import Image
+    try:
+        with Image.open(io.BytesIO(data)) as im:
+            w, h = im.size
+            layer = list(getattr(im, 'layer', None) or [])          # (id, h sampling, v sampling, table) per component
+    except Exception:                                                  # not an image Pillow can open
+        return 0, 0
+    if len(layer) <= 1:                                                # one component: one block per MCU
+        return w * h, -(-w // 8) * -(-h // 8)
+    hmax, vmax = max(c[1] for c in layer), max(c[2] for c in layer)
+    mcus = -(-w // (8 * hmax)) * -(-h // (8 * vmax))
+    return w * h, mcus * sum(c[1] * c[2] for c in layer)
+
+
+class GpuJpegDecoder:
+    """Decode JPEG files or byte strings on the GPU (pifpaf_jpeg_decode), bit-identically to
+    PIL.Image.open(f).convert('RGB').  Baseline / extended-sequential Huffman streams with 8-bit samples in one scan,
+    grayscale or YCbCr 4:4:4 / 4:2:2 / 4:2:0, take the 'gpu' route; every other stream (progressive, arithmetic,
+    CMYK, Adobe RGB, 4:4:0, ...) the 'pillow' route, decoded by Pillow on the host like the reference.
+
+    :param max_images: images per call
+    :param max_bytes: entropy-coded bytes per call (the scans of all streams of a call)
+    :param max_pixels: w * h of the largest image
+    :param max_blocks: 8x8 blocks per call, summed over its images (`jpeg_footprint`); default: max_images images of
+                       max_pixels pixels on a square MCU grid at 4:4:4
+    :param out_pixels: pixels per call, summed over its images (the output buffer); default max_images * max_pixels
+    The returned GPU-route images are views of one output buffer, valid until the next call."""
+
+    def __init__(self, max_images, max_bytes, max_pixels, *, max_blocks=None, out_pixels=None, device=0):
+        self.device = torch.device('cuda', device)
+        self.max_images, self.max_bytes, self.max_pixels = int(max_images), int(max_bytes), int(max_pixels)
+        if max_blocks is None:
+            side = -(-math.isqrt(self.max_pixels - 1) // 8) + 1 if self.max_pixels > 1 else 1
+            max_blocks = self.max_images * 3 * side * side
+        self.max_blocks = int(max_blocks)
+        self.out_pixels = int(out_pixels) if out_pixels is not None else self.max_images * self.max_pixels
+        self._handle = ctypes.c_void_p()
+        _lib.check(_lib.lib().pifpaf_jpeg_create(ctypes.byref(self._handle), device, self.max_images,
+                                                 self.max_bytes, self.max_pixels, self.max_blocks))
+        self._out = torch.empty((self.out_pixels * 3,), dtype=torch.uint8, device=self.device)
+        self.last_routes = []
+
+    def fits(self, n_images, n_bytes, max_pixels, n_blocks, n_pixels):
+        """can one call take n_images streams of n_bytes in all, the largest of max_pixels, n_blocks and n_pixels
+        summed (`jpeg_footprint`)"""
+        return (n_images <= self.max_images and n_bytes <= self.max_bytes and max_pixels <= self.max_pixels
+                and n_blocks <= self.max_blocks and n_pixels <= self.out_pixels)
+
+    def __call__(self, files_or_bytes, *, max_rounds=-1, stream=None, host_pillow=False):
+        """-> (images, routes): per stream a uint8 [h, w, 3] image (CUDA; with host_pillow the Pillow-route images
+        stay host numpy arrays) and 'gpu' or 'pillow'.  The GPU decode is enqueued on `stream` (default: the current
+        stream).  max_rounds caps the self-synchronising Huffman decode (-1: default, 0: serial); the images do not
+        depend on it.  A malformed stream raises RuntimeError before anything is enqueued."""
+        datas = [read_stream(f) for f in files_or_bytes]
+        n = len(datas)
+        st = stream if stream is not None else torch.cuda.current_stream(self.device)
+        ptrs = (ctypes.c_void_p * max(n, 1))(*[ctypes.cast(ctypes.c_char_p(d), ctypes.c_void_p) for d in datas])
+        sizes = (ctypes.c_int64 * max(n, 1))(*[len(d) for d in datas])
+        routes = (ctypes.c_int32 * max(n, 1))()
+        hw = (ctypes.c_int32 * max(2 * n, 1))()
+        offs = (ctypes.c_int64 * max(n, 1))()
+        _lib.check(_lib.lib().pifpaf_jpeg_decode(self._handle, n, ptrs, sizes, self._out.data_ptr(), self._out.numel(),
+                                                 int(max_rounds), routes, hw, offs, ctypes.c_void_p(st.cuda_stream)))
+        images, names = [], []
+        for i in range(n):
+            if routes[i] == 0:
+                h, w, o = hw[2 * i], hw[2 * i + 1], offs[i]
+                images.append(self._out[o:o + h * w * 3].view(h, w, 3))
+                names.append('gpu')
+            else:
+                img = pillow_rgb(datas[i])
+                if not host_pillow:
+                    with torch.cuda.stream(st):
+                        img = torch.from_numpy(np.ascontiguousarray(img)).to(self.device)
+                images.append(img)
+                names.append('pillow')
+        self.last_routes = names
+        return images, names
+
+    def stats(self):
+        """counters of the last call (synchronises): images per route, subsequences, self-synchronisation rounds that
+        decoded something, serial fallback decodes"""
+        s = (ctypes.c_int64 * 5)()
+        _lib.check(_lib.lib().pifpaf_jpeg_last_stats(self._handle, s, 5))
+        return dict(gpu=s[0], pillow=s[1], subsequences=s[2], sync_rounds=s[3], fallbacks=s[4])
+
+    def close(self):
+        if self._handle:
+            _lib.lib().pifpaf_jpeg_destroy(self._handle)
+            self._handle = ctypes.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:                   # interpreter shutdown
+            pass
 
 
 # ----------------------------------------------------------------------------- annotations, all of an image at once

@@ -357,3 +357,20 @@ def fields_digest(cif, caf):
     m.update(np.ascontiguousarray(cif, dtype=np.float32).tobytes())
     m.update(np.ascontiguousarray(caf, dtype=np.float32).tobytes())
     return m.hexdigest()
+
+
+def photo_like_image(h, w, seed=0):
+    """uint8 [h, w, 3] with the statistics JPEG encoders meet in photographs: smooth colour fields, oriented texture
+    and sensor-like noise (seeded; the input of the JPEG decode tests and tools/bench_jpeg.py)"""
+    rng = np.random.default_rng(seed)
+    y, x = np.mgrid[0:h, 0:w].astype(np.float64)
+    img = np.zeros((h, w, 3))
+    for c in range(3):
+        for _ in range(3):                                  # smooth fields
+            fx, fy = rng.uniform(0.2, 3.0, 2) * 2 * np.pi / max(h, w)
+            img[..., c] += rng.uniform(20, 60) * np.sin(fx * x + fy * y + rng.uniform(0, 2 * np.pi))
+        img[..., c] += rng.uniform(60, 190)
+    a = rng.uniform(0, np.pi)                               # texture
+    img += rng.uniform(5, 25) * np.sin((np.cos(a) * x + np.sin(a) * y) * rng.uniform(0.3, 1.2))[..., None]
+    img += rng.normal(0, rng.uniform(2, 10), img.shape)     # noise
+    return np.clip(img, 0, 255).astype(np.uint8)
