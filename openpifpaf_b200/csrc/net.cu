@@ -1834,9 +1834,9 @@ int make_tmap_dw(CUtensorMap* map, const void* base, uint64_t c, uint64_t w, uin
     return encode_tmap(map, "dw", base, 4, dims, lds, box, estr, swz, CU_TENSOR_MAP_L2_PROMOTION_NONE);
 }
 
-// launch with (or without) the programmatic-stream-serialization attribute
+// every kernel launch of net.cu: with (or without) the programmatic-stream-serialization attribute, counted and checked
 template <typename... KArgs, typename... Args>
-cudaError_t launch_k(bool pdl, void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args) {
+int launch_k(bool pdl, void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args) {
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = st;
     cudaLaunchAttribute attr[1];
@@ -1847,11 +1847,13 @@ cudaError_t launch_k(bool pdl, void (*kernel)(KArgs...), dim3 grid, dim3 block, 
         n++;
     }
     cfg.attrs = attr; cfg.numAttrs = n;
-    return cudaLaunchKernelEx(&cfg, kernel, std::forward<Args>(args)...);
+    PIFPAF_CUDA_TRY(cudaLaunchKernelEx(&cfg, kernel, std::forward<Args>(args)...));
+    PIFPAF_LAUNCH_CHECK();
+    return PIFPAF_OK;
 }
 
-// the TMA depthwise kernels, one entry per instantiation: pifpaf_net_dwconv picks the entry of an op (and encodes
-// its box), the launch takes kernel, block, shared memory and grid from it, pifpaf_net_create sets its shared-memory limit
+// the TMA depthwise kernels, one entry per instantiation: choose_dw_kernels picks the entry of an op (pifpaf_net_dwconv
+// encodes its box), the launch takes kernel, block and grid from it, pifpaf_net_create sets its shared-memory limit
 using DwTmaKernel = decltype(&k_dwconv5_tma<1, DW1_TH, DW1_TW, 4, 3>);
 struct DwTmaVariant {
     DwTmaKernel kernel;
@@ -1866,7 +1868,7 @@ const DwTmaVariant DW_TMA[DW_TMA_VARIANTS] = {
     {k_dwconv5_tma<1, DW1_TH, DW1_TW, 4, 3>, DwS1::THREADS, DwS1::SMEM, DW1_TH, DW1_TW, 2, DwS1::IW, DwS1::IH},
     {k_dwconv5_tma<2, DW2_TH, DW2_TW, 4, 2>, DwS2::THREADS, DwS2::SMEM, DW2_TH, DW2_TW, 1, DwS2::IW, DwS2::IH},
     // channel-block-fastest item order with the weights staged in shared memory (PIFPAF_DW_CBF=1): DW_K5_S2's
-    // window and grid, chosen at launch while the weights fit
+    // window and grid, chosen at emit while the weights fit
     {k_dwconv5_tma<2, DW2_TH, DW2_TW, 4, 2, true>, DwS2::THREADS, 226 * 1024, DW2_TH, DW2_TW, 1, DwS2::IW, DwS2::IH},
     {k_dwconv5_tma<1, DW1_TH, DW1_TW, 4, 4, false, 3>, DwS1K3::THREADS, DwS1K3::SMEM, DW1_TH, DW1_TW, 2, DwS1K3::IW,
      DwS1K3::IH},
@@ -1883,6 +1885,7 @@ const InConvKernel INPUT_CONV_KERNELS[2][4] = {
 
 struct Tensor { int h, w, c; __nv_bfloat16* data; };
 
+// the values are the op kinds pifpaf_net_forward_timed reports (a fused 1x1 -> depthwise pair: OP_FUSED)
 enum OpKind { OP_INPUT_CONV, OP_GEMM, OP_DW, OP_FUSED, OP_MAXPOOL };
 
 struct Op {
@@ -1891,7 +1894,7 @@ struct Op {
     GemmArgs g{};
     CUtensorMap tmap_a{}, tmap_b{}, tmap_src{};
     int a_tensor = -1; int rows_per_image = 0; int tiles_per_image = 0;
-    size_t smem = 0;
+    size_t smem = 0;                 // dynamic shared memory: k_gemm_wg, k_dw_gemm, the TMA depthwise kernel (dw_tma)
     // TMA-store epilogue (g.tma_store): the output views {base, columns, row pitch}, one per store map; the maps
     // bound rows at batch * rows_per_image and are re-encoded when the batch changes (store_rows: the M they hold)
     struct StoreView { const __nv_bfloat16* base; int cols; int ld; };
@@ -1901,7 +1904,8 @@ struct Op {
     // dw, max pool
     DwArgs dw{};
     CUtensorMap tmap_dw{};
-    const DwTmaVariant* dw_tma = nullptr;     // the TMA kernel of a depthwise op (nullptr: k_dwconv5 / k_dwconv)
+    const DwTmaVariant* dw_tma = nullptr;     // TMA route of a depthwise op (choose_dw_kernels; nullptr: none)
+    void (*dw_simt5)(DwArgs) = nullptr;       // its SIMT route: k_dwconv5<S> (nullptr: k_dwconv)
     int dw_dil = 1;                           // depthwise tap spacing (> 1: DW_K5_S1_D2 or k_dwconv)
     // fused depthwise -> GEMM (OP_FUSED): g + tmap_dw (windows) + tmap_b
     FusedArgs fu{};
@@ -2185,10 +2189,32 @@ int upload_dest_groups(pifpaf_net* net, int n_pad, int n_out, int h, int w, int 
     return rc;
 }
 
+// The kernels of a depthwise op, chosen once at emit; launch_dw only reads them.  TMA route (gemm_impl 0): a DW_TMA
+// entry and the shared memory of its launch.  SIMT route (gemm_impl 1, or no TMA entry): k_dwconv5<S> or k_dwconv.
+void choose_dw_kernels(const pifpaf_net* net, Op& op) {
+    const DwArgs& a = op.dw;
+    const int kernel = a.kernel, stride = a.stride, relu = a.relu, dilation = op.dw_dil;
+    if (dilation == 2 && kernel == 5 && stride == 1 && relu != ACT_RELU6) {
+        op.dw_tma = &DW_TMA[DW_K5_S1_D2];
+    } else if (dilation == 1 && (kernel == 3 || (kernel == 5 && relu != ACT_RELU6)) && (stride == 1 || stride == 2)) {
+        op.dw_tma = &DW_TMA[kernel == 3 ? (stride == 1 ? DW_K3_S1 : DW_K3_S2) : (stride == 1 ? DW_K5_S1 : DW_K5_S2)];
+    }
+    if (op.dw_tma) op.smem = op.dw_tma->smem;
+    // channel-block-fastest order with the weights staged in shared memory while they fit
+    const size_t smem_cf = op.smem + (size_t)26 * a.C8 * 8 * sizeof(float);
+    if (op.dw_tma == &DW_TMA[DW_K5_S2] && net->dw_cbf && (a.C8 + 7) / 8 > 1 &&
+        smem_cf <= (size_t)DW_TMA[DW_K5_S2_CBF].smem) {
+        op.dw_tma = &DW_TMA[DW_K5_S2_CBF];
+        op.smem = smem_cf;
+    }
+    if (kernel == 5 && dilation == 1 && (stride == 1 || stride == 2))
+        op.dw_simt5 = stride == 1 ? k_dwconv5<1> : k_dwconv5<2>;
+}
+
 // Decides, once all ops are known, which 1x1 GEMM -> depthwise pairs run as one k_pw_dw launch.  The GEMM qualifies
 // when it is plain (no residual, shuffle or implicit conv), reads one K block from column 0 of a tensor of at most
 // PWDW_K channels and writes column 0 of its output tensor; it is fused when the next op is the TMA depthwise 5x5,
-// stride 2, pad 2 reading that tensor from column 0, and no other op touches the tensor.
+// stride 2, pad 2 (in either item order) reading that tensor from column 0, and no other op touches the tensor.
 int plan_pw_dw(pifpaf_net* net) {
     net->pw_dw_planned = net->ops.size();
     for (Op& op : net->ops) { op.elided = false; op.pw_dw = false; }
@@ -2196,9 +2222,9 @@ int plan_pw_dw(pifpaf_net* net) {
     for (size_t i = 0; i + 1 < net->ops.size(); i++) {
         Op& gop = net->ops[i];
         Op& dop = net->ops[i + 1];
-        if (gop.kind != OP_GEMM || dop.kind != OP_DW || dop.dw_tma != &DW_TMA[DW_K5_S2]) continue;
         const GemmArgs& g = gop.g;
         const DwArgs& d = dop.dw;
+        if (gop.kind != OP_GEMM || dop.kind != OP_DW || !dop.dw_tma || d.kernel != 5 || d.stride != 2) continue;
         if (g.mode != MODE_PLAIN || g.conv_k != 0 || g.res != nullptr || g.num_k_blocks != 1 || g.a_col0 != 0 ||
             g.out_col_off != 0 || g.relu == ACT_RELU6)
             continue;
@@ -2248,25 +2274,100 @@ int launch_gemm(pifpaf_net* net, Op& op, int batch, int gemm_impl, bool pdl, cud
     if (gemm_impl == 1) {
         const long long jobs = (long long)g.m_blocks * 4 * (g.n_blocks * g.block_n / CHUNK);
         const int grid = (int)std::min<long long>((jobs + 3) / 4, (long long)n_sm * 16);
-        k_gemm_simt<<<grid, 128, 0, st>>>(g);
-    } else {
-        const int tiles = g.m_blocks * g.n_blocks;
-        int grid = std::min(tiles, n_sm);
-        if (g.b_resident) grid = std::max(1, std::min(n_sm / g.n_blocks, g.m_blocks)) * g.n_blocks;
-        if (g.tma_store && op.store_rows != g.M) {
-            for (size_t i = 0; i < op.store_views.size(); i++) {
-                const Op::StoreView& v = op.store_views[i];
-                const int rc = make_tmap_store(&op.smaps.m[i], v.base, (uint64_t)g.M, (uint64_t)v.cols, (uint64_t)v.ld);
-                if (rc != PIFPAF_OK) return rc;
-            }
-            op.store_rows = g.M;
-        }
-        auto* kern = GEMM_KERNELS[tile_groups(g.block_n)][tile_last(g.block_n)];
-        PIFPAF_CUDA_TRY(launch_k(pdl, kern, dim3(grid), dim3(GEMM_THREADS), op.smem, st, op.tmap_a, op.tmap_b,
-                                 g.src_tma ? op.tmap_src : op.tmap_a, op.smaps, g));
+        return launch_k(false, k_gemm_simt, dim3(grid), dim3(128), 0, st, g);
     }
-    PIFPAF_LAUNCH_CHECK();
-    return PIFPAF_OK;
+    int grid = std::min(g.m_blocks * g.n_blocks, n_sm);
+    if (g.b_resident) grid = std::max(1, std::min(n_sm / g.n_blocks, g.m_blocks)) * g.n_blocks;
+    if (g.tma_store && op.store_rows != g.M) {
+        for (size_t i = 0; i < op.store_views.size(); i++) {
+            const Op::StoreView& v = op.store_views[i];
+            const int rc = make_tmap_store(&op.smaps.m[i], v.base, (uint64_t)g.M, (uint64_t)v.cols, (uint64_t)v.ld);
+            if (rc != PIFPAF_OK) return rc;
+        }
+        op.store_rows = g.M;
+    }
+    auto* kern = GEMM_KERNELS[tile_groups(g.block_n)][tile_last(g.block_n)];
+    return launch_k(pdl, kern, dim3(grid), dim3(GEMM_THREADS), op.smem, st, op.tmap_a, op.tmap_b,
+                    g.src_tma ? op.tmap_src : op.tmap_a, op.smaps, g);
+}
+
+struct RawImages { const uint8_t* images; float mean[3], stdev[3]; };
+
+// the stem, on the f32 images or on the raw uint8 ones (u8).  Always the first op, so launched without PDL
+int launch_input_conv(const pifpaf_net* net, const Op& op, int batch, const float* images, const RawImages* u8,
+                      cudaStream_t st) {
+    InConvArgs a = op.ic;
+    a.in = images; a.B = batch;
+    const long long total = (long long)batch * a.Hout * a.Wout;
+    const int grid = (int)std::min<long long>((total + 255) / 256, (long long)effective_sms(net) * 16);
+    if (u8 != nullptr) {
+        a.in_u8 = u8->images;
+        for (int c = 0; c < 3; c++) { a.mean[c] = u8->mean[c]; a.stdev[c] = u8->stdev[c]; }
+    }
+    return launch_k(false, INPUT_CONV_KERNELS[u8 != nullptr][a.kernel / 2], dim3(grid), dim3(256),
+                    input_conv_smem_bytes(a.kernel, a.C8), st, a);
+}
+
+// the fused depthwise -> 1x1 op (k_dw_gemm)
+int launch_dw_gemm(const pifpaf_net* net, const Op& op, int batch, int gemm_impl, bool pdl, cudaStream_t st) {
+    PIFPAF_CHECK_ARG(gemm_impl == 0, "the fused depthwise -> 1x1 op has no SIMT debug variant (compile the net with fuse_dw=False)");
+    GemmArgs g = op.g;
+    g.M = batch * op.rows_per_image;
+    g.m_blocks = batch * op.tiles_per_image;
+    const int grid = std::max(1, std::min(effective_sms(net) / g.n_blocks, g.m_blocks)) * g.n_blocks;
+    auto* kern = DW_GEMM_KERNELS[tile_groups(g.block_n)][tile_last(g.block_n)];
+    return launch_k(pdl, kern, dim3(grid), dim3(FD_THREADS), op.smem, st, op.tmap_dw, op.tmap_b, g, op.fu);
+}
+
+// a depthwise op: k_pw_dw when plan_pw_dw paired it with the 1x1 before it, else the route choose_dw_kernels stored.
+// k_dwconv5 and k_dwconv run no griddepcontrol.wait, so they launch without PDL
+int launch_dw(const pifpaf_net* net, const Op& op, int batch, int gemm_impl, bool pdl, cudaStream_t st) {
+    const int n_sm = effective_sms(net);
+    DwArgs a = op.dw;
+    a.B = batch;
+    if (op.pw_dw && gemm_impl == 0) {
+        PwDwArgs p = op.pw;
+        p.dw.B = batch;
+        const long long total = (long long)batch * ((a.Hout + PWDW_TH - 1) / PWDW_TH) * ((a.Wout + PWDW_TW - 1) / PWDW_TW);
+        const int grid = (int)std::min<long long>(total, (long long)n_sm);     // 1 CTA per SM by shared memory
+        return launch_k(pdl, k_pw_dw<2, PWDW_TH, PWDW_TW, PWDW_BW>, dim3(grid), dim3(PwDwS2::THREADS), op.pw_smem, st,
+                        op.tmap_pw, p);
+    }
+    if (op.dw_tma && gemm_impl == 0) {
+        const DwTmaVariant* v = op.dw_tma;
+        const long long total = (long long)batch * ((a.Hout + v->th - 1) / v->th) * ((a.Wout + v->tw - 1) / v->tw) *
+                                ((a.C8 + 7) / 8);
+        const int grid = (int)std::min<long long>(total, (long long)n_sm * v->ctas_per_sm);
+        return launch_k(pdl, v->kernel, dim3(grid), dim3(v->threads), op.smem, st, op.tmap_dw, a);
+    }
+    if (op.dw_simt5) {
+        const long long total = (long long)batch * ((a.Hout + DW_OY - 1) / DW_OY) * DW_OY *
+                                ((a.Wout + DW_OX - 1) / DW_OX) * a.C8;
+        const int grid = (int)std::min<long long>((total + 255) / 256, (long long)n_sm * 64);
+        return launch_k(false, op.dw_simt5, dim3(grid), dim3(256), 0, st, a);
+    }
+    const long long total = (long long)batch * a.Hout * a.Wout * a.C8;
+    const int grid = (int)std::min<long long>((total + 255) / 256, (long long)n_sm * 32);
+    return launch_k(false, k_dwconv, dim3(grid), dim3(256), 0, st, a, op.dw_dil);
+}
+
+int launch_maxpool(const pifpaf_net* net, const Op& op, int batch, bool pdl, cudaStream_t st) {
+    DwArgs a = op.dw;
+    a.B = batch;
+    const long long total = (long long)batch * a.Hout * a.Wout * a.C8;
+    const int grid = (int)std::min<long long>((total + 255) / 256, (long long)effective_sms(net) * 32);
+    return launch_k(pdl, k_maxpool, dim3(grid), dim3(256), 0, st, a);
+}
+
+int launch_op(pifpaf_net* net, Op& op, int batch, int gemm_impl, bool pdl, cudaStream_t st, const float* images,
+              const RawImages* u8) {
+    switch (op.kind) {
+    case OP_INPUT_CONV: return launch_input_conv(net, op, batch, images, u8, st);
+    case OP_DW: return launch_dw(net, op, batch, gemm_impl, pdl, st);
+    case OP_FUSED: return launch_dw_gemm(net, op, batch, gemm_impl, pdl, st);
+    case OP_MAXPOOL: return launch_maxpool(net, op, batch, pdl, st);
+    default: return launch_gemm(net, op, batch, gemm_impl, pdl, st);
+    }
 }
 
 }  // namespace
@@ -2577,11 +2678,7 @@ int pifpaf_net_dwconv_dilated(pifpaf_net_t* net, int32_t in_tensor, int32_t in_c
     op.dw_dil = dilation;
     op.flops_per_image = 2.0 * ho * wo * channels * (double)kernel * kernel;
     op.bytes_per_image = ((double)tin.h * tin.w + (double)ho * wo) * channels * 2.0;
-    if (dilation == 2 && kernel == 5 && stride == 1 && relu != ACT_RELU6) {
-        op.dw_tma = &DW_TMA[DW_K5_S1_D2];
-    } else if (dilation == 1 && (kernel == 3 || (kernel == 5 && relu != ACT_RELU6)) && (stride == 1 || stride == 2)) {
-        op.dw_tma = &DW_TMA[kernel == 3 ? (stride == 1 ? DW_K3_S1 : DW_K3_S2) : (stride == 1 ? DW_K5_S1 : DW_K5_S2)];
-    }
+    choose_dw_kernels(net, op);
     if (op.dw_tma) {
         rc = make_tmap_dw(&op.tmap_dw, tin.data + in_col_off, (uint64_t)C, (uint64_t)tin.w, (uint64_t)tin.h,
                           (uint64_t)net->max_batch, (uint64_t)tin.c, op.dw_tma->box_w, op.dw_tma->box_h);
@@ -2758,8 +2855,6 @@ int pifpaf_net_head_output(pifpaf_net_t* net, int32_t head, float** dev_ptr,
     return PIFPAF_OK;
 }
 
-struct RawImages { const uint8_t* images; float mean[3], stdev[3]; };
-
 static int net_forward_impl(pifpaf_net_t* net, const float* images_dev, int32_t batch, int32_t gemm_impl,
                             cudaStream_t st, cudaEvent_t* events, const RawImages* u8 = nullptr) {
     PIFPAF_CHECK_ARG(net != nullptr, "null argument");
@@ -2777,7 +2872,6 @@ static int net_forward_impl(pifpaf_net_t* net, const float* images_dev, int32_t 
         const int rc = plan_pw_dw(net);
         if (rc != PIFPAF_OK) return rc;
     }
-    const int n_sm = effective_sms(net);
     int op_index = 0;
     net->elided_batch = 0;
     // PDL between consecutive ops (not in the per-op timing pass: the events would sit between the launches; not for
@@ -2787,78 +2881,12 @@ static int net_forward_impl(pifpaf_net_t* net, const float* images_dev, int32_t 
         if (events) PIFPAF_CUDA_TRY(cudaEventRecord(events[op_index], st));
         const bool pdl = pdl_on && op_index > 0;
         op_index++;
-        if (op.elided && gemm_impl == 0) {          // computed inside the k_pw_dw launch of the next op
+        if (op.elided && gemm_impl == 0) {          // computed inside the fused launch of the next op (plan_pw_dw)
             net->elided_batch = batch;
             continue;
         }
-        if (op.kind == OP_INPUT_CONV) {
-            InConvArgs a = op.ic;
-            a.in = images_dev; a.B = batch;
-            const long long total = (long long)batch * a.Hout * a.Wout;
-            const int grid = (int)std::min<long long>((total + 255) / 256, (long long)n_sm * 16);
-            const size_t smem = input_conv_smem_bytes(a.kernel, a.C8);
-            if (u8 != nullptr) {
-                a.in_u8 = u8->images;
-                for (int c = 0; c < 3; c++) { a.mean[c] = u8->mean[c]; a.stdev[c] = u8->stdev[c]; }
-            }
-            InConvKernel kern = INPUT_CONV_KERNELS[u8 != nullptr][a.kernel / 2];
-            kern<<<grid, 256, smem, st>>>(a);
-            PIFPAF_LAUNCH_CHECK();
-        } else if (op.kind == OP_FUSED) {
-            PIFPAF_CHECK_ARG(gemm_impl == 0, "the fused depthwise -> 1x1 op has no SIMT debug variant (compile the net with fuse_dw=False)");
-            GemmArgs g = op.g;
-            g.M = batch * op.rows_per_image;
-            g.m_blocks = batch * op.tiles_per_image;
-            const int grid = std::max(1, std::min(n_sm / g.n_blocks, g.m_blocks)) * g.n_blocks;
-            auto* kern = DW_GEMM_KERNELS[tile_groups(g.block_n)][tile_last(g.block_n)];
-            PIFPAF_CUDA_TRY(launch_k(pdl, kern, dim3(grid), dim3(FD_THREADS), op.smem, st, op.tmap_dw, op.tmap_b, g, op.fu));
-            PIFPAF_LAUNCH_CHECK();
-        } else if (op.kind == OP_DW) {
-            DwArgs a = op.dw;
-            a.B = batch;
-            if (op.pw_dw && gemm_impl == 0) {
-                PwDwArgs p = op.pw;
-                p.dw.B = batch;
-                const long long total = (long long)batch * ((a.Hout + PWDW_TH - 1) / PWDW_TH) * ((a.Wout + PWDW_TW - 1) / PWDW_TW);
-                const int grid = (int)std::min<long long>(total, (long long)n_sm);     // 1 CTA per SM by shared memory
-                PIFPAF_CUDA_TRY(launch_k(pdl, k_pw_dw<2, PWDW_TH, PWDW_TW, PWDW_BW>, dim3(grid), dim3(PwDwS2::THREADS),
-                                         op.pw_smem, st, op.tmap_pw, p));
-            } else if (op.dw_tma && gemm_impl == 0) {
-                const DwTmaVariant* v = op.dw_tma;
-                const int cblks = (a.C8 + 7) / 8;
-                const long long total = (long long)batch * ((a.Hout + v->th - 1) / v->th) * ((a.Wout + v->tw - 1) / v->tw) * cblks;
-                const int grid = (int)std::min<long long>(total, (long long)n_sm * v->ctas_per_sm);
-                size_t smem = v->smem;
-                // channel-block-fastest order with the weights staged in shared memory while they fit
-                const size_t smem_cf = smem + (size_t)26 * a.C8 * 8 * sizeof(float);
-                if (v == &DW_TMA[DW_K5_S2] && net->dw_cbf && cblks > 1 && smem_cf <= (size_t)DW_TMA[DW_K5_S2_CBF].smem) {
-                    v = &DW_TMA[DW_K5_S2_CBF];
-                    smem = smem_cf;
-                }
-                PIFPAF_CUDA_TRY(launch_k(pdl, v->kernel, dim3(grid), dim3(v->threads), smem, st, op.tmap_dw, a));
-            } else if (a.kernel == 5 && op.dw_dil == 1 && (a.stride == 1 || a.stride == 2)) {
-                const long long total = (long long)batch * ((a.Hout + DW_OY - 1) / DW_OY) * DW_OY *
-                                        ((a.Wout + DW_OX - 1) / DW_OX) * a.C8;
-                const int grid = (int)std::min<long long>((total + 255) / 256, (long long)n_sm * 64);
-                if (a.stride == 1) k_dwconv5<1><<<grid, 256, 0, st>>>(a);
-                else k_dwconv5<2><<<grid, 256, 0, st>>>(a);
-            } else {
-                const long long total = (long long)batch * a.Hout * a.Wout * a.C8;
-                const int grid = (int)std::min<long long>((total + 255) / 256, (long long)n_sm * 32);
-                k_dwconv<<<grid, 256, 0, st>>>(a, op.dw_dil);
-            }
-            PIFPAF_LAUNCH_CHECK();
-        } else if (op.kind == OP_MAXPOOL) {
-            DwArgs a = op.dw;
-            a.B = batch;
-            const long long total = (long long)batch * a.Hout * a.Wout * a.C8;
-            const int grid = (int)std::min<long long>((total + 255) / 256, (long long)n_sm * 32);
-            PIFPAF_CUDA_TRY(launch_k(pdl, k_maxpool, dim3(grid), dim3(256), 0, st, a));
-            PIFPAF_LAUNCH_CHECK();
-        } else {
-            const int rc = launch_gemm(net, op, batch, gemm_impl, pdl, st);
-            if (rc != PIFPAF_OK) return rc;
-        }
+        const int rc = launch_op(net, op, batch, gemm_impl, pdl, st, images_dev, u8);
+        if (rc != PIFPAF_OK) return rc;
     }
     if (events) PIFPAF_CUDA_TRY(cudaEventRecord(events[op_index], st));
     return PIFPAF_OK;
@@ -2897,10 +2925,9 @@ int pifpaf_net_forward_timed(pifpaf_net_t* net, const float* images_dev, int32_t
     for (size_t i = 0; i < n && rc == PIFPAF_OK; i++) {
         cudaEventElapsedTime(&op_ms[i], ev[i], ev[i + 1]);
         const Op& op = net->ops[i];
+        // the 1x1 -> depthwise pair that net_forward_impl skips and launch_dw runs as k_pw_dw
         const bool fused = gemm_impl == 0 && (op.elided || op.pw_dw);
-        if (op_kind)
-            op_kind[i] = op.kind == OP_MAXPOOL ? 4
-                       : fused || op.kind == OP_FUSED ? 3 : (op.kind == OP_INPUT_CONV ? 0 : (op.kind == OP_GEMM ? 1 : 2));
+        if (op_kind) op_kind[i] = fused ? OP_FUSED : op.kind;
         // an elided GEMM launches nothing (its events bracket no work) and its work is counted in the fused launch
         if (op_flops) op_flops[i] = !fused ? op.flops_per_image * batch : op.pw_dw ? op.pw_flops_per_image * batch : 0.0;
         if (op_bytes)
@@ -2927,12 +2954,11 @@ int pifpaf_net_tap_tensor(pifpaf_net_t* net, int32_t id, int32_t batch, float* o
             }
     float* d_tmp = nullptr;
     PIFPAF_CUDA_TRY(cudaMalloc(reinterpret_cast<void**>(&d_tmp), sizeof(float) * n));
-    k_bf16_to_f32<<<1024, 256>>>(t.data, d_tmp, n);
-    pifpaf::count_launch();
-    cudaError_t e = cudaMemcpy(out, d_tmp, sizeof(float) * n, cudaMemcpyDeviceToHost);
+    const int rc = launch_k(false, k_bf16_to_f32, dim3(1024), dim3(256), 0, 0, t.data, d_tmp, n);
+    const cudaError_t e = rc == PIFPAF_OK ? cudaMemcpy(out, d_tmp, sizeof(float) * n, cudaMemcpyDeviceToHost) : cudaSuccess;
     cudaFree(d_tmp);
     if (e != cudaSuccess) { pifpaf::set_error("tap copy failed: %s", cudaGetErrorString(e)); return PIFPAF_E_CUDA; }
-    return PIFPAF_OK;
+    return rc;
 }
 
 int pifpaf_net_set_tensor(pifpaf_net_t* net, int32_t id, int32_t batch, const float* data, int64_t n_elems) {
@@ -2943,13 +2969,14 @@ int pifpaf_net_set_tensor(pifpaf_net_t* net, int32_t id, int32_t batch, const fl
     PIFPAF_CUDA_TRY(cudaSetDevice(net->device));
     float* d_tmp = nullptr;
     PIFPAF_CUDA_TRY(cudaMalloc(reinterpret_cast<void**>(&d_tmp), sizeof(float) * n));
+    int rc = PIFPAF_OK;
     cudaError_t e = cudaMemcpy(d_tmp, data, sizeof(float) * n, cudaMemcpyHostToDevice);
     if (e == cudaSuccess) {
-        k_f32_to_bf16<<<1024, 256>>>(d_tmp, t.data, n);
-        pifpaf::count_launch();
-        e = cudaDeviceSynchronize();
+        rc = launch_k(false, k_f32_to_bf16, dim3(1024), dim3(256), 0, 0, d_tmp, t.data, n);
+        if (rc == PIFPAF_OK) e = cudaDeviceSynchronize();
     }
     cudaFree(d_tmp);
+    if (rc != PIFPAF_OK) return rc;
     if (e != cudaSuccess) { pifpaf::set_error("set_tensor failed: %s", cudaGetErrorString(e)); return PIFPAF_E_CUDA; }
     return PIFPAF_OK;
 }

@@ -141,8 +141,8 @@ DW_CBF_SMEM = 226 * 1024                     # DW_TMA[DW_K5_S2_CBF].smem
 
 
 def dw_kernel(channels, kernel, stride, relu, dilation=1, gemm_impl=0, cbf=False):
-    """the kernel a depthwise op launches: a DW_TMA entry ('DW_K5_S1', 'DW_K5_S2', 'DW_K5_S2_CBF', 'DW_K3_S1',
-    'DW_K3_S2', 'DW_K5_S1_D2'), 'k_dwconv5' or 'k_dwconv'.  cbf: PIFPAF_DW_CBF"""
+    """the kernel a depthwise op launches (choose_dw_kernels): a DW_TMA entry ('DW_K5_S1', 'DW_K5_S2', 'DW_K5_S2_CBF',
+    'DW_K3_S1', 'DW_K3_S2', 'DW_K5_S1_D2'), 'k_dwconv5' or 'k_dwconv'.  cbf: PIFPAF_DW_CBF"""
     tma = None
     if dilation == 2 and kernel == 5 and stride == 1 and relu != 2:
         tma = 'DW_K5_S1_D2'

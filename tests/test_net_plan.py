@@ -42,18 +42,22 @@ MIRRORED = [
     'if (net->gemm_tma_store && (int)map_tensor.size() <= MAX_STORE_MAPS) {',
     'inline int tile_groups(int block_n) { return (block_n + NGROUP - 1) / NGROUP - 1; }',
     'inline int tile_last(int block_n) { return (block_n - tile_groups(block_n) * NGROUP) / 16 - 1; }',
-    # depthwise kernel selection
+    # depthwise kernel selection (choose_dw_kernels)
+    'const DwArgs& a = op.dw; const int kernel = a.kernel, stride = a.stride, relu = a.relu, dilation = op.dw_dil; '
     'if (dilation == 2 && kernel == 5 && stride == 1 && relu != ACT_RELU6) { op.dw_tma = &DW_TMA[DW_K5_S1_D2]; } '
     'else if (dilation == 1 && (kernel == 3 || (kernel == 5 && relu != ACT_RELU6)) && (stride == 1 || stride == 2)) { '
-    'op.dw_tma = &DW_TMA[kernel == 3 ? (stride == 1 ? DW_K3_S1 : DW_K3_S2) : (stride == 1 ? DW_K5_S1 : DW_K5_S2)]; }',
-    'const size_t smem_cf = smem + (size_t)26 * a.C8 * 8 * sizeof(float); '
-    'if (v == &DW_TMA[DW_K5_S2] && net->dw_cbf && cblks > 1 && smem_cf <= (size_t)DW_TMA[DW_K5_S2_CBF].smem) {',
+    'op.dw_tma = &DW_TMA[kernel == 3 ? (stride == 1 ? DW_K3_S1 : DW_K3_S2) : (stride == 1 ? DW_K5_S1 : DW_K5_S2)]; } '
+    'if (op.dw_tma) op.smem = op.dw_tma->smem;',
+    'const size_t smem_cf = op.smem + (size_t)26 * a.C8 * 8 * sizeof(float); '
+    'if (op.dw_tma == &DW_TMA[DW_K5_S2] && net->dw_cbf && (a.C8 + 7) / 8 > 1 && '
+    'smem_cf <= (size_t)DW_TMA[DW_K5_S2_CBF].smem) { op.dw_tma = &DW_TMA[DW_K5_S2_CBF]; op.smem = smem_cf; } '
+    'if (kernel == 5 && dilation == 1 && (stride == 1 || stride == 2)) '
+    'op.dw_simt5 = stride == 1 ? k_dwconv5<1> : k_dwconv5<2>; }',
     '{k_dwconv5_tma<2, DW2_TH, DW2_TW, 4, 2, true>, DwS2::THREADS, 226 * 1024,',
-    '} else if (a.kernel == 5 && op.dw_dil == 1 && (a.stride == 1 || a.stride == 2)) {',
     'using DwS2 = DwTile<2, DW2_TH, DW2_TW, 4, 2>;',
     'static constexpr int SMEM = NSTAGE * BYTES + 128;',
     # plan_pw_dw and pw_dw_smem_bytes
-    'if (gop.kind != OP_GEMM || dop.kind != OP_DW || dop.dw_tma != &DW_TMA[DW_K5_S2]) continue;',
+    'if (gop.kind != OP_GEMM || dop.kind != OP_DW || !dop.dw_tma || d.kernel != 5 || d.stride != 2) continue;',
     'if (g.mode != MODE_PLAIN || g.conv_k != 0 || g.res != nullptr || g.num_k_blocks != 1 || g.a_col0 != 0 || '
     'g.out_col_off != 0 || g.relu == ACT_RELU6) continue;',
     'if (d.pad != 2 || d.in != g.out || d.in_col_off != 0) continue;',
