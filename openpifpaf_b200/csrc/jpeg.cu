@@ -4,11 +4,27 @@
 // libjpeg-turbo uses the accurate integer IDCT (jidctint), fancy upsampling (jdsample) and the fixed-point YCbCr->RGB
 // tables (jdcolor) by default: integer arithmetic throughout, restated here so the decoded image equals Pillow's.
 //
-// Host: marker parse only (nothing per entropy-coded byte): Huffman tables (9-bit lookup + canonical maxcode /
-// valoffset), quantisation tables in natural order, the MCU layout, validation, one pinned staging copy.
+// Host: marker parse: Huffman tables (9-bit lookup + canonical maxcode / valoffset), quantisation tables in natural
+// order, the MCU layout, validation; a walk over the scan (SSE2, sixteen bytes a step) for its end and the markers
+// inside it, which is also the staging copy of its bytes; the restart-interval table; one pinned copy to the device.
+// Damaged streams, as libjpeg decodes them (jdhuff.c, jdmarker.c):
+//   - The scan ends at the first marker after the SOS that is not RSTn (or a code below SOF0, which libjpeg's resync
+//     skips); FF fill bytes and FF00 are not markers.  Bytes after it (a trailer, a second image) are not staged.
+//   - Every marker in the scan ends a data segment.  Interval i > 0 expects RST((i - 1) mod 8) and gets its data
+//     segment by jpeg_resync_to_restart: the expected marker or one too far from it is taken, a prior one (or a code
+//     below SOF0) is skipped with its data, one of the next two or the scan's end is left unread: an empty segment.
+//   - Bits past a segment read as zeros.  The MCU that consumes them is finished from zeros (insufficient_data); the
+//     interval's later blocks stay all zero with an absolute DC of 0.  An empty segment after a starved interval
+//     decodes nothing (the flag survives a marker left unread); otherwise its first MCU is decoded from zeros.
+//   - JFIF needs an APP0 of at least 14 bytes; a JFIF / Adobe segment too short for Pillow's parser takes Pillow's
+//     route, which raises as the reference's loader does.
+//   - A damaged block can overshoot the IDCT's 16-bit lanes.  The IDCT follows the x86 SIMD code (jidctint-sse2 /
+//     -avx2) of the libjpeg-turbo bundled with Pillow's x86-64 wheels, which Pillow runs there: 16-bit products and
+//     sums, pass 1's shortcut for blocks whose coefficient rows 1..7 are zero, saturating packs.  Pillow on ARM (NEON),
+//     or with JSIMD_FORCENONE, gives other pixels for such blocks; clean streams decode the same on every back end.
 // Device, per batch:
-//   k_jpeg_unstuff_count / _scan / _write   drop the stuffed FF00 bytes (order-preserving compaction), record every
-//                                           RSTn position as the byte-aligned start of its restart interval
+//   k_jpeg_unstuff_count / _scan / _write   drop FF fill bytes, the 00 of FF00 and the markers (order-preserving
+//                                           compaction), record the compacted start of every data segment
 //   k_jpeg_subseq_setup                     cut each interval into SUBSEQ_BITS-bit subsequences
 //   k_jpeg_sync (one launch per round)      self-synchronising Huffman decode (Weissenberger & Schmidt, ICPP 2018):
 //                                           start_j := exit_{j-1} until no start changes, at most max_rounds rounds
@@ -16,12 +32,17 @@
 //                                           still differs from its predecessor's exit, then the block prefix sum
 //   k_jpeg_write                            decode again from the settled starts, int16 coefficients in natural order
 //   k_jpeg_dc                               DC differences -> values: segmented prefix sum per component and interval
-//   k_jpeg_idct                             jidctint islow, one thread per block, planes padded to the MCU grid
+//   k_jpeg_idct                             jidctint islow as the x86 SIMD code of Pillow's libjpeg-turbo computes it
+//                                           (16-bit products and sums, pass 1's shortcut, saturating packs),
+//                                           one thread per block, planes padded to the MCU grid
 //   k_jpeg_color                            fancy upsampling (h2v1 / h2v2) + YCbCr->RGB, uint8 HWC
 #include <algorithm>
 #include <cstdint>
 #include <cstring>
 #include <vector>
+#if defined(__SSE2__)
+#include <emmintrin.h>
+#endif
 
 #include "common.cuh"
 
@@ -57,6 +78,7 @@ struct Img {                               // one GPU-route image of the batch
     int64_t plane_off[3];                  // into the plane buffer
     int64_t seg_off;                       // raw scan segment in the byte buffer; its compacted bytes at the same offset
     int32_t seg_len, chunk_base, n_chunks, int_base, sub_base, sub_cap;
+    int32_t seg_base, n_seg;               // data segments (one more than the markers in the scan)
     int64_t blk_base, px_base, out_off;    // first coefficient block, first output pixel of the batch, RGB byte offset
     int32_t huff[3][2], quant[3];          // table indices per component (DC, AC)
 };
@@ -71,8 +93,11 @@ struct Dev {                               // device pointers of one decode
     int32_t* chunk_keep;                   // per chunk: kept bytes, then (after the scan) their compacted offset
     int32_t* chunk_rst;
     int32_t* comp_len;                     // per image
-    int32_t* int_lo;                       // per interval: compacted start byte (filled from the RST positions)
+    const int32_t* int_seg;                // per interval: its data segment, -1: empty (a marker left unread)
+    int32_t* seg_lo;                       // per data segment: compacted start byte
+    int32_t* int_lo;                       // per interval: compacted start and end byte
     int32_t* int_hi;
+    int32_t* int_blocks;                   // per interval: block starts up to the MCU that ran past its data
     int32_t* int_img;
     int32_t* int_sub;                      // first subsequence, number of subsequences
     int32_t* int_nsub;
@@ -92,14 +117,12 @@ struct Dev {                               // device pointers of one decode
 __host__ __device__ inline long long pack_state(long long bit, int blk, int k) { return (bit << 16) | (blk << 8) | k; }
 
 // ------------------------------------------------------------------------------------------------ unstuffing
-__device__ __forceinline__ bool is_rst(uint8_t b) { return b >= 0xD0 && b <= 0xD7; }
-
-// byte i of a segment is data (kept) unless it is the 00 of FF00, or either byte of an FF Dn restart marker
+// byte i of a scan is data (1) unless it is an FF fill byte, the 00 of FF00 or a marker's FF (0), or a marker's code
+// (2): an FF is data only before 00 (jpeg_fill_bit_buffer)
 __device__ __forceinline__ int classify(const uint8_t* s, int i, int n) {
     const uint8_t b = s[i];
-    const uint8_t prev = i > 0 ? s[i - 1] : 0;
-    if (prev == 0xFF && (b == 0x00 || is_rst(b))) return b == 0x00 ? 0 : 2;   // 2: the marker's second byte
-    if (b == 0xFF && i + 1 < n && is_rst(s[i + 1])) return 0;
+    if (b == 0xFF) return i + 1 < n && s[i + 1] == 0x00 ? 1 : 0;
+    if (i > 0 && s[i - 1] == 0xFF) return b == 0x00 ? 0 : 2;
     return 1;
 }
 
@@ -145,7 +168,7 @@ __device__ int block_exclusive_scan(int v, int* total) {
     return incl - v;
 }
 
-// one CTA per image: chunk offsets (kept bytes, restart markers), compacted length, interval table reset
+// one CTA per image: chunk offsets (kept bytes, markers), compacted length
 __global__ void __launch_bounds__(1024) k_jpeg_unstuff_scan(Dev d) {
     const Img& im = d.img[blockIdx.x];
     int carry_k = 0, carry_r = 0;
@@ -163,10 +186,8 @@ __global__ void __launch_bounds__(1024) k_jpeg_unstuff_scan(Dev d) {
         carry_r += tr;
     }
     if (threadIdx.x == 0) d.comp_len[blockIdx.x] = carry_k;
-    for (int i = threadIdx.x; i < im.n_int; i += 1024) {
-        d.int_lo[im.int_base + i] = i == 0 ? 0 : 0x7fffffff;   // a missing RSTn leaves its interval empty
-        d.int_img[im.int_base + i] = blockIdx.x;
-    }
+    if (threadIdx.x == 0) d.seg_lo[im.seg_base] = 0;
+    for (int i = threadIdx.x; i < im.n_int; i += 1024) d.int_img[im.int_base + i] = blockIdx.x;
 }
 
 __global__ void __launch_bounds__(256) k_jpeg_unstuff_write(Dev d, int n_chunks) {
@@ -182,7 +203,7 @@ __global__ void __launch_bounds__(256) k_jpeg_unstuff_write(Dev d, int n_chunks)
         if (t == 1) {
             o[out++] = s[i];
         } else if (t == 2) {
-            if (++rst < im.n_int) d.int_lo[im.int_base + rst] = out;
+            if (++rst < im.n_seg) d.seg_lo[im.seg_base + rst] = out;
         }
     }
 }
@@ -197,21 +218,22 @@ __global__ void __launch_bounds__(1024) k_jpeg_subseq_setup(Dev d) {
         const bool ok = i < im.n_int;
         int lo = 0, hi = 0, nsub = 0;
         if (ok) {
-            lo = min(d.int_lo[im.int_base + i], len);
-            hi = i + 1 < im.n_int ? min(d.int_lo[im.int_base + i + 1], len) : len;
-            hi = max(hi, lo);
+            const int sg = d.int_seg[im.int_base + i];
+            if (sg >= 0) {
+                lo = min(d.seg_lo[im.seg_base + sg], len);
+                hi = max(lo, sg + 1 < im.n_seg ? min(d.seg_lo[im.seg_base + sg + 1], len) : len);
+            }
             nsub = max(1, (int)(((long long)(hi - lo) * 8 + SUBSEQ_BITS - 1) / SUBSEQ_BITS));
         }
         int total;
         const int first = carry + block_exclusive_scan(nsub, &total);
         if (ok) {
+            d.int_lo[im.int_base + i] = lo;
             d.int_hi[im.int_base + i] = hi;
             d.int_sub[im.int_base + i] = im.sub_base + first;
             d.int_nsub[im.int_base + i] = nsub;
         }
         carry += total;
-        __syncthreads();
-        if (ok) d.int_lo[im.int_base + i] = lo;
     }
     __syncthreads();
     // fill the slots: interval of each (a binary search over the interval table), unused slots -1
@@ -261,8 +283,8 @@ __device__ __forceinline__ int huff_decode(const Huff& t, const BitReader& br, l
         l++;
         code = (int)(w >> (32 - l));
     }
-    if (l > 16) {                          // no such code: a zero symbol, like libjpeg
-        *len = 16;
+    if (l > 16) {                          // no such code: 17 bits read and a zero symbol, like libjpeg
+        *len = 17;
         return 0;
     }
     *len = l;
@@ -273,14 +295,16 @@ __device__ __forceinline__ int extend(int v, int s) { return (s && v < (1 << (s 
 
 // Decode from state until the first codeword boundary at or after end_bit; with coef, also write the coefficients
 // (DC: its difference) of block base + (block starts so far - 1) while that is below limit, and stop before the DC
-// of block `limit`.  Returns the exit state; *nstart = block starts.
+// of block `limit`.  The tail of an interval (end_bit: its last bit) goes on to the end of an MCU whose bits run past
+// the data, and decodes one more MCU when the data ends exactly at an MCU boundary: libjpeg finishes the MCU that runs
+// out of data from zero bits.  Returns the exit state; *nstart = block starts.
 template <bool WRITE>
 __device__ long long decode_run(const Dev& d, const Img& im, const BitReader& br, long long state, long long end_bit,
-                                int* nstart, int16_t* coef = nullptr, int limit = 0) {
+                                bool tail, int* nstart, int16_t* coef = nullptr, int limit = 0) {
     long long pos = state >> 16;
     int blk = (int)((state >> 8) & 255), k = (int)(state & 255);
     int ns = 0;
-    while (pos < end_bit) {
+    while (pos < end_bit || (tail && (pos == end_bit || blk != 0 || k != 0))) {
         const int c = im.blk_comp[blk];
         if (k == 0) {
             if (WRITE && ns >= limit) break;
@@ -322,7 +346,7 @@ struct SubView {
     const Img* im;
     BitReader br;
     long long end_bit;
-    bool first;
+    bool first, last;
 };
 
 __device__ __forceinline__ SubView sub_view(const Dev& d, int g) {
@@ -334,6 +358,7 @@ __device__ __forceinline__ SubView sub_view(const Dev& d, int g) {
     v.br.n = hi - lo;
     v.end_bit = min((long long)(j + 1) * SUBSEQ_BITS, (long long)(hi - lo) * 8);
     v.first = j == 0;
+    v.last = j + 1 == d.int_nsub[iv];
     return v;
 }
 
@@ -356,7 +381,7 @@ __global__ void __launch_bounds__(128) k_jpeg_sync(Dev d, int n_slots, int round
         }
     }
     int ns;
-    cur[g] = decode_run<false>(d, *v.im, v.br, st, v.end_bit, &ns);
+    cur[g] = decode_run<false>(d, *v.im, v.br, st, v.end_bit, v.last, &ns);
     d.start[g] = st;
     d.count[g] = ns;
     atomicMax(&d.stats[0], (unsigned long long)(round + 1));
@@ -387,7 +412,7 @@ __global__ void __launch_bounds__(128) k_jpeg_settle(Dev d, int n_int_total, int
                 const SubView v = sub_view(d, g);
                 const long long st = t0 + lane == 0 ? pack_state(0, 0, 0) : ex[g - 1];
                 int n;
-                ex[g] = decode_run<false>(d, *v.im, v.br, st, v.end_bit, &n);
+                ex[g] = decode_run<false>(d, *v.im, v.br, st, v.end_bit, v.last, &n);
                 d.start[g] = st;
                 d.count[g] = n;
                 fallbacks++;
@@ -405,6 +430,22 @@ __global__ void __launch_bounds__(128) k_jpeg_settle(Dev d, int n_int_total, int
     }
     const unsigned long long warp_fallbacks = __reduce_add_sync(0xffffffffu, (unsigned)fallbacks);   // every lane's
     if (lane == 0 && warp_fallbacks) atomicAdd(&d.stats[1], warp_fallbacks);
+    if (lane == 0) d.int_blocks[iv] = carry;
+}
+
+__device__ __forceinline__ int interval_block_count(const Img& im, int local) {
+    const long long mcu0 = (long long)local * im.ri;
+    return (int)((min(mcu0 + im.ri, (long long)im.mx * im.my) - mcu0) * im.bpm);
+}
+
+// blocks of an interval the decode keeps: those started up to the MCU that ran past its data.  An empty interval
+// after a starved one (all its blocks started there, or itself empty) keeps none.
+__device__ __forceinline__ int interval_live(const Dev& d, const Img& im, int local) {
+    const int iv = im.int_base + local;
+    if (local > 0 && d.int_seg[iv] < 0 &&
+        (d.int_seg[iv - 1] < 0 || d.int_blocks[iv - 1] <= interval_block_count(im, local - 1)))
+        return 0;
+    return min(d.int_blocks[iv], interval_block_count(im, local));
 }
 
 // ------------------------------------------------------------------------------------------------ write pass
@@ -416,18 +457,18 @@ __global__ void __launch_bounds__(128) k_jpeg_write(Dev d, int n_slots) {
     const Img& im = *v.im;
     const int local = iv - im.int_base;
     const long long mcu0 = (long long)local * im.ri;
-    const int cnt = (int)((min(mcu0 + im.ri, (long long)im.mx * im.my) - mcu0) * im.bpm);
+    const int cnt = interval_live(d, im, local);
     const int acc = d.acc[g];
     const long long st = d.start[g];
     const int mid = (st & 255) != 0;       // the first block was begun by the previous subsequence
     if (acc - mid >= cnt) return;
     int16_t* base = d.coef + (im.blk_base + mcu0 * im.bpm + acc) * 64;
     int ns;
-    decode_run<true>(d, im, v.br, st, v.end_bit, &ns, base, cnt - acc);
+    decode_run<true>(d, im, v.br, st, v.end_bit, v.last, &ns, base, cnt - acc);
 }
 
 // DC differences -> values: one CTA per (image, component), prefix sum over the component's blocks in scan order,
-// restarted at every interval
+// restarted at every interval; a block past its interval's live blocks keeps an absolute DC of 0
 __global__ void __launch_bounds__(1024) k_jpeg_dc(Dev d) {
     const Img& im = d.img[blockIdx.x / 3];
     const int c = blockIdx.x % 3;
@@ -446,8 +487,10 @@ __global__ void __launch_bounds__(1024) k_jpeg_dc(Dev d) {
             const long long mcu = e / nbc;
             const int t = (int)(e % nbc);
             blk = im.blk_base + mcu * im.bpm + im.comp_first[c] + t;
-            v = d.coef[blk * 64];
-            f = t == 0 && mcu % im.ri == 0;
+            const int local = (int)(mcu / im.ri);
+            const bool dead = (mcu - (long long)local * im.ri) * im.bpm + im.comp_first[c] + t >= interval_live(d, im, local);
+            v = dead ? 0 : d.coef[blk * 64];
+            f = (t == 0 && mcu % im.ri == 0) || dead;
         }
         sv[threadIdx.x] = v;
         sf[threadIdx.x] = (unsigned char)f;
@@ -477,16 +520,20 @@ __global__ void __launch_bounds__(1024) k_jpeg_dc(Dev d) {
 // ------------------------------------------------------------------------------------------------ reconstruction
 constexpr int CONST_BITS = 13, PASS1_BITS = 2;
 
+// jidctint's 1-D pass as libjpeg-turbo's SSE2 / AVX2 code computes it: in0 +- in4, in7 + in3 and in5 + in1 are 16-bit
+// adds (paddw / psubw); every other term is a pmaddwd of 16-bit inputs into 32 bits, which does not overflow
+__device__ __forceinline__ long long add16(long long a, long long b) { return (int16_t)(a + b); }
+
 __device__ __forceinline__ void idct_1d(const int* s, int stride, int shift, int* out, int ostride) {
     const long long s0 = s[0], s1 = s[stride], s2 = s[2 * stride], s3 = s[3 * stride], s4 = s[4 * stride],
                     s5 = s[5 * stride], s6 = s[6 * stride], s7 = s[7 * stride];
     long long z1 = (s2 + s6) * 4433;
     const long long tmp2 = z1 + s6 * -15137, tmp3 = z1 + s2 * 6270;
-    const long long tmp0 = (s0 + s4) * (1 << CONST_BITS), tmp1 = (s0 - s4) * (1 << CONST_BITS);
+    const long long tmp0 = add16(s0, s4) * (1 << CONST_BITS), tmp1 = add16(s0, -s4) * (1 << CONST_BITS);
     const long long tmp10 = tmp0 + tmp3, tmp13 = tmp0 - tmp3, tmp11 = tmp1 + tmp2, tmp12 = tmp1 - tmp2;
     long long t0 = s7, t1 = s5, t2 = s3, t3 = s1;
     z1 = t0 + t3;
-    long long z2 = t1 + t2, z3 = t0 + t2, z4 = t1 + t3;
+    long long z2 = t1 + t2, z3 = add16(t0, t2), z4 = add16(t1, t3);
     const long long z5 = (z3 + z4) * 9633;
     t0 *= 2446; t1 *= 16819; t2 *= 25172; t3 *= 12299;
     z1 *= -7373; z2 *= -20995; z3 *= -16069; z4 *= -3196;
@@ -523,10 +570,21 @@ __global__ void __launch_bounds__(128) k_jpeg_idct(Dev d, int n_img, long long n
     const int* q = d.quant + im.quant[c] * 64;
     const int16_t* in = d.coef + b * 64;
     int x[64], ws[64];
+    bool rows0 = true;                                     // coefficient rows 1..7 all zero
 #pragma unroll
-    for (int i = 0; i < 64; i++) x[i] = (int)in[i] * q[i];
+    for (int i = 0; i < 64; i++) {
+        x[i] = (int16_t)((int)in[i] * q[i]);              // libjpeg-turbo's SIMD IDCT: pmullw
+        if (i >= 8) rows0 = rows0 && in[i] == 0;
+    }
+    if (rows0) {                                           // pass 1's shortcut: psllw, wrapping in 16 bits
 #pragma unroll
-    for (int col = 0; col < 8; col++) idct_1d(x + col, 8, CONST_BITS - PASS1_BITS, ws + col, 8);
+        for (int i = 0; i < 64; i++) ws[i] = (int16_t)(x[i & 7] * (1 << PASS1_BITS));
+    } else {
+#pragma unroll
+        for (int col = 0; col < 8; col++) idct_1d(x + col, 8, CONST_BITS - PASS1_BITS, ws + col, 8);
+#pragma unroll
+        for (int i = 0; i < 64; i++) ws[i] = min(max(ws[i], -32768), 32767);  // packssdw
+    }
     const int my = (int)(mcu / im.mx), mx = (int)(mcu % im.mx);
     const int prow = (my * im.comp_v[c] + im.blk_v[t]) * 8, pcol = (mx * im.comp_h[c] + im.blk_h[t]) * 8;
     uint8_t* o = d.plane + im.plane_off[c] + (long long)prow * im.plane_w[c] + pcol;
@@ -535,11 +593,8 @@ __global__ void __launch_bounds__(128) k_jpeg_idct(Dev d, int n_img, long long n
         int v[8];
         idct_1d(ws + row * 8, 1, CONST_BITS + PASS1_BITS + 3, v, 1);
 #pragma unroll
-        for (int i = 0; i < 8; i++) {
-            int m = v[i] & 1023;                           // IDCT_range_limit: 10-bit wrap, then clamp around 128
-            m = m >= 512 ? m - 1024 : m;
-            o[(long long)row * im.plane_w[c] + i] = (uint8_t)min(max(m + 128, 0), 255);
-        }
+        for (int i = 0; i < 8; i++)                        // packsswb, + 128
+            o[(long long)row * im.plane_w[c] + i] = (uint8_t)(min(max(v[i], -128), 127) + 128);
     }
 }
 
@@ -593,6 +648,7 @@ struct Parsed {
     std::vector<Comp> comps;               // in scan order
     int ri;
     int64_t seg_lo, seg_hi;
+    std::vector<uint8_t> markers;          // codes of the markers inside the scan, in order
     const Huff* dc[4];
     const Huff* ac[4];
     const int32_t* q[4];
@@ -626,14 +682,38 @@ int build_huff(const uint8_t* bits, const uint8_t* vals, int n, bool is_dc, Huff
     return PIFPAF_OK;
 }
 
+// First i' >= i with s[i'] == FF and s[i' + 1] != 00 (a marker or an FF fill byte; n if none), sixteen bytes at a
+// time.  With dst, s[i, i') is copied to dst[i - base, ...) on the way (up to 16 bytes more; dst_room bounds it).
+// The entropy-coded bytes are read once: the walk is the staging copy.
+int64_t find_marker(const uint8_t* s, int64_t i, int64_t n, uint8_t* dst = nullptr, int64_t base = 0,
+                    int64_t dst_room = 0) {
+#if defined(__SSE2__)
+    const __m128i ff = _mm_set1_epi8((char)0xFF), z = _mm_setzero_si128();
+    for (; i + 17 <= n; i += 16) {
+        const __m128i a = _mm_loadu_si128(reinterpret_cast<const __m128i*>(s + i));
+        const __m128i b = _mm_loadu_si128(reinterpret_cast<const __m128i*>(s + i + 1));
+        if (dst && i - base + 16 <= dst_room) _mm_storeu_si128(reinterpret_cast<__m128i*>(dst + (i - base)), a);
+        const int m = _mm_movemask_epi8(_mm_andnot_si128(_mm_cmpeq_epi8(b, z), _mm_cmpeq_epi8(a, ff)));
+        if (m) return i + __builtin_ctz(m);
+    }
+#endif
+    for (; i + 1 < n; i++) {
+        if (dst && i - base < dst_room) dst[i - base] = s[i];
+        if (s[i] == 0xFF && s[i + 1] != 0) return i;
+    }
+    return n;
+}
+
 #define JPEG_BAD(idx, msg)                                                  \
     do {                                                                    \
         ::pifpaf::set_error("bad argument: JPEG %d: %s", (idx), (msg));     \
         return PIFPAF_E_BADARG;                                             \
     } while (0)
 
-// The tables of one stream live in `tabs` / `quant` (per stream: 4 DC + 4 AC tables, 4 quantisation tables).
-int parse_jpeg(int idx, const uint8_t* s, int64_t n, int64_t max_pixels, Huff* tabs, int32_t* quant, Parsed* out) {
+// The tables of one stream live in `tabs` / `quant` (per stream: 4 DC + 4 AC tables, 4 quantisation tables).  A GPU
+// route stream's scan bytes are copied to dst (room: the staging bytes left) by the walk that finds the scan's end.
+int parse_jpeg(int idx, const uint8_t* s, int64_t n, int64_t max_pixels, Huff* tabs, int32_t* quant, uint8_t* dst,
+               int64_t room, Parsed* out) {
     bool have_dc[4] = {}, have_ac[4] = {}, have_q[4] = {};
     bool frame = false, jfif = false;
     int adobe = -1, prec = 0, ri = 0;
@@ -692,10 +772,16 @@ int parse_jpeg(int idx, const uint8_t* s, int64_t n, int64_t max_pixels, Huff* t
         } else if (m == 0xDD) {
             if (sl != 2) JPEG_BAD(idx, "bad DRI length");
             ri = (seg[0] << 8) | seg[1];
-        } else if (m == 0xE0) {
-            jfif = jfif || (sl >= 5 && std::memcmp(seg, "JFIF\0", 5) == 0);
-        } else if (m == 0xEE) {
-            if (sl >= 12 && std::memcmp(seg, "Adobe", 5) == 0) adobe = seg[11];
+        } else if (m == 0xE0 || m == 0xEE) {
+            // Pillow's parser reads a 16-bit version at byte 5 of a JFIF or Adobe segment and refuses a shorter one
+            const bool jf = m == 0xE0 && sl >= 4 && std::memcmp(seg, "JFIF", 4) == 0;
+            const bool ad = m == 0xEE && sl >= 5 && std::memcmp(seg, "Adobe", 5) == 0;
+            if ((jf || ad) && sl < 7) {
+                out->route = PIFPAF_JPEG_PILLOW;
+                return PIFPAF_OK;
+            }
+            jfif = jfif || (jf && sl >= 14 && seg[4] == 0);          // libjpeg's examine_app0: APP0_DATA_LEN
+            if (ad && sl >= 12) adobe = seg[11];
         } else if (m == 0xDA) {
             if (!frame) JPEG_BAD(idx, "SOS before SOF");
             if (sl < 1 || sl != 4 + 2 * seg[0]) JPEG_BAD(idx, "bad SOS length");
@@ -745,10 +831,28 @@ int parse_jpeg(int idx, const uint8_t* s, int64_t n, int64_t max_pixels, Huff* t
                 out->route = PIFPAF_JPEG_PILLOW;
                 return PIFPAF_OK;
             }
+            // the entropy-coded bytes: FF00 is a data FF, FF fill bytes belong to the marker after them; RSTn and the
+            // codes below SOF0 end a data segment, the first other marker ends the scan
+            out->markers.clear();
             int64_t end = -1;
-            for (int64_t i = n - 2; i >= pos; i--)
-                if (s[i] == 0xFF && s[i + 1] == 0xD9) { end = i; break; }
-            if (end < pos) JPEG_BAD(idx, "no EOI after the scan (truncated stream)");
+            for (int64_t i = pos; end < 0;) {
+                const int64_t a = find_marker(s, i, n, dst, pos, room);
+                int64_t j = a;
+                while (j < n && s[j] == 0xFF) j++;
+                if (j >= n) JPEG_BAD(idx, "no EOI after the scan (truncated stream)");
+                for (int64_t k = a; k <= j && k - pos < room; k++) dst[k - pos] = s[k];
+                const int c = s[j];
+                if (c != 0 && (c < 0xC0 || (c >= 0xD0 && c <= 0xD7))) out->markers.push_back((uint8_t)c);
+                else if (c != 0) end = a;
+                i = j + 1;
+            }
+            bool eoi = false;
+            for (int64_t i = end; !eoi;) {
+                const int64_t a = find_marker(s, i, n);
+                if (a + 1 >= n) JPEG_BAD(idx, "no EOI after the scan (truncated stream)");
+                eoi = s[a + 1] == 0xD9;
+                i = a + 1;
+            }
             out->comps.clear();
             for (int ci : used) out->comps.push_back(comps[ci]);
             if (nf == 1) out->comps[0].h = out->comps[0].v = 1;   // not interleaved: one block per MCU
@@ -771,6 +875,7 @@ struct pifpaf_jpeg {
     uint8_t* d_stage;                      // mirror of the pinned staging area
     uint8_t* d_comp;
     int32_t *d_chunk_keep, *d_chunk_rst, *d_comp_len, *d_int_lo, *d_int_hi, *d_int_img, *d_int_sub, *d_int_nsub;
+    int32_t *d_int_blocks, *d_seg_lo;
     int32_t *d_sub_int, *d_sub_j, *d_count, *d_acc;
     long long *d_start, *d_exit0, *d_exit1;
     int16_t* d_coef;
@@ -787,15 +892,46 @@ struct pifpaf_jpeg {
 
 namespace {
 
-int64_t stage_layout(int64_t max_images, int64_t max_chunks, int64_t max_bytes, int64_t* off) {
+// the last region holds the batch's scan bytes, then (8-byte aligned after them) its interval table
+int64_t stage_layout(int64_t max_images, int64_t max_chunks, int64_t max_bytes, int64_t max_intervals, int64_t* off) {
     int64_t o = 0;
     auto take = [&](int64_t bytes) { const int64_t r = o; o = (o + bytes + 255) / 256 * 256; return r; };
     off[0] = take(max_images * sizeof(Img));
     off[1] = take(max_images * 8 * sizeof(Huff));
     off[2] = take(max_images * 4 * 64 * sizeof(int32_t));
     off[3] = take(max_chunks * sizeof(int32_t));
-    off[4] = take(max_bytes + 8);
+    off[4] = take(max_bytes + 16 + max_intervals * sizeof(int32_t));
     return o;
+}
+
+inline int64_t int_table_off(int64_t bytes) { return (bytes + 8 + 7) / 8 * 8; }
+
+// restart interval -> its data segment (segment k follows the k-th marker of the scan; -1: none, the interval decodes
+// an empty segment).  libjpeg's read_restart_marker / jpeg_resync_to_restart: interval i > 0 expects
+// RST((i - 1) mod 8); the expected marker, or one too far from it, is taken (action 1); a code below SOF0 or one of
+// the two RSTs before the expected one is skipped with the data after it (action 2); one of the next two, or the
+// scan's end, is left unread (action 3).
+void interval_segments(const std::vector<uint8_t>& markers, int n_int, int32_t* out) {
+    const int nm = (int)markers.size();
+    int cur = 0;
+    out[0] = 0;
+    for (int i = 1; i < n_int; i++) {
+        const int want = (i - 1) & 7;
+        out[i] = -1;
+        for (;;) {
+            const int c = cur < nm ? markers[cur] : 0xD9;
+            int action = 1;
+            if (c < 0xC0) action = 2;
+            else if (c < 0xD0 || c > 0xD7) action = 3;
+            else {
+                const int dn = (c - 0xD0 - want) & 7;
+                action = dn == 1 || dn == 2 ? 3 : dn == 6 || dn == 7 ? 2 : 1;
+            }
+            if (action == 3) break;
+            cur++;
+            if (action == 1) { out[i] = cur; break; }
+        }
+    }
 }
 
 inline unsigned grid(long long n, int threads) { return (unsigned)std::max<long long>(1, (n + threads - 1) / threads); }
@@ -816,11 +952,12 @@ int pifpaf_jpeg_create(pifpaf_jpeg_t** out, int32_t device, int32_t max_images, 
     h->max_bytes = max_bytes;
     h->max_pixels = max_pixels;
     h->max_blocks = max_blocks;
-    h->max_intervals = max_bytes / 2 + max_images;                      // every RSTn takes two bytes
+    h->max_intervals = max_bytes / 2 + max_images;                      // also bounds the data segments: a marker
+                                                                        // takes two bytes
     h->max_subs = max_bytes * 8 / SUBSEQ_BITS + h->max_intervals + max_images;
     h->max_chunks = max_bytes / CHUNK + max_images;
     int64_t off[5];
-    h->stage_bytes = stage_layout(max_images, h->max_chunks, max_bytes, off);
+    h->stage_bytes = stage_layout(max_images, h->max_chunks, max_bytes, h->max_intervals, off);
     int rc = PIFPAF_OK;
     auto alloc = [&](auto** p, size_t n) { if (rc == PIFPAF_OK) rc = pifpaf::dev_alloc(p, n, h->owned); };
     alloc(&h->d_stage, h->stage_bytes);
@@ -828,7 +965,9 @@ int pifpaf_jpeg_create(pifpaf_jpeg_t** out, int32_t device, int32_t max_images, 
     alloc(&h->d_chunk_keep, h->max_chunks);
     alloc(&h->d_chunk_rst, h->max_chunks);
     alloc(&h->d_comp_len, max_images);
-    for (int32_t** p : {&h->d_int_lo, &h->d_int_hi, &h->d_int_img, &h->d_int_sub, &h->d_int_nsub}) alloc(p, h->max_intervals);
+    for (int32_t** p : {&h->d_int_lo, &h->d_int_hi, &h->d_int_img, &h->d_int_sub, &h->d_int_nsub, &h->d_int_blocks,
+                        &h->d_seg_lo})
+        alloc(p, h->max_intervals);
     for (int32_t** p : {&h->d_sub_int, &h->d_sub_j, &h->d_count, &h->d_acc}) alloc(p, h->max_subs);
     for (long long** p : {&h->d_start, &h->d_exit0, &h->d_exit1}) alloc(p, h->max_subs);
     alloc(&h->d_coef, h->max_blocks * 64);
@@ -877,7 +1016,7 @@ int pifpaf_jpeg_decode(pifpaf_jpeg_t* h, int32_t n, const uint8_t* const* data, 
     PIFPAF_CUDA_TRY(cudaSetDevice(h->device));
     PIFPAF_CUDA_TRY(cudaEventSynchronize(h->staged));      // the previous batch's staging copy has been read
     int64_t off[5];
-    stage_layout(h->max_images, h->max_chunks, h->max_bytes, off);
+    stage_layout(h->max_images, h->max_chunks, h->max_bytes, h->max_intervals, off);
     Img* imgs = reinterpret_cast<Img*>(h->h_stage + off[0]);
     Huff* tabs = reinterpret_cast<Huff*>(h->h_stage + off[1]);
     int32_t* quant = reinterpret_cast<int32_t*>(h->h_stage + off[2]);
@@ -885,12 +1024,13 @@ int pifpaf_jpeg_decode(pifpaf_jpeg_t* h, int32_t n, const uint8_t* const* data, 
     uint8_t* raw = h->h_stage + off[4];
     // pass 1: parse and validate everything; nothing is launched or copied unless every stream is accepted
     int n_gpu = 0;
-    int64_t bytes = 0, chunks = 0, blocks = 0, px = 0, out = 0, intervals = 0, subs = 0;
+    int64_t bytes = 0, chunks = 0, blocks = 0, px = 0, out = 0, intervals = 0, subs = 0, segs = 0;
     std::vector<Parsed> ps(n);
     for (int i = 0; i < n; i++) {
         PIFPAF_CHECK_ARG(data[i] != nullptr && sizes[i] >= 0, "null stream");
         Parsed& p = ps[i];
-        PIFPAF_TRY(parse_jpeg(i, data[i], sizes[i], h->max_pixels, tabs + 8 * n_gpu, quant + 4 * 64 * n_gpu, &p));
+        PIFPAF_TRY(parse_jpeg(i, data[i], sizes[i], h->max_pixels, tabs + 8 * n_gpu, quant + 4 * 64 * n_gpu, raw + bytes,
+                              h->max_bytes + 16 - bytes, &p));
         routes[i] = p.route;
         hw[2 * i] = p.route == PIFPAF_JPEG_GPU ? p.h : 0;
         hw[2 * i + 1] = p.route == PIFPAF_JPEG_GPU ? p.w : 0;
@@ -935,6 +1075,8 @@ int pifpaf_jpeg_decode(pifpaf_jpeg_t* h, int32_t n, const uint8_t* const* data, 
         im.n_chunks = (im.seg_len + CHUNK - 1) / CHUNK;
         im.chunk_base = (int32_t)chunks;
         im.int_base = (int32_t)intervals;
+        im.seg_base = (int32_t)segs;
+        im.n_seg = (int32_t)p.markers.size() + 1;
         im.sub_base = (int32_t)subs;
         im.sub_cap = (int32_t)(((int64_t)im.seg_len * 8 + SUBSEQ_BITS - 1) / SUBSEQ_BITS + im.n_int);
         im.blk_base = blocks;
@@ -943,13 +1085,14 @@ int pifpaf_jpeg_decode(pifpaf_jpeg_t* h, int32_t n, const uint8_t* const* data, 
         bytes += im.seg_len;
         chunks += im.n_chunks;
         intervals += im.n_int;
+        segs += im.n_seg;
         subs += im.sub_cap;
         blocks += n_mcu * im.bpm;
         px += (int64_t)p.w * p.h;
         out += (int64_t)p.w * p.h * 3;
         if (bytes > h->max_bytes) JPEG_BAD(i, "the batch's scan data exceeds the handle's max_bytes");
         if (blocks > h->max_blocks) JPEG_BAD(i, "the batch's 8x8 blocks exceed the handle's max_blocks");
-        if (intervals > h->max_intervals || subs > h->max_subs || chunks > h->max_chunks)
+        if (intervals > h->max_intervals || segs > h->max_intervals || subs > h->max_subs || chunks > h->max_chunks)
             JPEG_BAD(i, "the batch's restart intervals exceed the handle's capacity");
         if (out > out_bytes) JPEG_BAD(i, "the output buffer is too small for the batch");
         out_offsets[i] = im.out_off;
@@ -961,15 +1104,17 @@ int pifpaf_jpeg_decode(pifpaf_jpeg_t* h, int32_t n, const uint8_t* const* data, 
     h->last_stream = st;
     PIFPAF_CUDA_TRY(cudaMemsetAsync(h->d_stats, 0, 2 * sizeof(unsigned long long), st));
     if (n_gpu == 0) return PIFPAF_OK;
-    // pass 2: stage the scan bytes and the chunk table, one copy
+    // pass 2: stage the chunk table and the interval table (the scan bytes were staged by the walk), one copy
+    int32_t* int_seg = reinterpret_cast<int32_t*>(raw + int_table_off(bytes));
     for (int i = 0, g = 0; i < n; i++) {
         if (ps[i].route != PIFPAF_JPEG_GPU) continue;
         const Img& im = imgs[g];
-        std::memcpy(raw + im.seg_off, data[i] + ps[i].seg_lo, im.seg_len);
         for (int c = 0; c < im.n_chunks; c++) chunk_img[im.chunk_base + c] = g;
+        interval_segments(ps[i].markers, im.n_int, int_seg + im.int_base);
         g++;
     }
-    PIFPAF_CUDA_TRY(cudaMemcpyAsync(h->d_stage, h->h_stage, off[4] + bytes, cudaMemcpyHostToDevice, st));
+    PIFPAF_CUDA_TRY(cudaMemcpyAsync(h->d_stage, h->h_stage, off[4] + int_table_off(bytes) + intervals * sizeof(int32_t),
+                                    cudaMemcpyHostToDevice, st));
     PIFPAF_CUDA_TRY(cudaEventRecord(h->staged, st));
 
     Dev d;
@@ -978,6 +1123,9 @@ int pifpaf_jpeg_decode(pifpaf_jpeg_t* h, int32_t n, const uint8_t* const* data, 
     d.quant = reinterpret_cast<const int32_t*>(h->d_stage + off[2]);
     d.chunk_img = reinterpret_cast<const int32_t*>(h->d_stage + off[3]);
     d.raw = h->d_stage + off[4];
+    d.int_seg = reinterpret_cast<const int32_t*>(d.raw + int_table_off(bytes));
+    d.seg_lo = h->d_seg_lo;
+    d.int_blocks = h->d_int_blocks;
     d.comp = h->d_comp;
     d.chunk_keep = h->d_chunk_keep; d.chunk_rst = h->d_chunk_rst; d.comp_len = h->d_comp_len;
     d.int_lo = h->d_int_lo; d.int_hi = h->d_int_hi; d.int_img = h->d_int_img; d.int_sub = h->d_int_sub;

@@ -2,11 +2,14 @@
 
 Each step is the same integer arithmetic the kernels do, written for clarity rather than speed:
   parse              marker walk, routing ('gpu' / 'pillow') and validation, as pifpaf_jpeg_decode's host code
+  scan_markers       the host's walk over the entropy-coded bytes: the scan's end and the markers inside it
+  interval_segments  the host's restart-interval table: libjpeg's resync policy over those markers
   huff_table         9-bit lookup + canonical maxcode / valoffset per DHT table
-  unstuff            FF00 removal and restart-interval starts (k_jpeg_unstuff)
+  unstuff            marker and FF00 removal, the compacted start of each data segment (k_jpeg_unstuff)
   decode_run         the Huffman decoder state machine over one interval (k_jpeg_sync / k_jpeg_write)
   self_sync          Weissenberger & Schmidt's self-synchronising decode, rounds capped, serial fallback
-  idct_islow         libjpeg's jidctint (CONST_BITS 13, PASS1_BITS 2) with the post-IDCT range limit
+  coefficients_serial  libjpeg's own decode loop (decode_mcu, insufficient_data), the yardstick for self_sync
+  idct_islow         libjpeg's jidctint (CONST_BITS 13, PASS1_BITS 2) as libjpeg-turbo's x86 SIMD code computes it
   upsample_h2v1/h2v2 libjpeg-turbo's fancy upsamplers (jdsample.c)
   ycc_to_rgb         jdcolor.c's fixed-point tables (SCALEBITS 16)
 `decode(data)` chains them into what `np.asarray(PIL.Image.open(data).convert('RGB'))` returns for 'gpu' streams.
@@ -130,8 +133,12 @@ def parse(data, max_pixels=1 << 62):
                 raise JpegError('bad DRI length')
             ri = (seg[0] << 8) | seg[1]
         elif m == 0xE0:
-            jfif = jfif or seg[:5] == b'JFIF\x00'
+            if seg[:4] == b'JFIF' and len(seg) < 7:
+                return 'pillow', 'JFIF segment Pillow cannot parse'
+            jfif = jfif or (len(seg) >= 14 and seg[:5] == b'JFIF\x00')     # libjpeg's examine_app0
         elif m == 0xEE:
+            if seg[:5] == b'Adobe' and len(seg) < 7:
+                return 'pillow', 'Adobe segment Pillow cannot parse'
             if seg[:5] == b'Adobe' and len(seg) >= 12:
                 adobe = seg[11]
         elif m == 0xDA:
@@ -188,9 +195,7 @@ def _scan(data, pos, seg, frame, qt, dc, ac, ri, jfif, adobe, max_pixels):
         return 'pillow', 'Huffman table not defined'
     if order != list(range(ns)):
         return 'pillow', 'scan order differs from frame order'
-    end = data.rfind(b'\xff\xd9')
-    if end < pos:
-        raise JpegError('no EOI after the scan (truncated stream)')
+    end, markers = scan_markers(data, pos)
     comps = [comps[i] for i in order]
     if len(comps) == 1:
         comps[0]['h'] = comps[0]['v'] = 1          # a one-component scan is not interleaved: 1 block per MCU
@@ -198,31 +203,86 @@ def _scan(data, pos, seg, frame, qt, dc, ac, ri, jfif, adobe, max_pixels):
     mx, my = -(-w // (8 * hmax)), -(-h // (8 * vmax))
     blocks = [(ci, bv, bh) for ci, c in enumerate(comps) for bv in range(c['v']) for bh in range(c['h'])]
     n_mcu = mx * my
+    n_int = -(-n_mcu // (ri or n_mcu))
     return 'gpu', dict(w=w, h=h, comps=comps, hmax=hmax, vmax=vmax, mx=mx, my=my, blocks=blocks, ri=ri or n_mcu,
-                       n_intervals=-(-n_mcu // (ri or n_mcu)), seg=(pos, end))
+                       n_intervals=n_int, seg=(pos, end), n_segments=len(markers) + 1,
+                       int_seg=interval_segments(n_int, markers))
+
+
+def scan_markers(data, pos):
+    """-> (end, marker codes): the host's walk over the entropy-coded bytes from pos.  FF00 is a data FF and FF fill
+    bytes belong to the marker they precede.  RSTn, and the codes below SOF0 that libjpeg's resync skips, end a data
+    segment and are listed; the first other marker ends the scan (end: its first FF).  An EOI must follow."""
+    n, i, markers = len(data), pos, []
+    while True:
+        a = data.find(b'\xff', i)
+        if a < 0:
+            raise JpegError('no EOI after the scan (truncated stream)')
+        j = a
+        while j < n and data[j] == 0xFF:
+            j += 1
+        if j >= n:
+            raise JpegError('no EOI after the scan (truncated stream)')
+        c = data[j]
+        if c != 0 and (0xD0 <= c <= 0xD7 or c < 0xC0):
+            markers.append(c)
+        elif c != 0:
+            if data.find(b'\xff\xd9', a) < 0:
+                raise JpegError('no EOI after the scan (truncated stream)')
+            return a, markers
+        i = j + 1
+
+
+def interval_segments(n_int, markers):
+    """restart interval -> the data segment it decodes (segment k follows the k-th marker; -1: none).  libjpeg's
+    read_restart_marker / jpeg_resync_to_restart: interval i > 0 expects RST((i - 1) mod 8).  The expected marker is
+    taken (action 1), and so is one too far from it; a marker below SOF0 or one of the two before the expected one is
+    skipped with the data after it (action 2); one of the next two, or any other marker (the scan's end), is left
+    unread and the interval decodes an empty segment (action 3)."""
+    out, cur = [0], 0
+    for i in range(1, n_int):
+        want = (i - 1) & 7
+        while True:
+            c = markers[cur] if cur < len(markers) else 0xD9
+            if c < 0xC0:
+                action = 2
+            elif not 0xD0 <= c <= 0xD7:
+                action = 3
+            else:
+                action = {0: 1, 1: 3, 2: 3, 6: 2, 7: 2}.get((c - 0xD0 - want) & 7, 1)
+            if action == 2:
+                cur += 1
+                continue
+            if action == 1:
+                cur += 1
+            out.append(cur if action == 1 else -1)
+            break
+    return out
 
 
 # ------------------------------------------------------------------------------------------------------ entropy data
 def unstuff(data, seg):
-    """-> (compacted bytes, [start byte of each interval]).  FF00 -> FF; FF D0..D7 dropped and recorded."""
+    """-> (compacted bytes, [compacted start of each data segment]).  Data bytes are kept (FF00 -> FF); FF fill bytes
+    and every marker inside the scan are dropped, and each marker starts the next data segment."""
     s = data[seg[0]:seg[1]]
     out, starts = bytearray(), [0]
-    i = 0
-    while i < len(s):
-        b = s[i]
-        if b == 0xFF and i + 1 < len(s):
-            nb = s[i + 1]
-            if nb == 0x00:
+    for i, b in enumerate(s):
+        nxt = s[i + 1] if i + 1 < len(s) else None
+        if b == 0xFF:
+            if nxt == 0x00:
                 out.append(0xFF)
-                i += 2
-                continue
-            if 0xD0 <= nb <= 0xD7:
+        elif i > 0 and s[i - 1] == 0xFF:
+            if b != 0x00:
                 starts.append(len(out))
-                i += 2
-                continue
-        out.append(b)
-        i += 1
+        else:
+            out.append(b)
     return bytes(out), starts
+
+
+def interval_bounds(hdr, buf, starts):
+    """[(lo, hi, empty)] per restart interval: its data segment's compacted byte range"""
+    ends = list(starts[1:]) + [len(buf)]
+    return [(starts[g], ends[g], False) if g >= 0 else (0, 0, True) for g in hdr['int_seg']]
 
 
 class Bits:
@@ -251,7 +311,7 @@ def huff_decode(tbl, bits, pos):
         ln += 1
         code = bits.peek(pos, ln) if ln <= 16 else code
     if ln > 16:
-        return 0, 16                               # corrupt code: a zero symbol, like libjpeg
+        return 0, 17                               # corrupt code: 17 bits read and a zero symbol, like libjpeg
     return int(tbl['vals'][int(tbl['valoffset'][ln]) + code]), ln
 
 
@@ -259,15 +319,17 @@ def extend(v, s):
     return v - (1 << s) + 1 if s and v < (1 << (s - 1)) else v
 
 
-def decode_run(hdr, bits, state, end_bit, emit=None, max_blocks=None):
+def decode_run(hdr, bits, state, end_bit, emit=None, max_blocks=None, tail=False):
     """Decode from state (bit, block in MCU, k) until the first codeword boundary at or after end_bit (or after
-    max_blocks block starts).  emit(block_starts_so_far_minus_one, natural index, value) receives every coefficient
-    (DC: the difference).  -> (exit state, number of block starts)"""
+    max_blocks block starts).  The tail of an interval (end_bit: its last bit) goes on to the end of an MCU whose bits
+    run past its data, and decodes one more MCU if its data ends exactly at an MCU boundary: libjpeg finishes the MCU
+    that runs out of data with zero bits.  emit(block_starts_so_far_minus_one, natural index, value) receives every
+    coefficient (DC: the difference).  -> (exit state, number of block starts)"""
     pos, blk, k = state
     comps, blocks = hdr['comps'], hdr['blocks']
     bpm = len(blocks)
     nstart = 0
-    while pos < end_bit:
+    while pos < end_bit or (tail and (pos == end_bit or blk or k)):
         c = comps[blocks[blk][0]]
         if k == 0:
             if max_blocks is not None and nstart >= max_blocks:
@@ -307,50 +369,96 @@ def interval_blocks(hdr, i):
     return (min(lo + hdr['ri'], n_mcu) - lo) * len(hdr['blocks'])
 
 
+def decode_block(comp, bits, pos, out):
+    """libjpeg's decode_mcu_slow for one block: -> bit position after it; out[natural index] = value (DC: the
+    difference).  Written apart from decode_run's state machine on purpose."""
+    s, ln = huff_decode(comp['dc'], bits, pos)
+    pos += ln
+    out[0] = extend(bits.peek(pos, s), s) if s else 0
+    pos += s
+    k = 1
+    while k < 64:
+        rs, ln = huff_decode(comp['ac'], bits, pos)
+        pos += ln
+        r, s = rs >> 4, rs & 15
+        if s:
+            k += r
+            out[ZIGZAG[min(k, 63)]] = extend(bits.peek(pos, s), s)
+            pos += s
+        elif r != 15:
+            break
+        else:
+            k += 15
+        k += 1
+    return pos
+
+
 def coefficients_serial(hdr, buf, starts):
-    """int64 [n_blocks, 64] in scan order, DC resolved (the serial decode, libjpeg's order)"""
+    """int64 [n_blocks, 64] in scan order, DC resolved: libjpeg's decode loop.  Bits past an interval's data read as
+    zeros.  The MCU whose bits run past the data sets insufficient_data; every later MCU is left all zero (DC an
+    absolute 0) until a restart that takes its marker clears the flag.  An interval whose marker was left unread
+    keeps it."""
     nb = len(hdr['blocks'])
     coef = np.zeros((hdr['mx'] * hdr['my'] * nb, 64), dtype=np.int64)
-    ends = list(starts[1:hdr['n_intervals']]) + [len(buf)]
-    for i in range(hdr['n_intervals']):
-        lo = starts[i] if i < len(starts) else len(buf)
-        hi = ends[i] if i < len(ends) else len(buf)
-        base, cnt = i * hdr['ri'] * nb, interval_blocks(hdr, i)
-
-        def emit(b, z, v):
-            coef[base + b, z] = v
-        decode_run(hdr, Bits(buf, lo, hi), (0, 0, 0), 1 << 62, emit, max_blocks=cnt)
-    resolve_dc(hdr, coef)
+    insufficient = False
+    for i, (lo, hi, empty) in enumerate(interval_bounds(hdr, buf, starts)):
+        insufficient = insufficient and empty
+        bits, pos, last_dc = Bits(buf, lo, hi), 0, [0] * len(hdr['comps'])
+        base = i * hdr['ri'] * nb
+        for m in range(interval_blocks(hdr, i) // nb):
+            if insufficient:
+                break
+            for t, (ci, _, _) in enumerate(hdr['blocks']):
+                row = coef[base + m * nb + t]
+                pos = decode_block(hdr['comps'][ci], bits, pos, row)
+                last_dc[ci] += int(row[0])
+                row[0] = ((last_dc[ci] + 32768) & 0xFFFF) - 32768                 # (JCOEF) of the int predictor
+            insufficient = pos > 8 * (hi - lo)
     return coef
 
 
-def resolve_dc(hdr, coef):
-    """DC differences -> DC values: a prefix sum per component, reset at every interval start"""
+def resolve_dc(hdr, coef, live):
+    """DC differences -> DC values: a prefix sum per component, reset at every interval start; a block at or after
+    its interval's live count keeps an absolute DC of 0 (k_jpeg_dc)"""
     nb = len(hdr['blocks'])
     comp_of = np.array([b[0] for b in hdr['blocks']])
     blk_comp = np.tile(comp_of, coef.shape[0] // nb)
     interval = np.arange(coef.shape[0]) // (hdr['ri'] * nb)
+    dead = np.arange(coef.shape[0]) - interval * hdr['ri'] * nb >= np.asarray(live)[interval]
+    coef[dead, 0] = 0
     for c in range(len(hdr['comps'])):
         sel = np.nonzero(blk_comp == c)[0]
         d = coef[sel, 0]
-        cs = np.cumsum(d)
         seg = interval[sel]
-        first = np.r_[True, seg[1:] != seg[:-1]]
+        first = np.r_[True, seg[1:] != seg[:-1]] | dead[sel]
+        cs = np.cumsum(d)
         head = np.maximum.accumulate(np.where(first, np.arange(len(sel)), 0))
-        coef[sel, 0] = cs - (cs - d)[head]
+        coef[sel, 0] = (cs - (cs - d)[head]).astype(np.int32).astype(np.int16)
 
 
 def subsequences(hdr, buf, starts, S):
-    """[(interval, Bits, start bit, end bit, first of its interval)]: each interval cut into S-bit pieces (at least one)"""
-    ends = list(starts[1:hdr['n_intervals']]) + [len(buf)]
+    """[(interval, Bits, start bit, end bit, first of its interval, last of its interval)]: each interval cut into
+    S-bit pieces (at least one)"""
     subs = []
-    for i in range(hdr['n_intervals']):
-        lo = min(starts[i], len(buf)) if i < len(starts) else len(buf)
-        hi = max(lo, min(ends[i], len(buf)) if i < len(ends) else len(buf))
+    for i, (lo, hi, _) in enumerate(interval_bounds(hdr, buf, starts)):
         nbits, bits = 8 * (hi - lo), Bits(buf, lo, hi)
-        for j in range(max(1, -(-nbits // S))):
-            subs.append((i, bits, j * S, min((j + 1) * S, nbits), j == 0))
+        n = max(1, -(-nbits // S))
+        for j in range(n):
+            subs.append((i, bits, j * S, min((j + 1) * S, nbits), j == 0, j == n - 1))
     return subs
+
+
+def interval_live(hdr, buf, starts, decoded):
+    """blocks of each interval the decode keeps (k_jpeg_write / k_jpeg_dc): decoded[i] is the interval's block starts
+    up to the MCU that ran past its data.  At most the interval's blocks started there: the interval starved.  An
+    empty interval after a starved one is dead (libjpeg's flag survives a marker left unread): it keeps none."""
+    bounds = interval_bounds(hdr, buf, starts)
+    live = []
+    for i, n in enumerate(decoded):
+        cnt = interval_blocks(hdr, i)
+        starved_before = i > 0 and (bounds[i - 1][2] or decoded[i - 1] <= interval_blocks(hdr, i - 1))
+        live.append(0 if bounds[i][2] and starved_before else min(n, cnt))
+    return live
 
 
 def self_sync(hdr, buf, starts, S, max_rounds):
@@ -359,7 +467,7 @@ def self_sync(hdr, buf, starts, S, max_rounds):
     fixed point every start is exact by induction from the first subsequence of each interval.  After max_rounds rounds
     a serial pass per interval re-decodes each subsequence whose start still differs from its predecessor's exit
     (max_rounds 0: every subsequence).  The write pass then decodes each subsequence again from its settled start into
-    block (interval base + the block starts of the subsequences before it).
+    block (interval base + the block starts of the subsequences before it), up to the interval's live blocks.
     -> (coefficients like coefficients_serial, rounds that decoded something, fallback decodes)"""
     nb = len(hdr['blocks'])
     subs = subsequences(hdr, buf, starts, S)
@@ -375,7 +483,7 @@ def self_sync(hdr, buf, starts, S, max_rounds):
                 if subs[j][4] or prev[j - 1] == start[j]:
                     continue
                 start[j] = prev[j - 1]
-            exit_[j], count[j] = decode_run(hdr, subs[j][1], start[j], subs[j][3])
+            exit_[j], count[j] = decode_run(hdr, subs[j][1], start[j], subs[j][3], tail=subs[j][5])
             work = True
         rounds += work
         if not work:
@@ -385,21 +493,26 @@ def self_sync(hdr, buf, starts, S, max_rounds):
         if max_rounds == 0 or (not subs[j][4] and exit_[j - 1] != start[j]):
             if not subs[j][4]:
                 start[j] = exit_[j - 1]
-            exit_[j], count[j] = decode_run(hdr, subs[j][1], start[j], subs[j][3])
+            exit_[j], count[j] = decode_run(hdr, subs[j][1], start[j], subs[j][3], tail=subs[j][5])
             fallbacks += 1
+    decoded = [0] * hdr['n_intervals']
+    for j in range(n):
+        decoded[subs[j][0]] += count[j]
+    live = interval_live(hdr, buf, starts, decoded)
     coef = np.zeros((hdr['mx'] * hdr['my'] * nb, 64), dtype=np.int64)
     acc = 0
     for j in range(n):
         i = subs[j][0]
         acc = 0 if subs[j][4] else acc
-        base, cnt = i * hdr['ri'] * nb, interval_blocks(hdr, i)
+        base, cnt = i * hdr['ri'] * nb, live[i]
 
         def emit(b, z, v, at=base + acc, lim=cnt - acc):
             if b < lim:                            # b == -1: the block the previous subsequence began
                 coef[at + b, z] = v
-        decode_run(hdr, subs[j][1], start[j], subs[j][3], emit, max_blocks=max(cnt - acc, 0))
+        if cnt:
+            decode_run(hdr, subs[j][1], start[j], subs[j][3], emit, max_blocks=max(cnt - acc, 0), tail=subs[j][5])
         acc += count[j]
-    resolve_dc(hdr, coef)
+    resolve_dc(hdr, coef, live)
     return coef, rounds, fallbacks
 
 
@@ -409,16 +522,22 @@ FIX = dict(p298=2446, p390=3196, p541=4433, p765=6270, p899=7373, p1175=9633, p1
 CONST_BITS, PASS1_BITS = 13, 2
 
 
+def wrap16(x):
+    return ((x + 32768) & 0xFFFF) - 32768
+
+
 def _idct_1d(s0, s1, s2, s3, s4, s5, s6, s7, shift):
+    """jidctint's 1-D pass as libjpeg-turbo's SSE2 / AVX2 code computes it: in0 +- in4, in7 + in3 and in5 + in1 are
+    16-bit adds (paddw / psubw); every other term is a pmaddwd of 16-bit inputs into 32 bits, which does not overflow"""
     F = FIX
     z1 = (s2 + s6) * F['p541']
     tmp2 = z1 + s6 * -F['p1847']
     tmp3 = z1 + s2 * F['p765']
-    tmp0 = (s0 + s4) << CONST_BITS
-    tmp1 = (s0 - s4) << CONST_BITS
+    tmp0 = wrap16(s0 + s4) << CONST_BITS
+    tmp1 = wrap16(s0 - s4) << CONST_BITS
     tmp10, tmp13, tmp11, tmp12 = tmp0 + tmp3, tmp0 - tmp3, tmp1 + tmp2, tmp1 - tmp2
     t0, t1, t2, t3 = s7, s5, s3, s1
-    z1, z2, z3, z4 = t0 + t3, t1 + t2, t0 + t2, t1 + t3
+    z1, z2, z3, z4 = t0 + t3, t1 + t2, wrap16(t0 + t2), wrap16(t1 + t3)
     z5 = (z3 + z4) * F['p1175']
     t0, t1, t2, t3 = t0 * F['p298'], t1 * F['p2053'], t2 * F['p3072'], t3 * F['p1501']
     z1, z2, z3, z4 = z1 * -F['p899'], z2 * -F['p2562'], z3 * -F['p1961'], z4 * -F['p390']
@@ -432,15 +551,22 @@ def _idct_1d(s0, s1, s2, s3, s4, s5, s6, s7, shift):
 
 
 def idct_islow(coef, q):
-    """coef int64 [N, 64] natural order, q [64] -> uint8 [N, 8, 8] (jidctint.c, range-limited like IDCT_range_limit)"""
-    d = (coef * q[None, :]).reshape(-1, 8, 8)
+    """coef int64 [N, 64] natural order, q [64] -> uint8 [N, 8, 8]: jidctint.c's arithmetic as the x86 SIMD islow IDCT
+    of libjpeg-turbo (jidctint-sse2 / -avx2, what Pillow's bundled libjpeg-turbo runs on x86-64) computes it:
+      - the dequantised product is a 16-bit multiply (pmullw);
+      - pass 1: a block whose coefficient rows 1..7 are all zero takes a shortcut, every workspace row = the
+        dequantised row 0 << PASS1_BITS in 16 bits (psllw, wrapping); otherwise the 1-D pass with its 16-bit sums,
+        packed to int16 with saturation (packssdw);
+      - pass 2: the 1-D pass with its 16-bit sums, the output saturated to int8 (packssdw, packsswb) plus 128.
+    The C code (and other SIMD back ends) agree unless a damaged block overshoots 16 bits or the sample range."""
+    d = wrap16(coef * q[None, :]).reshape(-1, 8, 8)
     cols = _idct_1d(*[d[:, i, :] for i in range(8)], CONST_BITS - PASS1_BITS)      # pass 1: columns
-    ws = np.stack(cols, axis=1)                                                    # [N, row, col]
+    ws = np.clip(np.stack(cols, axis=1), -32768, 32767)                            # [N, row, col]
+    dc_rows = ~(coef.reshape(-1, 8, 8)[:, 1:, :] != 0).any(axis=(1, 2))
+    ws[dc_rows] = wrap16(d[dc_rows, :1, :] << PASS1_BITS)
     rows = _idct_1d(*[ws[:, :, i] for i in range(8)], CONST_BITS + PASS1_BITS + 3)  # pass 2: rows
     out = np.stack(rows, axis=2)
-    m = out & 1023
-    s = np.where(m >= 512, m - 1024, m)
-    return np.clip(s + 128, 0, 255).astype(np.uint8)
+    return (np.clip(out, -128, 127) + 128).astype(np.uint8)
 
 
 def planes(hdr, coef):
