@@ -232,6 +232,35 @@ int pifpaf_image_resize_bilinear_u8(const uint8_t* src_dev, int32_t src_h, int32
  * transforms/pad.py:52-54; CenterPadTight uses (124, 116, 104), transforms/pad.py:100-101) */
 int pifpaf_image_fill_rgb(uint8_t* dst_dev, int64_t n_pixels, int32_t r, int32_t g, int32_t b, void* stream);
 
+/* The reference's precise rescale: transforms.RescaleAbsolute(fast=False) (the default of every evaluation
+ * preprocess, and Predictor under --precise-rescaling) -> scipy.ndimage.zoom(im, (th / h, tw / w, 1), order=1)
+ * (transforms/scale.py:60-67), then CenterPad / CenterPadTight.  A whole batch in one launch: one thread per canvas
+ * pixel of canvas [n_images][canvas_h][canvas_w][3] writes the image's pad colour outside its window and, inside,
+ * scipy's float64 order-1 interpolation converted to uint8 as scipy does (openpifpaf_b200/preprocess.py states the
+ * rules).  Per axis and output index, a tap holds scipy's first input index and weights; i0 = -1 marks an output
+ * row or column that scipy's mode='constant' sets to cval = 0.  The host restatement builds the taps
+ * (preprocess.scipy_zoom_tables), so one definition of the coordinate arithmetic serves both.
+ *   images / taps: HOST arrays; they are checked here (sizes >= 1, the window inside the canvas, each table within
+ *   taps and its indices within the source) and staged into workspace_dev, which holds at least
+ *   n_images * sizeof(pifpaf_zoom_image_t) + n_taps * sizeof(pifpaf_zoom_tap_t) bytes.  src: device [h][w][3].
+ *   A refused call (PIFPAF_E_BADARG) stages and writes nothing. */
+typedef struct {
+    double w0, w1;          /* weights of input i0 and i1 */
+    int32_t i0, i1;         /* input indices; i0 = -1: outside the input, cval */
+} pifpaf_zoom_tap_t;
+typedef struct {
+    const uint8_t* src;     /* device [h][w][3] */
+    int32_t h, w;           /* source size */
+    int32_t th, tw;         /* target size */
+    int32_t left, top;      /* window offset in the canvas */
+    int32_t ytab, xtab;     /* first tap of the row table (th taps) and the column table (tw taps) */
+    uint8_t fill[4];        /* pad colour r, g, b; fill[3] is unused */
+} pifpaf_zoom_image_t;
+int pifpaf_image_zoom_linear_u8(const pifpaf_zoom_image_t* images, int32_t n_images,
+                                const pifpaf_zoom_tap_t* taps, int64_t n_taps,
+                                void* workspace_dev, int64_t workspace_bytes,
+                                uint8_t* canvas_dev, int32_t canvas_h, int32_t canvas_w, void* stream);
+
 
 /* ------------------------------------------------------------------------ */
 /* Baseline JPEG decode, bit-identical to PIL.Image.open(f).convert('RGB') (datasets/image_list.py:18; Pillow's

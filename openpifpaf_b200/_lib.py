@@ -41,6 +41,12 @@ class CifDetParams(ctypes.Structure):
     ]
 
 
+class ZoomImage(ctypes.Structure):
+    """pifpaf_zoom_image_t"""
+    _fields_ = [('src', VP), ('h', c_i32), ('w', c_i32), ('th', c_i32), ('tw', c_i32), ('left', c_i32),
+                ('top', c_i32), ('ytab', c_i32), ('xtab', c_i32), ('fill', ctypes.c_uint8 * 4)]
+
+
 # every symbol include/pifpaf_b200.h declares: name -> (restype, argtypes)
 SYMBOLS = {
     'pifpaf_last_error': (ctypes.c_char_p, []),
@@ -73,6 +79,7 @@ SYMBOLS = {
     'pifpaf_image_resize_bilinear_u8': (ctypes.c_int, [VP, c_i32, c_i32, VP, c_i64, c_i32, c_i32, VP, VP, c_i32,
                                                         VP, VP, c_i32, VP, VP]),
     'pifpaf_image_fill_rgb': (ctypes.c_int, [VP, c_i64, c_i32, c_i32, c_i32, VP]),
+    'pifpaf_image_zoom_linear_u8': (ctypes.c_int, [VP, c_i32, VP, c_i64, VP, c_i64, VP, c_i32, c_i32, VP]),
     'pifpaf_jpeg_create': (ctypes.c_int, [P(VP), c_i32, c_i32, c_i64, c_i64, c_i64]),
     'pifpaf_jpeg_destroy': (None, [VP]),
     'pifpaf_jpeg_decode': (ctypes.c_int, [VP, c_i32, P(VP), P(c_i64), VP, c_i64, c_i32, P(c_i32), P(c_i32), P(c_i64),

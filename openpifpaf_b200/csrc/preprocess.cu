@@ -2,6 +2,7 @@
 //
 // Replaces, for the inference path of the reference's Predictor (predictor.py:85-102):
 //   transforms.RescaleAbsolute(long_edge, fast=True)   transforms/scale.py:154-176 -> PIL.Image.resize(BILINEAR)
+//   transforms.RescaleAbsolute(long_edge, fast=False)  transforms/scale.py:60-67 -> scipy.ndimage.zoom(order=1)
 //   transforms.CenterPad / CenterPadTight              transforms/pad.py:15-110
 // ToTensor + Normalize (transforms/__init__.py:26-33) already run inside the stem kernel (pifpaf_net_forward_u8).
 //
@@ -11,6 +12,14 @@
 // the antialiased triangle filter, normalised, in fixed point with 22 fractional bits (host side:
 // openpifpaf_b200/preprocess.py, IEEE double arithmetic in Pillow's order), accumulated in 32-bit integers from
 // 1 << 21 and shifted down -- integer arithmetic, so the resized image equals Pillow's bit for bit.
+//
+// The precise rescale, transforms.RescaleAbsolute(fast=False) -> scipy.ndimage.zoom(order=1) (transforms/scale.py:
+// 60-67), is k_zoom_linear: one thread per canvas pixel of a whole batch, pad colour outside the window, inside it
+// scipy's zoom_shift for order 1 in float64.  The per-axis taps come from the host restatement
+// (preprocess.scipy_zoom_tables).  The channel axis zooms by exactly 1, so its weights are exactly 1 and 0: each of
+// the four (y, x) terms is (v * wy) * wx, and the channel's zero-weight terms add +0.0, which changes nothing.  The
+// sum runs in scipy's order from 0.0, and the uint8 store is scipy's: t > 0 ? t + 0.5 : 0, clamped to 255,
+// truncated.  This file is built with FMA contraction on, so the arithmetic is written with __dmul_rn / __dadd_rn.
 #include <algorithm>
 #include <cstdint>
 
@@ -81,7 +90,60 @@ __global__ void __launch_bounds__(256) k_fill_rgb(uint8_t* __restrict__ dst, lon
     }
 }
 
+// scipy's uint8 store of an interpolated value (CASE_INTERP_OUT_UINT): round half up by adding 0.5, clamp, truncate
+__device__ __forceinline__ uint8_t scipy_u8(double t) {
+    t = t > 0.0 ? __dadd_rn(t, 0.5) : 0.0;
+    t = t > 255.0 ? 255.0 : t;
+    return (uint8_t)__double2uint_rz(t);
+}
+
+// canvas [n][ch][cw][3]: one thread per pixel, each image's window at (left, top) is scipy.ndimage.zoom(order=1)
+// of its source, everything else its pad colour
+__global__ void __launch_bounds__(256) k_zoom_linear(const pifpaf_zoom_image_t* __restrict__ images,
+                                                     const pifpaf_zoom_tap_t* __restrict__ taps,
+                                                     uint8_t* __restrict__ canvas, int ch, int cw, long long total) {
+    const long long plane = (long long)ch * cw;
+    for (long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x; t < total; t += (long long)gridDim.x * blockDim.x) {
+        const int b = (int)(t / plane);
+        const int p = (int)(t - (long long)b * plane);
+        const pifpaf_zoom_image_t& im = images[b];
+        const int yy = p / cw - im.top, xx = p % cw - im.left;
+        uint8_t* o = canvas + 3 * t;
+        if (yy < 0 || yy >= im.th || xx < 0 || xx >= im.tw) {
+            o[0] = im.fill[0]; o[1] = im.fill[1]; o[2] = im.fill[2];
+            continue;
+        }
+        const pifpaf_zoom_tap_t ty = taps[im.ytab + yy], tx = taps[im.xtab + xx];
+        if (ty.i0 < 0 || tx.i0 < 0) {                      // mode='constant': outside the input, cval = 0
+            o[0] = 0; o[1] = 0; o[2] = 0;
+            continue;
+        }
+        const uint8_t* r0 = im.src + (size_t)ty.i0 * im.w * 3;
+        const uint8_t* r1 = im.src + (size_t)ty.i1 * im.w * 3;
+        const int c0 = 3 * tx.i0, c1 = 3 * tx.i1;
+#pragma unroll
+        for (int c = 0; c < 3; c++) {
+            double s = __dmul_rn(__dmul_rn((double)r0[c0 + c], ty.w0), tx.w0);
+            s = __dadd_rn(s, __dmul_rn(__dmul_rn((double)r0[c1 + c], ty.w0), tx.w1));
+            s = __dadd_rn(s, __dmul_rn(__dmul_rn((double)r1[c0 + c], ty.w1), tx.w0));
+            s = __dadd_rn(s, __dmul_rn(__dmul_rn((double)r1[c1 + c], ty.w1), tx.w1));
+            o[c] = scipy_u8(s);
+        }
+    }
+}
+
 inline int grid_for(long long total) { return (int)std::min<long long>((total + 255) / 256, 132LL * 16); }
+
+// the taps of one axis of one image lie within the staged table and index its source
+bool taps_ok(const pifpaf_zoom_tap_t* taps, int64_t n_taps, int64_t first, int32_t n_out, int32_t n_in) {
+    if (first < 0 || first + n_out > n_taps) return false;
+    for (int32_t k = 0; k < n_out; k++) {
+        const pifpaf_zoom_tap_t& tp = taps[first + k];
+        if (tp.i0 == -1) continue;
+        if (tp.i0 < 0 || tp.i0 >= n_in || tp.i1 < 0 || tp.i1 >= n_in) return false;
+    }
+    return true;
+}
 
 }  // namespace
 
@@ -134,6 +196,38 @@ int pifpaf_image_resize_bilinear_u8(const uint8_t* src_dev, int32_t src_h, int32
         k_copy_rows<<<grid_for((long long)dst_h * dst_w * 3), 256, 0, st>>>(src_dev, dst_h, dst_w * 3, dst_dev, dst_pitch_bytes);
         PIFPAF_LAUNCH_CHECK();
     }
+    return PIFPAF_OK;
+}
+
+int pifpaf_image_zoom_linear_u8(const pifpaf_zoom_image_t* images, int32_t n_images,
+                                const pifpaf_zoom_tap_t* taps, int64_t n_taps,
+                                void* workspace_dev, int64_t workspace_bytes,
+                                uint8_t* canvas_dev, int32_t canvas_h, int32_t canvas_w, void* stream_v) {
+    PIFPAF_CHECK_ARG(images != nullptr && n_images >= 1, "no images");
+    PIFPAF_CHECK_ARG(taps != nullptr && n_taps >= 1, "tap tables missing");
+    PIFPAF_CHECK_ARG(canvas_dev != nullptr && workspace_dev != nullptr, "canvas or workspace pointer is null");
+    PIFPAF_CHECK_ARG(canvas_h >= 1 && canvas_w >= 1, "bad canvas size");
+    const size_t desc_bytes = sizeof(pifpaf_zoom_image_t) * (size_t)n_images;
+    const size_t tap_bytes = sizeof(pifpaf_zoom_tap_t) * (size_t)n_taps;
+    PIFPAF_CHECK_ARG(workspace_bytes >= 0 && (size_t)workspace_bytes >= desc_bytes + tap_bytes, "workspace too small");
+    for (int32_t i = 0; i < n_images; i++) {
+        const pifpaf_zoom_image_t& im = images[i];
+        PIFPAF_CHECK_ARG(im.src != nullptr, "image pointer is null");
+        PIFPAF_CHECK_ARG(im.h >= 1 && im.w >= 1 && im.th >= 1 && im.tw >= 1, "bad image size");
+        PIFPAF_CHECK_ARG(im.left >= 0 && im.top >= 0 && (int64_t)im.left + im.tw <= canvas_w
+                         && (int64_t)im.top + im.th <= canvas_h, "window outside the canvas");
+        PIFPAF_CHECK_ARG(taps_ok(taps, n_taps, im.ytab, im.th, im.h), "row taps missing or outside the source");
+        PIFPAF_CHECK_ARG(taps_ok(taps, n_taps, im.xtab, im.tw, im.w), "column taps missing or outside the source");
+    }
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_v);
+    auto* ws = static_cast<uint8_t*>(workspace_dev);
+    PIFPAF_CUDA_TRY(cudaMemcpyAsync(ws, images, desc_bytes, cudaMemcpyHostToDevice, st));
+    PIFPAF_CUDA_TRY(cudaMemcpyAsync(ws + desc_bytes, taps, tap_bytes, cudaMemcpyHostToDevice, st));
+    const long long total = (long long)n_images * canvas_h * canvas_w;
+    k_zoom_linear<<<grid_for(total), 256, 0, st>>>(reinterpret_cast<const pifpaf_zoom_image_t*>(ws),
+                                                   reinterpret_cast<const pifpaf_zoom_tap_t*>(ws + desc_bytes),
+                                                   canvas_dev, canvas_h, canvas_w, total);
+    PIFPAF_LAUNCH_CHECK();
     return PIFPAF_OK;
 }
 

@@ -4,13 +4,16 @@ Reference (paths relative to the reference's src/openpifpaf/):
   Predictor._preprocess_factory        predictor.py:85-102   NormalizeAnnotations, RescaleAbsolute, CenterPad /
                                                              CenterPadTight(16), EVAL_TRANSFORM
   transforms.RescaleAbsolute / _scale  transforms/scale.py:28-100,154-176   (fast=True, OpenCV absent:
-                                                             PIL.Image.resize((w, h), BILINEAR), scale.py:56-59)
+                                                             PIL.Image.resize((w, h), BILINEAR), scale.py:56-59;
+                                                             fast=False: scipy.ndimage.zoom(order=1), scale.py:60-67)
   transforms.CenterPad / CenterPadTight  transforms/pad.py:15-110
   Annotation.inverse_transform / json_data / score / bbox   annotation.py:96-214
 
 `GpuPreprocess` takes the RAW uint8 images of a batch, resizes them on the GPU bit-identically to Pillow
 (pifpaf_image_resize_bilinear_u8; Pillow's ImagingResample restated, this module builds its coefficient tables) straight
-into the centre of a padded uint8 canvas, and returns the canvas -- the input of `CompiledNet.forward_uint8`, whose stem
+into the centre of a padded uint8 canvas -- or, with fast_rescaling=False (RescaleAbsolute(fast=False),
+transforms/scale.py:60-67), bit-identically to scipy.ndimage.zoom(order=1) (pifpaf_image_zoom_linear_u8, the whole
+batch in one launch; `scipy_zoom_tables` / `zoom_linear_reference` restate scipy) -- and returns the canvas -- the input of `CompiledNet.forward_uint8`, whose stem
 applies ToTensor + Normalize -- together with the per-image `meta` dicts the reference's transforms would have produced.
 `GpuJpegDecoder` decodes baseline JPEG files on the GPU bit-identically to PIL.Image.open(f).convert('RGB')
 (datasets/image_list.py:18), the step before them; streams the GPU does not decode are decoded by Pillow.
@@ -28,6 +31,7 @@ import torch
 from . import _lib
 
 PRECISION_BITS = 32 - 8 - 2          # Pillow src/libImaging/Resample.c
+BILINEAR = 2                         # PIL.Image.Resampling.BILINEAR, RescaleAbsolute's default resample
 TIGHT_PAD_FILL = (124, 116, 104)     # transforms/pad.py:100-101
 
 
@@ -81,6 +85,66 @@ def resize_bilinear_reference(image, target_w, target_h):
     if target_h != h:
         img = one_pass(img, *pil_bilinear_coeffs(h, target_h), axis=0)
     return img
+
+
+ZOOM_TAP = np.dtype([('w0', '<f8'), ('w1', '<f8'), ('i0', '<i4'), ('i1', '<i4')])     # pifpaf_zoom_tap_t
+
+
+def scipy_zoom_tables(n_in, n_out):
+    """One axis of scipy.ndimage.zoom(..., order=1, mode='constant', cval=0, grid_mode=False) from n_in to n_out
+    samples: per output index a pifpaf_zoom_tap_t (`ZOOM_TAP`) -- first input index i0, second index i1, weights
+    w0 / w1, and i0 = -1 where scipy writes cval.  Established from scipy's wrapper (ndimage/_interpolation.py) and by
+    probing its zoom_shift:
+    - zoom = (n_in - 1) / (n_out - 1) in float64, and 1 where n_out - 1 == 0 (numpy.divide(..., where=zoom_div != 0)):
+      a 1-sample output reads input 0, a 1-sample input is read at 0 by every output;
+    - output index k samples the input at cc = k * zoom (grid_mode=False, no shift);
+    - mode='constant': cc > n_in - 1 is outside the input, and the whole output row / column is cval.  The last
+      index can land an ulp above n_in - 1 (28 -> 27 samples: 27 * (27 / 26) = 27.000000000000004), so some
+      sizes get a black last row or column;
+    - i0 = floor(cc), x = cc - i0, w0 = 1 - x and w1 = 1 - w0 (not x: the weights are completed to sum to 1).  At
+      cc = n_in - 1, w1 = 0 and scipy reads a mirrored index; i1 is clamped to n_in - 1 here, which gives the same
+      zero term."""
+    n_in, n_out = int(n_in), int(n_out)
+    if n_in < 1 or n_out < 1:
+        raise RuntimeError(f'zoom from {n_in} to {n_out} samples: sizes must be at least 1')
+    zoom = (n_in - 1) / (n_out - 1) if n_out != 1 else 1.0
+    cc = np.arange(n_out, dtype=np.float64) * zoom
+    outside = cc > n_in - 1
+    i0 = np.floor(cc)
+    w0 = 1.0 - (cc - i0)
+    taps = np.zeros((n_out,), dtype=ZOOM_TAP)
+    taps['w0'] = w0
+    taps['w1'] = 1.0 - w0
+    taps['i0'] = np.where(outside, -1, i0)
+    taps['i1'] = np.where(outside, -1, np.minimum(i0 + 1, n_in - 1))
+    return taps
+
+
+def zoom_linear_reference(image, target_w, target_h):
+    """numpy restatement of scipy.ndimage.zoom(image, (target_h / h, target_w / w, 1), order=1) on a uint8 [h, w, 3]
+    image (transforms/scale.py:60-67), from `scipy_zoom_tables`; the GPU kernel k_zoom_linear does the same.
+    - The channel axis zooms 3 -> 3 by exactly 1: its weights are exactly 1 and 0, so each of the four (y, x) terms
+      is (v * wy) * wx (scipy multiplies the weights onto the value axis by axis), and its zero-weight terms add
+      +0.0.  The terms are summed from 0.0 in scipy's filter order: (y0, x0), (y0, x1), (y1, x0), (y1, x1).
+    - A sample with a row or column outside the input is cval = 0.
+    - uint8 conversion: t > 0 ? t + 0.5 : 0, clamped to 255, truncated -- ties round up, unlike numpy.round, and
+      the float64 sum decides which side of a .5 a sample lands on.
+    - scipy returns the input unchanged when both factors are 1; the tables then give exactly that."""
+    img = np.asarray(image, dtype=np.uint8)
+    h, w = img.shape[:2]
+    ty, tx = scipy_zoom_tables(h, target_h), scipy_zoom_tables(w, target_w)
+    v = img.astype(np.float64)
+    wy0, wy1 = ty['w0'][:, None, None], ty['w1'][:, None, None]
+    wx0, wx1 = tx['w0'][None, :, None], tx['w1'][None, :, None]
+    y0, y1 = np.maximum(ty['i0'], 0), np.maximum(ty['i1'], 0)
+    x0, x1 = np.maximum(tx['i0'], 0), np.maximum(tx['i1'], 0)
+    t = 0.0 + (v[y0][:, x0] * wy0) * wx0
+    t = t + (v[y0][:, x1] * wy0) * wx1
+    t = t + (v[y1][:, x0] * wy1) * wx0
+    t = t + (v[y1][:, x1] * wy1) * wx1
+    t = np.where((ty['i0'] < 0)[:, None, None] | (tx['i0'] < 0)[None, :, None], 0.0, t)
+    t = np.minimum(np.where(t > 0, t + 0.5, 0.0), 255.0)
+    return t.astype(np.uint8)
 
 
 def rescale_target(w, h, long_edge):
@@ -158,16 +222,31 @@ def resize_path(w, h, target_w, target_h, dst_pitch_bytes):
 class GpuPreprocess:
     """:param long_edge: RescaleAbsolute target (None: no rescale, like --long-edge unset)
     :param batched: True -> CenterPad(long_edge) squares (predictor.py:91-93, batch size > 1);
-                    False -> CenterPadTight(16) (predictor.py:94-95)"""
+                    False -> CenterPadTight(16) (predictor.py:94-95)
+    :param fast_rescaling: the reference's Predictor.fast_rescaling / RescaleAbsolute(fast=...): True resizes like
+                    PIL.Image.resize (pifpaf_image_resize_bilinear_u8); False like scipy.ndimage.zoom(order=1), the
+                    precise rescale of --precise-rescaling and of every evaluation preprocess
+                    (pifpaf_image_zoom_linear_u8, the whole batch in one launch)
+    :param resample: RescaleAbsolute's resample; only BILINEAR (2, its default) is built"""
 
-    def __init__(self, long_edge=None, batched=True, *, device=0, multiple=16):
+    def __init__(self, long_edge=None, batched=True, *, fast_rescaling=True, resample=BILINEAR, device=0, multiple=16):
         if batched and not long_edge:
             raise RuntimeError('--long-edge must be provided for batch size > 1')      # predictor.py:92
+        if resample != BILINEAR:
+            raise RuntimeError(f'resample={resample!r} is not built: only BILINEAR ({BILINEAR}; scipy order 1) is')
         self.long_edge = int(long_edge) if long_edge else None
         self.batched = bool(batched)
+        self.fast_rescaling = bool(fast_rescaling)
         self.multiple = int(multiple)
         self.device = torch.device('cuda', device)
         self._coeff_cache = {}
+        self._zoom_cache = {}
+
+    def _zoom_taps(self, n_in, n_out):
+        key = (n_in, n_out)
+        if key not in self._zoom_cache:
+            self._zoom_cache[key] = scipy_zoom_tables(n_in, n_out)
+        return self._zoom_cache[key]
 
     def _coeffs(self, n_in, n_out):
         key = (n_in, n_out)
@@ -208,6 +287,8 @@ class GpuPreprocess:
         st = stream if stream is not None else torch.cuda.current_stream(self.device)
         if any(im.is_cuda for im in imgs):
             st.wait_stream(torch.cuda.current_stream(self.device))     # CUDA inputs (and .contiguous()) are written there
+        if not self.fast_rescaling:
+            return self._zoom(imgs, sizes, plans, (cw, ch), fill, st)
         L = _lib.lib()
         sp = ctypes.c_void_p(st.cuda_stream)
         with torch.cuda.stream(st):
@@ -232,6 +313,43 @@ class GpuPreprocess:
                 keep.append((src, tmp))
                 metas.append(reference_meta(w, h, tw, th, np.asarray(ltrb), rescaled=self.long_edge is not None))
             self._keepalive = keep
+        return canvas, metas
+
+    def _zoom(self, imgs, sizes, plans, canvas_size, fill, st):
+        """the fast_rescaling=False path of __call__: every image's taps (one table per distinct (in, out) pair) and
+        descriptor staged, and the whole canvas written, by one pifpaf_image_zoom_linear_u8"""
+        cw, ch = canvas_size
+        B = len(imgs)
+        tables, offsets, n_taps = [], {}, 0
+
+        def tap_offset(n_in, n_out):
+            nonlocal n_taps
+            if (n_in, n_out) not in offsets:
+                offsets[(n_in, n_out)] = n_taps
+                tables.append(self._zoom_taps(n_in, n_out))
+                n_taps += n_out
+            return offsets[(n_in, n_out)]
+
+        descs = (_lib.ZoomImage * B)()
+        metas, srcs = [], []
+        with torch.cuda.stream(st):
+            canvas = torch.empty((B, ch, cw, 3), dtype=torch.uint8, device=self.device)
+            for d, im, (w, h), (tw, th, ltrb, _), f in zip(descs, imgs, sizes, plans, fill):
+                src = im.pin_memory().to(self.device, non_blocking=True) if not im.is_cuda else im
+                srcs.append(src)
+                d.src, d.h, d.w, d.th, d.tw, d.left, d.top = src.data_ptr(), h, w, th, tw, ltrb[0], ltrb[1]
+                d.ytab, d.xtab = tap_offset(h, th), tap_offset(w, tw)
+                if not all(0 <= c <= 255 for c in f):
+                    raise RuntimeError(f'fill colour out of range: {f}')
+                d.fill[:3] = f
+                metas.append(reference_meta(w, h, tw, th, np.asarray(ltrb), rescaled=self.long_edge is not None))
+            taps = np.ascontiguousarray(np.concatenate(tables))
+            ws_bytes = ctypes.sizeof(descs) + taps.nbytes
+            workspace = torch.empty((ws_bytes,), dtype=torch.uint8, device=self.device)
+            _lib.check(_lib.lib().pifpaf_image_zoom_linear_u8(
+                descs, B, taps.ctypes.data, taps.size, workspace.data_ptr(), ws_bytes, canvas.data_ptr(), ch, cw,
+                ctypes.c_void_p(st.cuda_stream)))
+            self._keepalive = (srcs, workspace)
         return canvas, metas
 
 
