@@ -261,6 +261,37 @@ int pifpaf_image_zoom_linear_u8(const pifpaf_zoom_image_t* images, int32_t n_ima
                                 void* workspace_dev, int64_t workspace_bytes,
                                 uint8_t* canvas_dev, int32_t canvas_h, int32_t canvas_w, void* stream);
 
+/* The reference's fast rescale where OpenCV is importable: transforms.RescaleAbsolute(fast=True) (Predictor's
+ * default) -> cv2.resize(im, (tw, th), interpolation=INTER_LINEAR) (transforms/scale.py:41-55), then CenterPad /
+ * CenterPadTight.  A whole batch in one launch, laid out as pifpaf_image_zoom_linear_u8: one thread per canvas pixel
+ * writes the pad colour outside the image's window and, inside, OpenCV's fixed-point bilinear value: per channel the
+ * horizontal products H = v[i0] * c0 + v[i1] * c1 of the two source rows, then
+ * ((((H0 >> 4) * c0y) >> 16) + (((H1 >> 4) * c1y) >> 16) + 2) >> 2 saturated to uint8 (integer arithmetic only;
+ * openpifpaf_b200/preprocess.py, opencv_linear_tables / opencv_linear_reference, states the rules).  A tap holds
+ * the two source indices of one output row or column and their 11-bit coefficients.
+ *   images / taps: HOST arrays; they are checked here (sizes >= 1, pitch >= 3 * w, the window inside the canvas,
+ *   each table within taps, its indices within the source, coefficients >= 0 summing to at most 2048) and staged
+ *   into workspace_dev, which holds at least n_images * sizeof(pifpaf_cv_image_t) + n_taps * sizeof(pifpaf_cv_tap_t)
+ *   bytes.  src: device rows of 3 * w bytes, pitch bytes apart.
+ *   A refused call (PIFPAF_E_BADARG) stages and writes nothing. */
+typedef struct {
+    int32_t i0, i1;         /* source indices, within [0, n_in) */
+    int16_t c0, c1;         /* their coefficients, 2048 = 1 */
+} pifpaf_cv_tap_t;
+typedef struct {
+    const uint8_t* src;     /* device, row y at src + y * pitch */
+    int64_t pitch;          /* source row pitch in bytes */
+    int32_t h, w;           /* source size */
+    int32_t th, tw;         /* target size */
+    int32_t left, top;      /* window offset in the canvas */
+    int32_t ytab, xtab;     /* first tap of the row table (th taps) and the column table (tw taps) */
+    uint8_t fill[4];        /* pad colour r, g, b; fill[3] is unused */
+} pifpaf_cv_image_t;
+int pifpaf_image_resize_linear_cv_u8(const pifpaf_cv_image_t* images, int32_t n_images,
+                                     const pifpaf_cv_tap_t* taps, int64_t n_taps,
+                                     void* workspace_dev, int64_t workspace_bytes,
+                                     uint8_t* canvas_dev, int32_t canvas_h, int32_t canvas_w, void* stream);
+
 
 /* ------------------------------------------------------------------------ */
 /* Baseline JPEG decode, bit-identical to PIL.Image.open(f).convert('RGB') (datasets/image_list.py:18; Pillow's

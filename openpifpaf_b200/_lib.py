@@ -47,6 +47,12 @@ class ZoomImage(ctypes.Structure):
                 ('top', c_i32), ('ytab', c_i32), ('xtab', c_i32), ('fill', ctypes.c_uint8 * 4)]
 
 
+class CvImage(ctypes.Structure):
+    """pifpaf_cv_image_t"""
+    _fields_ = [('src', VP), ('pitch', c_i64), ('h', c_i32), ('w', c_i32), ('th', c_i32), ('tw', c_i32),
+                ('left', c_i32), ('top', c_i32), ('ytab', c_i32), ('xtab', c_i32), ('fill', ctypes.c_uint8 * 4)]
+
+
 # every symbol include/pifpaf_b200.h declares: name -> (restype, argtypes)
 SYMBOLS = {
     'pifpaf_last_error': (ctypes.c_char_p, []),
@@ -80,6 +86,7 @@ SYMBOLS = {
                                                         VP, VP, c_i32, VP, VP]),
     'pifpaf_image_fill_rgb': (ctypes.c_int, [VP, c_i64, c_i32, c_i32, c_i32, VP]),
     'pifpaf_image_zoom_linear_u8': (ctypes.c_int, [VP, c_i32, VP, c_i64, VP, c_i64, VP, c_i32, c_i32, VP]),
+    'pifpaf_image_resize_linear_cv_u8': (ctypes.c_int, [VP, c_i32, VP, c_i64, VP, c_i64, VP, c_i32, c_i32, VP]),
     'pifpaf_jpeg_create': (ctypes.c_int, [P(VP), c_i32, c_i32, c_i64, c_i64, c_i64]),
     'pifpaf_jpeg_destroy': (None, [VP]),
     'pifpaf_jpeg_decode': (ctypes.c_int, [VP, c_i32, P(VP), P(c_i64), VP, c_i64, c_i32, P(c_i32), P(c_i32), P(c_i64),

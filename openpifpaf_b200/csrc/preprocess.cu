@@ -3,6 +3,8 @@
 // Replaces, for the inference path of the reference's Predictor (predictor.py:85-102):
 //   transforms.RescaleAbsolute(long_edge, fast=True)   transforms/scale.py:154-176 -> PIL.Image.resize(BILINEAR)
 //   transforms.RescaleAbsolute(long_edge, fast=False)  transforms/scale.py:60-67 -> scipy.ndimage.zoom(order=1)
+//   transforms.RescaleAbsolute(long_edge, fast=True)   transforms/scale.py:41-55 -> cv2.resize(INTER_LINEAR) when
+//                                                      OpenCV is importable
 //   transforms.CenterPad / CenterPadTight              transforms/pad.py:15-110
 // ToTensor + Normalize (transforms/__init__.py:26-33) already run inside the stem kernel (pifpaf_net_forward_u8).
 //
@@ -20,6 +22,13 @@
 // the four (y, x) terms is (v * wy) * wx, and the channel's zero-weight terms add +0.0, which changes nothing.  The
 // sum runs in scipy's order from 0.0, and the uint8 store is scipy's: t > 0 ? t + 0.5 : 0, clamped to 255,
 // truncated.  This file is built with FMA contraction on, so the arithmetic is written with __dmul_rn / __dadd_rn.
+//
+// The fast rescale where OpenCV is importable, cv2.resize(INTER_LINEAR) (transforms/scale.py:41-55), is
+// k_resize_linear_cv, laid out like k_zoom_linear.  OpenCV resizes separably in fixed point (resize.cpp:
+// resizeGeneric_, HResizeLinear into int32 rows, VResizeLinearVec_32s8u down to uint8); two taps per axis, so each
+// thread recomputes the horizontal products of its two source rows in registers.  Integer arithmetic only, with
+// OpenCV's int16 SIMD lanes restated in int32: the host refuses coefficients that would not fit them.  The per-axis
+// taps come from the host restatement (preprocess.opencv_linear_tables), which states the coordinate rules.
 #include <algorithm>
 #include <cstdint>
 
@@ -132,6 +141,37 @@ __global__ void __launch_bounds__(256) k_zoom_linear(const pifpaf_zoom_image_t* 
     }
 }
 
+// canvas [n][ch][cw][3]: one thread per pixel, each image's window at (left, top) is cv2.resize(INTER_LINEAR) of
+// its source, everything else its pad colour
+__global__ void __launch_bounds__(256) k_resize_linear_cv(const pifpaf_cv_image_t* __restrict__ images,
+                                                          const pifpaf_cv_tap_t* __restrict__ taps,
+                                                          uint8_t* __restrict__ canvas, int ch, int cw, long long total) {
+    const long long plane = (long long)ch * cw;
+    for (long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x; t < total; t += (long long)gridDim.x * blockDim.x) {
+        const int b = (int)(t / plane);
+        const int p = (int)(t - (long long)b * plane);
+        const pifpaf_cv_image_t& im = images[b];
+        const int yy = p / cw - im.top, xx = p % cw - im.left;
+        uint8_t* o = canvas + 3 * t;
+        if (yy < 0 || yy >= im.th || xx < 0 || xx >= im.tw) {
+            o[0] = im.fill[0]; o[1] = im.fill[1]; o[2] = im.fill[2];
+            continue;
+        }
+        const pifpaf_cv_tap_t ty = taps[im.ytab + yy], tx = taps[im.xtab + xx];
+        const uint8_t* r0 = im.src + ty.i0 * im.pitch;
+        const uint8_t* r1 = im.src + ty.i1 * im.pitch;
+        const int c0 = 3 * tx.i0, c1 = 3 * tx.i1;
+#pragma unroll
+        for (int c = 0; c < 3; c++) {
+            // HResizeLinear: exact int32 sums; VResizeLinearVec_32s8u: >> 4 into int16, mulhi, add, (+ 2) >> 2
+            const int h0 = (int)r0[c0 + c] * tx.c0 + (int)r0[c1 + c] * tx.c1;
+            const int h1 = (int)r1[c0 + c] * tx.c0 + (int)r1[c1 + c] * tx.c1;
+            const int v = ((((h0 >> 4) * ty.c0) >> 16) + (((h1 >> 4) * ty.c1) >> 16) + 2) >> 2;
+            o[c] = (uint8_t)(v > 255 ? 255 : v);
+        }
+    }
+}
+
 inline int grid_for(long long total) { return (int)std::min<long long>((total + 255) / 256, 132LL * 16); }
 
 // the taps of one axis of one image lie within the staged table and index its source
@@ -141,6 +181,18 @@ bool taps_ok(const pifpaf_zoom_tap_t* taps, int64_t n_taps, int64_t first, int32
         const pifpaf_zoom_tap_t& tp = taps[first + k];
         if (tp.i0 == -1) continue;
         if (tp.i0 < 0 || tp.i0 >= n_in || tp.i1 < 0 || tp.i1 >= n_in) return false;
+    }
+    return true;
+}
+
+// the taps of one axis of one image lie within the staged table, index its source, and keep OpenCV's int16 lanes
+// from saturating: coefficients >= 0 summing to at most 2048, so (H >> 4) <= 255 * 2048 >> 4 < 2^15
+bool cv_taps_ok(const pifpaf_cv_tap_t* taps, int64_t n_taps, int64_t first, int32_t n_out, int32_t n_in) {
+    if (first < 0 || first + n_out > n_taps) return false;
+    for (int32_t k = 0; k < n_out; k++) {
+        const pifpaf_cv_tap_t& tp = taps[first + k];
+        if (tp.i0 < 0 || tp.i0 >= n_in || tp.i1 < 0 || tp.i1 >= n_in) return false;
+        if (tp.c0 < 0 || tp.c1 < 0 || tp.c0 + tp.c1 > 2048) return false;
     }
     return true;
 }
@@ -227,6 +279,41 @@ int pifpaf_image_zoom_linear_u8(const pifpaf_zoom_image_t* images, int32_t n_ima
     k_zoom_linear<<<grid_for(total), 256, 0, st>>>(reinterpret_cast<const pifpaf_zoom_image_t*>(ws),
                                                    reinterpret_cast<const pifpaf_zoom_tap_t*>(ws + desc_bytes),
                                                    canvas_dev, canvas_h, canvas_w, total);
+    PIFPAF_LAUNCH_CHECK();
+    return PIFPAF_OK;
+}
+
+int pifpaf_image_resize_linear_cv_u8(const pifpaf_cv_image_t* images, int32_t n_images,
+                                     const pifpaf_cv_tap_t* taps, int64_t n_taps,
+                                     void* workspace_dev, int64_t workspace_bytes,
+                                     uint8_t* canvas_dev, int32_t canvas_h, int32_t canvas_w, void* stream_v) {
+    PIFPAF_CHECK_ARG(images != nullptr && n_images >= 1, "no images");
+    PIFPAF_CHECK_ARG(taps != nullptr && n_taps >= 1, "tap tables missing");
+    PIFPAF_CHECK_ARG(canvas_dev != nullptr && workspace_dev != nullptr, "canvas or workspace pointer is null");
+    PIFPAF_CHECK_ARG(canvas_h >= 1 && canvas_w >= 1, "bad canvas size");
+    const size_t desc_bytes = sizeof(pifpaf_cv_image_t) * (size_t)n_images;
+    const size_t tap_bytes = sizeof(pifpaf_cv_tap_t) * (size_t)n_taps;
+    PIFPAF_CHECK_ARG(workspace_bytes >= 0 && (size_t)workspace_bytes >= desc_bytes + tap_bytes, "workspace too small");
+    for (int32_t i = 0; i < n_images; i++) {
+        const pifpaf_cv_image_t& im = images[i];
+        PIFPAF_CHECK_ARG(im.src != nullptr, "image pointer is null");
+        PIFPAF_CHECK_ARG(im.h >= 1 && im.w >= 1 && im.th >= 1 && im.tw >= 1, "bad image size");
+        PIFPAF_CHECK_ARG(im.pitch >= 3 * (int64_t)im.w, "source pitch too small");
+        PIFPAF_CHECK_ARG(im.left >= 0 && im.top >= 0 && (int64_t)im.left + im.tw <= canvas_w
+                         && (int64_t)im.top + im.th <= canvas_h, "window outside the canvas");
+        PIFPAF_CHECK_ARG(cv_taps_ok(taps, n_taps, im.ytab, im.th, im.h), "row taps missing, outside the source or "
+                         "with coefficients outside [0, 2048]");
+        PIFPAF_CHECK_ARG(cv_taps_ok(taps, n_taps, im.xtab, im.tw, im.w), "column taps missing, outside the source or "
+                         "with coefficients outside [0, 2048]");
+    }
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_v);
+    auto* ws = static_cast<uint8_t*>(workspace_dev);
+    PIFPAF_CUDA_TRY(cudaMemcpyAsync(ws, images, desc_bytes, cudaMemcpyHostToDevice, st));
+    PIFPAF_CUDA_TRY(cudaMemcpyAsync(ws + desc_bytes, taps, tap_bytes, cudaMemcpyHostToDevice, st));
+    const long long total = (long long)n_images * canvas_h * canvas_w;
+    k_resize_linear_cv<<<grid_for(total), 256, 0, st>>>(reinterpret_cast<const pifpaf_cv_image_t*>(ws),
+                                                        reinterpret_cast<const pifpaf_cv_tap_t*>(ws + desc_bytes),
+                                                        canvas_dev, canvas_h, canvas_w, total);
     PIFPAF_LAUNCH_CHECK();
     return PIFPAF_OK;
 }

@@ -158,7 +158,8 @@ class Predictor:
         self.last_nn_time = self.last_decoder_time = time.perf_counter() - t0
         return result
 
-    def raw_images(self, images, *, json_data=False, fill=None, score_weights=None, fast_rescaling=True):
+    def raw_images(self, images, *, json_data=False, fill=None, score_weights=None, fast_rescaling=True,
+                   opencv_rescaling=False):
         """The reference's Predictor.numpy_images / images (predictor.py:155-196) for a list of RAW uint8 [h, w, 3]
         images with everything after the JPEG decode on the GPU: RescaleAbsolute(long edge = the compiled input size)
         + CenterPad (`preprocess.GpuPreprocess`, bit-identical to the reference's Pillow path), ToTensor + Normalize in
@@ -166,17 +167,20 @@ class Predictor:
         image at once.  fill: the pad colour as for `GpuPreprocess` (a list has one colour per image of `images`).
         fast_rescaling: the reference's Predictor.fast_rescaling; False (its --precise-rescaling) rescales like
         scipy.ndimage.zoom(order=1) instead of Pillow (`GpuPreprocess(fast_rescaling=False)`).
+        opencv_rescaling: True rescales like cv2.resize(INTER_LINEAR), which the reference's fast rescale uses when
+        OpenCV is importable (`GpuPreprocess(opencv=True)`); with fast_rescaling=False scipy is used either way, as in
+        the reference.
         Returns per image (data [N, K, 3] (x, y, v) in original-image pixels, joint_scales [N, K], meta) or, with
         json_data, (list of dicts, meta)."""
         if self.net.in_h != self.net.in_w:
             raise RuntimeError('raw_images needs a net compiled for a square input (CenterPad(long_edge))')
         if getattr(self, '_gpu_preprocess', None) is None:
             self._gpu_preprocess = {}
-        fast_rescaling = bool(fast_rescaling)
-        if fast_rescaling not in self._gpu_preprocess:
-            self._gpu_preprocess[fast_rescaling] = _preprocess.GpuPreprocess(
-                self.net.in_w, batched=True, fast_rescaling=fast_rescaling, device=self.device.index)
-        preprocess = self._gpu_preprocess[fast_rescaling]
+        key = (bool(fast_rescaling), bool(fast_rescaling) and bool(opencv_rescaling))
+        if key not in self._gpu_preprocess:
+            self._gpu_preprocess[key] = _preprocess.GpuPreprocess(
+                self.net.in_w, batched=True, fast_rescaling=key[0], opencv=key[1], device=self.device.index)
+        preprocess = self._gpu_preprocess[key]
         out = []
         for chunk, chunk_fill in raw_image_chunks(images, self.net.max_batch, fill):
             with torch.cuda.stream(self.stream):
@@ -192,12 +196,13 @@ class Predictor:
                     out.append((data, scales, meta))
         return out
 
-    def jpeg_images(self, files_or_bytes, *, json_data=False, fill=None, score_weights=None, fast_rescaling=True):
+    def jpeg_images(self, files_or_bytes, *, json_data=False, fill=None, score_weights=None, fast_rescaling=True,
+                    opencv_rescaling=False):
         """`raw_images` of the JPEG files (paths or bytes) decoded like the reference's Predictor.images
         (PIL.Image.open(f).convert('RGB'), datasets/image_list.py:18), but on the GPU (`preprocess.GpuJpegDecoder`;
         streams it does not decode are decoded by Pillow).  Chunked by max_batch; each chunk's decode is enqueued on
-        the predictor's stream ahead of its resize (fast_rescaling as for raw_images).  Returns what raw_images
-        returns, per file."""
+        the predictor's stream ahead of its resize (fast_rescaling and opencv_rescaling as for raw_images).  Returns
+        what raw_images returns, per file."""
         files = list(files_or_bytes)
         if isinstance(fill, list) and len(fill) != len(files):
             raise RuntimeError(f'fill has {len(fill)} colours for {len(files)} images')
@@ -207,7 +212,7 @@ class Predictor:
             dec = self._jpeg_decoder(datas)
             images, _ = dec(datas, stream=self.stream, host_pillow=True)
             out.extend(self.raw_images(images, json_data=json_data, fill=chunk_fill, score_weights=score_weights,
-                                       fast_rescaling=fast_rescaling))
+                                       fast_rescaling=fast_rescaling, opencv_rescaling=opencv_rescaling))
         return out
 
     def _jpeg_decoder(self, datas):

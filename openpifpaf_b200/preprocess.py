@@ -5,6 +5,8 @@ Reference (paths relative to the reference's src/openpifpaf/):
                                                              CenterPadTight(16), EVAL_TRANSFORM
   transforms.RescaleAbsolute / _scale  transforms/scale.py:28-100,154-176   (fast=True, OpenCV absent:
                                                              PIL.Image.resize((w, h), BILINEAR), scale.py:56-59;
+                                                             fast=True, OpenCV importable: cv2.resize(INTER_LINEAR),
+                                                             scale.py:41-55;
                                                              fast=False: scipy.ndimage.zoom(order=1), scale.py:60-67)
   transforms.CenterPad / CenterPadTight  transforms/pad.py:15-110
   Annotation.inverse_transform / json_data / score / bbox   annotation.py:96-214
@@ -13,8 +15,11 @@ Reference (paths relative to the reference's src/openpifpaf/):
 (pifpaf_image_resize_bilinear_u8; Pillow's ImagingResample restated, this module builds its coefficient tables) straight
 into the centre of a padded uint8 canvas -- or, with fast_rescaling=False (RescaleAbsolute(fast=False),
 transforms/scale.py:60-67), bit-identically to scipy.ndimage.zoom(order=1) (pifpaf_image_zoom_linear_u8, the whole
-batch in one launch; `scipy_zoom_tables` / `zoom_linear_reference` restate scipy) -- and returns the canvas -- the input of `CompiledNet.forward_uint8`, whose stem
-applies ToTensor + Normalize -- together with the per-image `meta` dicts the reference's transforms would have produced.
+batch in one launch; `scipy_zoom_tables` / `zoom_linear_reference` restate scipy) -- or, with opencv=True,
+bit-identically to cv2.resize(INTER_LINEAR) (pifpaf_image_resize_linear_cv_u8, one launch as well;
+`opencv_linear_tables` / `opencv_linear_reference` restate OpenCV) -- and returns the canvas -- the input of
+`CompiledNet.forward_uint8`, whose stem applies ToTensor + Normalize -- together with the per-image `meta` dicts the
+reference's transforms would have produced.
 `GpuJpegDecoder` decodes baseline JPEG files on the GPU bit-identically to PIL.Image.open(f).convert('RGB')
 (datasets/image_list.py:18), the step before them; streams the GPU does not decode are decoded by Pillow.
 `inverse_transform_batch` / `json_data_batch` are the array forms of `Annotation.inverse_transform` / `json_data` for all
@@ -147,6 +152,68 @@ def zoom_linear_reference(image, target_w, target_h):
     return t.astype(np.uint8)
 
 
+CV_TAP = np.dtype([('i0', '<i4'), ('i1', '<i4'), ('c0', '<i2'), ('c1', '<i2')])     # pifpaf_cv_tap_t
+CV_COEF_ONE = 1 << 11                # INTER_RESIZE_COEF_SCALE, modules/imgproc/src/resize.cpp
+
+
+def opencv_linear_tables(n_in, n_out, horizontal=True):
+    """One axis of cv2.resize(..., interpolation=INTER_LINEAR) on uint8 from n_in to n_out samples
+    (modules/imgproc/src/resize.cpp: cv::resize -> resizeGeneric_ with HResizeLinear / VResizeLinear): per output
+    index a pifpaf_cv_tap_t (`CV_TAP`) -- the two source indices i0 / i1 and their 11-bit coefficients c0 / c1.
+    - scale = 1 / (n_out / n_in) in double; f = (float)((k + 0.5) * scale - 0.5); s = floor(f); f -= s in float.
+    - c0 = saturate_cast<short>((1.f - f) * 2048), c1 = saturate_cast<short>(f * 2048): float products rounded to
+      nearest, ties to even.
+    - Border clamp, columns (horizontal=True): where s < 0 or s >= n_in - 1 OpenCV sets f = 0 and s to the border
+      column, so the tap is (border, 2048) and (border, 0).
+    - Rows (horizontal=False) keep f: s and s + 1 are clipped into [0, n_in - 1] and both coefficients stay, so a
+      border row of an upscale reads the edge row twice with fractional weights.  The vertical pass truncates each
+      product on its own (`opencv_linear_reference`), so this is not the same as weights (2048, 0): it is the border
+      rule that makes the first and last rows of upscales differ by 1 from a clamped restatement.
+    c0 + c1 = 2048 in every tap."""
+    n_in, n_out = int(n_in), int(n_out)
+    if n_in < 1 or n_out < 1:
+        raise RuntimeError(f'resize from {n_in} to {n_out} samples: sizes must be at least 1')
+    scale = 1.0 / (n_out / n_in)
+    f = ((np.arange(n_out, dtype=np.float64) + 0.5) * scale - 0.5).astype(np.float32)
+    s = np.floor(f)
+    f = f - s
+    s = s.astype(np.int64)
+    if horizontal:
+        border = (s < 0) | (s >= n_in - 1)
+        f = np.where(border, np.float32(0), f)
+        s = np.clip(s, 0, n_in - 1)
+    one = np.float32(CV_COEF_ONE)
+    taps = np.zeros((n_out,), dtype=CV_TAP)
+    taps['i0'] = np.clip(s, 0, n_in - 1)
+    taps['i1'] = np.clip(s + 1, 0, n_in - 1)
+    taps['c0'] = np.clip(np.rint((np.float32(1) - f) * one), -32768, 32767)
+    taps['c1'] = np.clip(np.rint(f * one), -32768, 32767)
+    return taps
+
+
+def opencv_linear_reference(image, target_w, target_h):
+    """numpy restatement of cv2.resize(image, (target_w, target_h), interpolation=cv2.INTER_LINEAR) on a uint8
+    [h, w, 3] image (transforms/scale.py:41-55, RescaleAbsolute(fast=True) when OpenCV is importable), from
+    `opencv_linear_tables`; the GPU kernel k_resize_linear_cv does the same integer arithmetic.
+    - Horizontal pass, exact in int32: H = v[i0] * c0 + v[i1] * c1 per source row and channel.
+    - Vertical pass, as OpenCV's SIMD VResizeLinearVec_32s8u computes it on every element (also the last ones of a
+      row, and 1-pixel images): each row's H is shifted right by 4 into int16, multiplied by its coefficient keeping
+      the high 16 bits, the two products added, then (t + 2) >> 2 saturated to uint8.  Not the textbook rounding
+      (H0 * c0 + H1 * c1 + 2^21) >> 22: each product is truncated on its own.
+    - Exactly 2x down on both axes OpenCV switches INTER_LINEAR to INTER_AREA's fast path, (a + b + c + d + 2) >> 2.
+      The linear taps are then (i, 1024) and (i + 1, 1024) on both axes and the vertical pass gives the same sum, so
+      no pixel changes and no separate rule is needed.
+    - An unchanged size is a copy; the taps are then (k, 2048) and give exactly that."""
+    img = np.asarray(image, dtype=np.uint8)
+    h, w = img.shape[:2]
+    tx, ty = opencv_linear_tables(w, target_w, True), opencv_linear_tables(h, target_h, False)
+    v = img.astype(np.int64)
+    hp = v[:, tx['i0']] * tx['c0'][None, :, None] + v[:, tx['i1']] * tx['c1'][None, :, None]
+    c0y, c1y = ty['c0'][:, None, None], ty['c1'][:, None, None]
+    t = (((hp[ty['i0']] >> 4) * c0y) >> 16) + (((hp[ty['i1']] >> 4) * c1y) >> 16)
+    return np.clip((t + 2) >> 2, 0, 255).astype(np.uint8)
+
+
 def rescale_target(w, h, long_edge):
     """RescaleAbsolute.__call__ (transforms/scale.py:163-176)"""
     s = long_edge / max(h, w)
@@ -227,9 +294,13 @@ class GpuPreprocess:
                     PIL.Image.resize (pifpaf_image_resize_bilinear_u8); False like scipy.ndimage.zoom(order=1), the
                     precise rescale of --precise-rescaling and of every evaluation preprocess
                     (pifpaf_image_zoom_linear_u8, the whole batch in one launch)
+    :param opencv: with fast_rescaling, resize like cv2.resize(INTER_LINEAR) instead of Pillow -- what
+                    RescaleAbsolute(fast=True) does when OpenCV is importable (pifpaf_image_resize_linear_cv_u8, the
+                    whole batch in one launch).  Without fast_rescaling scipy is used either way, as in the reference
     :param resample: RescaleAbsolute's resample; only BILINEAR (2, its default) is built"""
 
-    def __init__(self, long_edge=None, batched=True, *, fast_rescaling=True, resample=BILINEAR, device=0, multiple=16):
+    def __init__(self, long_edge=None, batched=True, *, fast_rescaling=True, opencv=False, resample=BILINEAR, device=0,
+                 multiple=16):
         if batched and not long_edge:
             raise RuntimeError('--long-edge must be provided for batch size > 1')      # predictor.py:92
         if resample != BILINEAR:
@@ -237,16 +308,19 @@ class GpuPreprocess:
         self.long_edge = int(long_edge) if long_edge else None
         self.batched = bool(batched)
         self.fast_rescaling = bool(fast_rescaling)
+        self.opencv = bool(opencv) and self.fast_rescaling
         self.multiple = int(multiple)
         self.device = torch.device('cuda', device)
         self._coeff_cache = {}
-        self._zoom_cache = {}
+        self._tap_cache = {}
 
-    def _zoom_taps(self, n_in, n_out):
-        key = (n_in, n_out)
-        if key not in self._zoom_cache:
-            self._zoom_cache[key] = scipy_zoom_tables(n_in, n_out)
-        return self._zoom_cache[key]
+    def _taps(self, n_in, n_out, horizontal):
+        """one axis's taps for the one-launch paths: scipy's (the same for both axes) or OpenCV's"""
+        key = (n_in, n_out, horizontal and self.opencv)
+        if key not in self._tap_cache:
+            self._tap_cache[key] = (opencv_linear_tables(n_in, n_out, horizontal) if self.opencv
+                                    else scipy_zoom_tables(n_in, n_out))
+        return self._tap_cache[key]
 
     def _coeffs(self, n_in, n_out):
         key = (n_in, n_out)
@@ -287,8 +361,8 @@ class GpuPreprocess:
         st = stream if stream is not None else torch.cuda.current_stream(self.device)
         if any(im.is_cuda for im in imgs):
             st.wait_stream(torch.cuda.current_stream(self.device))     # CUDA inputs (and .contiguous()) are written there
-        if not self.fast_rescaling:
-            return self._zoom(imgs, sizes, plans, (cw, ch), fill, st)
+        if self.opencv or not self.fast_rescaling:
+            return self._one_launch(imgs, sizes, plans, (cw, ch), fill, st)
         L = _lib.lib()
         sp = ctypes.c_void_p(st.cuda_stream)
         with torch.cuda.stream(st):
@@ -315,22 +389,25 @@ class GpuPreprocess:
             self._keepalive = keep
         return canvas, metas
 
-    def _zoom(self, imgs, sizes, plans, canvas_size, fill, st):
-        """the fast_rescaling=False path of __call__: every image's taps (one table per distinct (in, out) pair) and
-        descriptor staged, and the whole canvas written, by one pifpaf_image_zoom_linear_u8"""
+    def _one_launch(self, imgs, sizes, plans, canvas_size, fill, st):
+        """the scipy (fast_rescaling=False) and OpenCV paths of __call__: every image's taps (one table per distinct
+        (in, out) pair and, for OpenCV, axis) and descriptor staged, and the whole canvas written, by one
+        pifpaf_image_zoom_linear_u8 / pifpaf_image_resize_linear_cv_u8"""
         cw, ch = canvas_size
         B = len(imgs)
         tables, offsets, n_taps = [], {}, 0
 
-        def tap_offset(n_in, n_out):
+        def tap_offset(n_in, n_out, horizontal):
             nonlocal n_taps
-            if (n_in, n_out) not in offsets:
-                offsets[(n_in, n_out)] = n_taps
-                tables.append(self._zoom_taps(n_in, n_out))
+            key = (n_in, n_out, horizontal and self.opencv)
+            if key not in offsets:
+                offsets[key] = n_taps
+                tables.append(self._taps(n_in, n_out, horizontal))
                 n_taps += n_out
-            return offsets[(n_in, n_out)]
+            return offsets[key]
 
-        descs = (_lib.ZoomImage * B)()
+        L = _lib.lib()
+        descs = ((_lib.CvImage if self.opencv else _lib.ZoomImage) * B)()
         metas, srcs = [], []
         with torch.cuda.stream(st):
             canvas = torch.empty((B, ch, cw, 3), dtype=torch.uint8, device=self.device)
@@ -338,7 +415,9 @@ class GpuPreprocess:
                 src = im.pin_memory().to(self.device, non_blocking=True) if not im.is_cuda else im
                 srcs.append(src)
                 d.src, d.h, d.w, d.th, d.tw, d.left, d.top = src.data_ptr(), h, w, th, tw, ltrb[0], ltrb[1]
-                d.ytab, d.xtab = tap_offset(h, th), tap_offset(w, tw)
+                d.ytab, d.xtab = tap_offset(h, th, False), tap_offset(w, tw, True)
+                if self.opencv:
+                    d.pitch = w * 3
                 if not all(0 <= c <= 255 for c in f):
                     raise RuntimeError(f'fill colour out of range: {f}')
                 d.fill[:3] = f
@@ -346,9 +425,9 @@ class GpuPreprocess:
             taps = np.ascontiguousarray(np.concatenate(tables))
             ws_bytes = ctypes.sizeof(descs) + taps.nbytes
             workspace = torch.empty((ws_bytes,), dtype=torch.uint8, device=self.device)
-            _lib.check(_lib.lib().pifpaf_image_zoom_linear_u8(
-                descs, B, taps.ctypes.data, taps.size, workspace.data_ptr(), ws_bytes, canvas.data_ptr(), ch, cw,
-                ctypes.c_void_p(st.cuda_stream)))
+            entry = L.pifpaf_image_resize_linear_cv_u8 if self.opencv else L.pifpaf_image_zoom_linear_u8
+            _lib.check(entry(descs, B, taps.ctypes.data, taps.size, workspace.data_ptr(), ws_bytes, canvas.data_ptr(),
+                             ch, cw, ctypes.c_void_p(st.cuda_stream)))
             self._keepalive = (srcs, workspace)
         return canvas, metas
 
