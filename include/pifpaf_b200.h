@@ -457,8 +457,22 @@ int pifpaf_net_heads(pifpaf_net_t* net, int32_t in_tensor, int32_t k_cols, int32
 int pifpaf_net_heads_upsampled(pifpaf_net_t* net, int32_t in_tensor, int32_t k_cols, int32_t n_heads,
                                const int32_t* n_fields, const int32_t* n_comp, const int32_t* comp_ops,
                                int32_t upsample_stride, const float* weight, const float* bias);
+/* The head outputs of the last forward and their size (n_fields, n_comp, h, w) at the current input size. */
 int pifpaf_net_head_output(pifpaf_net_t* net, int32_t head, float** dev_ptr,
                            int32_t* n_fields, int32_t* n_comp, int32_t* h, int32_t* w);
+
+/* Input size of the following forwards.  The sizes the net was emitted at are its CAPACITY: buffers stay as they
+ * were allocated, and at a smaller size every tensor [batch][h][w][c_phys] and every head output is packed densely
+ * from the start of its buffer.  in_h x in_w is the stem's input (a net without a stem: its first tensor's size);
+ * tensor_hw[2 * t], tensor_hw[2 * t + 1] is the h, w of tensor t at that size, one pair per tensor in order of
+ * creation (openpifpaf_b200/network.py derives them with the rule the ops were lowered with).  The table is checked
+ * against every op's output rule (kernel, stride, pad, dilation); a size where a tensor would exceed its capacity in
+ * h or w, or where an op would have an empty output, or a table that disagrees with the ops, is PIFPAF_E_BADARG and
+ * leaves the previous size in force.  Only host-side launch arguments and tensor maps change (they go by value into
+ * every launch), so a forward still running at the previous size is not disturbed.  Taps, head outputs,
+ * pifpaf_net_set_tensor, the forwards and pifpaf_net_flops_per_image then work at the new size. */
+int pifpaf_net_set_input_size(pifpaf_net_t* net, int32_t in_h, int32_t in_w, int32_t n_tensors,
+                              const int32_t* tensor_hw);
 
 /* Head-output buffering.  n_buffers == 2: successive forwards alternate between two sets of head-output buffers, so
  * that the decode of forward i (reading set i & 1 on another stream) may overlap forward i+1;

@@ -111,6 +111,7 @@ SYMBOLS = {
     'pifpaf_net_heads': (ctypes.c_int, [VP, c_i32, c_i32, c_i32, VP, VP, VP, VP, VP]),
     'pifpaf_net_heads_upsampled': (ctypes.c_int, [VP, c_i32, c_i32, c_i32, VP, VP, VP, c_i32, VP, VP]),
     'pifpaf_net_head_output': (ctypes.c_int, [VP, c_i32, P(VP), P(c_i32), P(c_i32), P(c_i32), P(c_i32)]),
+    'pifpaf_net_set_input_size': (ctypes.c_int, [VP, c_i32, c_i32, c_i32, VP]),
     'pifpaf_net_set_head_buffers': (ctypes.c_int, [VP, c_i32]),
     'pifpaf_net_set_sm_limit': (ctypes.c_int, [VP, c_i32]),
     'pifpaf_net_forward': (ctypes.c_int, [VP, VP, c_i32, c_i32, VP]),

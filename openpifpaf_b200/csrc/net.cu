@@ -1883,7 +1883,9 @@ const InConvKernel INPUT_CONV_KERNELS[2][4] = {
     {k_input_conv<1, false>, k_input_conv<3, false>, k_input_conv<5, false>, k_input_conv<7, false>},
     {k_input_conv<1, true>, k_input_conv<3, true>, k_input_conv<5, true>, k_input_conv<7, true>}};
 
-struct Tensor { int h, w, c; __nv_bfloat16* data; };
+// h, w: the size at the net's current input size (pifpaf_net_set_input_size); the buffer holds max_batch images at
+// the capacity cap_h x cap_w it was created for, and a smaller size packs them densely [batch][h][w][c] from its start
+struct Tensor { int h, w, c; __nv_bfloat16* data; int cap_h, cap_w; };
 
 // the values are the op kinds pifpaf_net_forward_timed reports (a fused 1x1 -> depthwise pair: OP_FUSED)
 enum OpKind { OP_INPUT_CONV, OP_GEMM, OP_DW, OP_FUSED, OP_MAXPOOL };
@@ -1915,6 +1917,12 @@ struct Op {
     double bytes_per_image = 0;      // algorithmic activation bytes (inputs once + outputs once)
     double weight_bytes = 0;
     int n_real = 0;                  // output channels that are not padding (emit_gemm)
+    // what op_geometry needs besides the kernel arguments to recompute the work per image at another size
+    long long nnz = 0;               // GEMM / fused: non-zero weights (emit_gemm, pifpaf_net_dw_conv1x1_scatter)
+    int k_real = 0;                  // flat GEMM: input channels some weight reads
+    int c_real = 0;                  // stem: output channels; depthwise, max pool, fused: channels (without padding)
+    int in_col_off = 0;              // fused: first column of the depthwise input window
+    int shuffle_t = -1;              // shuffle GEMM: the pass-through tensor (tmap_src)
     double a_bytes_per_image = 0;    // GEMM: the input part of bytes_per_image
     double dw_out_bytes_per_image = 0;   // depthwise: the output part of bytes_per_image
     std::vector<int> touches;        // tensor ids the op reads or writes (-1: none)
@@ -1952,7 +1960,8 @@ struct pifpaf_net {
     size_t pw_dw_planned = 0;            // ops.size() when plan_pw_dw last ran
     int elided_batch = 0;                // > 0: the last forward elided GEMMs (at this batch); pifpaf_net_tap_tensor re-runs them
     int head_fields[4] = {0, 0, 0, 0}, head_comp[4] = {0, 0, 0, 0}, head_h = 0, head_w = 0;
-    int in_h = 0, in_w = 0;
+    int in_h = 0, in_w = 0;              // the stem's input at the current size (0: a heads-only net)
+    int cap_in_h = 0, cap_in_w = 0;      // ... and at the capacity the net was created for
 };
 
 namespace {
@@ -2109,22 +2118,14 @@ int emit_gemm(pifpaf_net* net, Op& op, int in_tensor, int in_col_off, int k_cols
     if (rc != PIFPAF_OK) return rc;
 
     GemmArgs& g = op.g;
-    const size_t rows_max = (size_t)net->max_batch * tin.h * tin.w;
     g.N = n_out; g.K = k_cols; g.a_col0 = in_col_off;
     g.block_n = block_n; g.n_blocks = n_blocks;
     g.num_k_blocks = num_k_blocks;
     g.bias = gw.bias;
     g.a = tin.data + in_col_off; g.lda = tin.c; g.wgt = gw.w; g.ldw = k_pad;
-    op.a_tensor = in_tensor; op.rows_per_image = tin.h * tin.w;
-    op.n_real = gw.n_real;
-    op.flops_per_image = 2.0 * (double)op.rows_per_image * (double)gw.nnz;
-    op.bytes_per_image = (double)op.rows_per_image * gw.k_real * 2.0;      // A read once (bf16); outputs added by the caller
-    op.a_bytes_per_image = op.bytes_per_image;
+    op.a_tensor = in_tensor;
+    op.n_real = gw.n_real; op.nnz = gw.nnz; op.k_real = gw.k_real;
     op.weight_bytes = (double)gw.nnz * 2.0;
-    // the map covers the whole tensor; the view's first column is a TMA coordinate (16-byte aligned).
-    // Columns past the view multiply zero weight rows (B is zero padded), columns past the tensor are zero filled.
-    rc = make_tmap(&op.tmap_a, tin.data, rows_max, (uint64_t)tin.c, (uint64_t)tin.c, BM);
-    if (rc != PIFPAF_OK) return rc;
     rc = make_tmap(&op.tmap_b, gw.w, (uint64_t)n_pad, (uint64_t)k_pad, (uint64_t)k_pad, (uint32_t)block_n);
     return rc;
 }
@@ -2147,7 +2148,6 @@ int set_plain_epilogue(const pifpaf_net* net, Op& op, int relu, const Tensor& to
                        int residual_tensor, int residual_col_off) {
     GemmArgs& g = op.g;
     g.mode = MODE_PLAIN; g.relu = relu; g.out = to.data; g.ldo = to.c; g.out_col_off = out_col_off;
-    op.bytes_per_image += (double)op.rows_per_image * op.n_real * 2.0 * (residual_tensor >= 0 ? 2.0 : 1.0);
     if (residual_tensor >= 0) return set_residual(net, g, residual_tensor, residual_col_off, to.h, to.w);
     if (net->gemm_tma_store && g.relu != ACT_RELU6) {
         g.tma_store = 1;
@@ -2209,6 +2209,100 @@ void choose_dw_kernels(const pifpaf_net* net, Op& op) {
     }
     if (kernel == 5 && dilation == 1 && (stride == 1 || stride == 2))
         op.dw_simt5 = stride == 1 ? k_dwconv5<1> : k_dwconv5<2>;
+}
+
+// output rows (or columns) of a window of `kernel` taps `dil` apart, moved by `stride`, over n input rows zero padded
+// by `pad` on both sides; 0 where the window does not fit (an empty layer)
+inline int conv_out(int n, int kernel, int stride, int pad, int dil) {
+    const int span = dil * (kernel - 1) + 1;
+    return n + 2 * pad < span ? 0 : (n + 2 * pad - span) / stride + 1;
+}
+
+// the output size of an op on an hin x win input (the stem's input: the image).  1x1 GEMMs, the fused depthwise ->
+// 1x1 op (5x5, stride 1, pad 2) and the heads keep the size; the heads' PixelShuffle crop is op_geometry's.
+void op_out_hw(const Op& op, int hin, int win, int* ho, int* wo) {
+    int k = 1, s = 1, p = 0, d = 1;
+    if (op.kind == OP_INPUT_CONV) { k = op.ic.kernel; s = op.ic.stride; p = op.ic.pad; }
+    else if (op.kind == OP_DW || op.kind == OP_MAXPOOL) { k = op.dw.kernel; s = op.dw.stride; p = op.dw.pad; d = op.dw_dil; }
+    else if (op.g.conv_k > 0) { k = op.g.conv_k; s = op.g.conv_stride; p = op.g.conv_pad; d = op.g.conv_dil; }
+    *ho = conv_out(hin, k, s, p, d);
+    *wo = conv_out(win, k, s, p, d);
+}
+
+// The size-dependent part of an op, from the current h x w of its input tensor (the stem: net->in_h x in_w): the
+// spatial arguments of its kernels, the tensor maps that carry a spatial dimension, rows and tiles per image, the
+// heads' output size and the work per image.  Emit runs it at the capacity, pifpaf_net_set_input_size at each size.
+// Nothing else depends on the size: weights, biases, the scatter destination tables (base + column, row pitch) and the
+// heads' column table in device memory depend on channels only, and store maps follow the batch rows at launch.
+int op_geometry(pifpaf_net* net, Op& op) {
+    const Tensor* tin = op.a_tensor >= 0 ? &net->tensors[op.a_tensor] : nullptr;
+    const int hin = tin ? tin->h : net->in_h, win = tin ? tin->w : net->in_w;
+    const uint64_t nb = (uint64_t)net->max_batch;
+    int ho, wo;
+    op_out_hw(op, hin, win, &ho, &wo);
+    PIFPAF_CHECK_ARG(ho >= 1 && wo >= 1, "a layer would have an empty output at this input size");
+    if (op.kind == OP_INPUT_CONV) {
+        InConvArgs& a = op.ic;
+        a.Hin = hin; a.Win = win; a.Hout = ho; a.Wout = wo;
+        op.flops_per_image = 2.0 * ho * wo * op.c_real * 3.0 * a.kernel * a.kernel;
+        op.bytes_per_image = (double)hin * win * 3 * 4.0 + (double)ho * wo * op.c_real * 2.0;
+        return PIFPAF_OK;
+    }
+    if (op.kind == OP_DW || op.kind == OP_MAXPOOL) {
+        DwArgs& a = op.dw;
+        a.Hin = hin; a.Win = win; a.Hout = ho; a.Wout = wo;
+        op.bytes_per_image = ((double)hin * win + (double)ho * wo) * op.c_real * 2.0;
+        if (op.kind == OP_MAXPOOL) return PIFPAF_OK;
+        op.flops_per_image = 2.0 * ho * wo * op.c_real * (double)a.kernel * a.kernel;
+        op.dw_out_bytes_per_image = (double)ho * wo * op.c_real * 2.0;
+        if (!op.dw_tma) return PIFPAF_OK;
+        return make_tmap_dw(&op.tmap_dw, a.in + a.in_col_off, (uint64_t)a.C8 * 8, (uint64_t)win, (uint64_t)hin, nb,
+                            (uint64_t)a.ld_in, op.dw_tma->box_w, op.dw_tma->box_h);
+    }
+    GemmArgs& g = op.g;
+    if (g.conv_k > 0) {
+        // implicit-GEMM conv (OP_GEMM) or fused depthwise -> 1x1 (OP_FUSED): M tiles are PH x PW output patches, and
+        // the window map ends at the image edge (its zero fill is the conv padding)
+        g.Hi = hin; g.Wi = win; g.Ho = ho; g.Wo = wo;
+        g.tiles_x = (wo + PW - 1) / PW; g.tiles_y = (ho + PH - 1) / PH;
+        op.rows_per_image = ho * wo; op.tiles_per_image = g.tiles_x * g.tiles_y;
+        if (op.kind == OP_FUSED) {
+            op.flops_per_image = 2.0 * (double)op.rows_per_image * ((double)op.nnz + 25.0 * op.c_real);
+            op.bytes_per_image = (double)op.rows_per_image * (op.c_real + op.n_real) * 2.0;  // dw input once + 1x1 output once
+            using T = DwTile<1, PH, PW, 4, 1>;
+            return make_tmap_dw(&op.tmap_dw, tin->data + op.in_col_off, (uint64_t)op.fu.C, (uint64_t)win, (uint64_t)hin,
+                                nb, (uint64_t)tin->c, T::IW, T::IH);
+        }
+        // dense shapes: every weight and input channel counted
+        op.flops_per_image = 2.0 * (double)ho * wo * g.N * g.K * (g.conv_k * g.conv_k);
+        op.bytes_per_image = (double)hin * win * g.K * 2.0 + (double)ho * wo * g.N * 2.0 * (g.res != nullptr ? 2.0 : 1.0);
+        return make_tmap_conv(&op.tmap_a, g.a, (uint64_t)g.K, (uint64_t)win, (uint64_t)hin, nb, (uint64_t)g.lda,
+                              g.conv_stride);
+    }
+    // flat 1x1 GEMM over batch * hin * win rows
+    op.rows_per_image = hin * win;
+    op.flops_per_image = 2.0 * (double)op.rows_per_image * (double)op.nnz;
+    op.a_bytes_per_image = (double)op.rows_per_image * op.k_real * 2.0;      // A read once (bf16)
+    double out_bytes = (double)op.rows_per_image * op.n_real * 2.0;
+    if (g.mode == MODE_PLAIN && g.res != nullptr) out_bytes = (double)op.rows_per_image * op.n_real * 2.0 * 2.0;
+    if (g.mode == MODE_SHUFFLE) out_bytes = (double)op.rows_per_image * op.n_real * 2.0 * 3.0;  // + pass-through in and out
+    if (g.mode == MODE_HEADS) {
+        // PixelShuffle(up) + crop (heads.py:336-343): low_cut = (up - 1) / 2, high_cut = ceil((up - 1) / 2)
+        g.hw = hin * win; g.w = win;
+        g.out_h = hin * g.up - g.up_low - g.up / 2; g.out_w = win * g.up - g.up_low - g.up / 2;
+        PIFPAF_CHECK_ARG(g.out_h >= 1 && g.out_w >= 1, "feature map too small for this upsample_stride");
+        net->head_h = g.out_h; net->head_w = g.out_w;
+        out_bytes = (double)g.out_h * g.out_w * (op.n_real / (g.up * g.up)) * 4.0;
+    }
+    op.bytes_per_image = op.a_bytes_per_image + out_bytes;
+    // the map covers the whole tensor; the view's first column is a TMA coordinate (16-byte aligned).
+    // Columns past the view multiply zero weight rows (B is zero padded), columns past the tensor are zero filled.
+    int rc = make_tmap(&op.tmap_a, tin->data, nb * hin * win, (uint64_t)tin->c, (uint64_t)tin->c, BM);
+    if (rc != PIFPAF_OK || g.mode != MODE_SHUFFLE) return rc;
+    // pass-through tile [BM rows][block_n cols], dense rows in shared memory (no swizzle)
+    const Tensor& ts = net->tensors[op.shuffle_t];
+    return make_tmap_plain(&op.tmap_src, ts.data + g.src0_col_off, nb * ts.h * ts.w,
+                           (uint64_t)std::min(ts.c - g.src0_col_off, pad16(g.N)), (uint64_t)ts.c, (uint32_t)g.block_n, BM);
 }
 
 // Decides, once all ops are known, which 1x1 GEMM -> depthwise pairs run as one k_pw_dw launch.  The GEMM qualifies
@@ -2422,7 +2516,7 @@ int pifpaf_net_tensor(pifpaf_net_t* net, int32_t h, int32_t w, int32_t c_phys, i
     PIFPAF_CHECK_ARG(net != nullptr && id != nullptr, "null argument");
     PIFPAF_CHECK_ARG(h >= 1 && w >= 1 && c_phys >= 16 && c_phys % 16 == 0, "tensor shape: c_phys must be a multiple of 16");
     PIFPAF_CUDA_TRY(cudaSetDevice(net->device));
-    Tensor t; t.h = h; t.w = w; t.c = c_phys; t.data = nullptr;
+    Tensor t; t.h = t.cap_h = h; t.w = t.cap_w = w; t.c = c_phys; t.data = nullptr;
     // + one tile of slack rows so that TMA boxes of the last partial M tile stay in mapped memory
     int rc = net_alloc(net, &t.data, ((size_t)net->max_batch * h * w + BM) * c_phys, true);
     if (rc != PIFPAF_OK) return rc;
@@ -2438,8 +2532,8 @@ int pifpaf_net_input_conv(pifpaf_net_t* net, int32_t in_h, int32_t in_w, int32_t
     PIFPAF_CHECK_ARG(out_tensor >= 0 && out_tensor < (int)net->tensors.size(), "bad tensor id");
     PIFPAF_CHECK_ARG(relu >= ACT_NONE && relu <= ACT_RELU6, "activation code must be 0 (none), 1 (ReLU) or 2 (ReLU6)");
     const Tensor& to = net->tensors[out_tensor];
-    const int ho = (in_h + 2 * pad - kernel) / stride + 1, wo = (in_w + 2 * pad - kernel) / stride + 1;
-    PIFPAF_CHECK_ARG(to.h == ho && to.w == wo && to.c >= pad8(c_out), "output tensor shape mismatch");
+    const int ho = conv_out(in_h, kernel, stride, pad, 1), wo = conv_out(in_w, kernel, stride, pad, 1);
+    PIFPAF_CHECK_ARG(ho >= 1 && wo >= 1 && to.h == ho && to.w == wo && to.c >= pad8(c_out), "output tensor shape mismatch");
     PIFPAF_CHECK_ARG(kernel == 1 || kernel == 3 || kernel == 5 || kernel == 7, "input conv kernel must be 1, 3, 5 or 7");
     PIFPAF_CHECK_ARG(c_out >= 1 && input_conv_smem_bytes(kernel, pad8(c_out) / 8) <= (size_t)INCONV_SMEM_MAX,
                      "input conv: the weights of a kxk conv with this many output channels do not fit in shared memory");
@@ -2460,12 +2554,13 @@ int pifpaf_net_input_conv(pifpaf_net_t* net, int32_t in_h, int32_t in_w, int32_t
     rc = net_upload(net, &d_b, b); if (rc != PIFPAF_OK) return rc;
     InConvArgs& a = op.ic;
     a.in = nullptr; a.out = to.data; a.ld_out = to.c; a.weight = d_w; a.bias = d_b;
-    a.Hin = in_h; a.Win = in_w; a.Hout = ho; a.Wout = wo; a.C8 = C / 8;
+    a.C8 = C / 8;
     a.kernel = kernel; a.stride = stride; a.pad = pad; a.relu = relu;
-    op.flops_per_image = 2.0 * ho * wo * c_out * 3.0 * kernel * kernel;
-    op.bytes_per_image = (double)in_h * in_w * 3 * 4.0 + (double)ho * wo * c_out * 2.0;
+    op.c_real = c_out;
     op.touches = {out_tensor};
-    net->in_h = in_h; net->in_w = in_w;
+    net->in_h = net->cap_in_h = in_h; net->in_w = net->cap_in_w = in_w;
+    rc = op_geometry(net, op);
+    if (rc != PIFPAF_OK) return rc;
     net->ops.push_back(op);
     return PIFPAF_OK;
 }
@@ -2502,18 +2597,14 @@ int pifpaf_net_conv1x1(pifpaf_net_t* net, int32_t in_tensor, int32_t in_col_off,
                          "shuffle source window");
         PIFPAF_CHECK_ARG(out_col_off == 0 && to.c >= 2 * n_out, "shuffle output tensor must hold 2*n_out channels");
         g.mode = MODE_SHUFFLE; g.relu = relu; g.out = to.data; g.ldo = to.c; g.out_col_off = out_col_off;
-        // outputs: n_out bf16 per row, and the pass-through half read and re-written
-        op.bytes_per_image += (double)op.rows_per_image * op.n_real * 2.0 * 3.0;
         g.src0 = ts.data; g.ld0 = ts.c; g.src0_col_off = shuffle_src_col_off;
         g.half = n_out; g.gap = 0;
         g.src_tma = gemm_smem_bytes(g.block_n, g.n_blocks, 2, true) <= GEMM_SMEM_BUDGET ? 1 : 0;
-        // pass-through tile [BM rows][block_n cols], dense rows in shared memory (no swizzle)
-        rc = make_tmap_plain(&op.tmap_src, ts.data + shuffle_src_col_off, (uint64_t)net->max_batch * ts.h * ts.w,
-                             (uint64_t)std::min(ts.c - shuffle_src_col_off, pad16(n_out)), (uint64_t)ts.c,
-                             (uint32_t)g.block_n, BM);
-        if (rc != PIFPAF_OK) return rc;
+        op.shuffle_t = shuffle_src_tensor;
     }
     plan_gemm_smem(op);
+    rc = op_geometry(net, op);
+    if (rc != PIFPAF_OK) return rc;
     op.touches = {in_tensor, out_tensor, shuffle_src_tensor};
     net->ops.push_back(op);
     return PIFPAF_OK;
@@ -2549,8 +2640,9 @@ int pifpaf_net_conv1x1_scatter(pifpaf_net_t* net, int32_t in_tensor, int32_t in_
             op.store_views.push_back(Op::StoreView{to.data, to.c, to.c});
         }
     }
-    op.bytes_per_image += (double)op.rows_per_image * op.n_real * 2.0;
     plan_gemm_smem(op);
+    rc = op_geometry(net, op);
+    if (rc != PIFPAF_OK) return rc;
     op.touches.assign(piece_tensor, piece_tensor + n_pieces);
     op.touches.push_back(in_tensor);
     net->ops.push_back(op);
@@ -2581,9 +2673,8 @@ int pifpaf_net_conv_dilated(pifpaf_net_t* net, int32_t in_tensor, int32_t in_col
     PIFPAF_CUDA_TRY(cudaSetDevice(net->device));
     const Tensor& tin = net->tensors[in_tensor];
     const Tensor& to = net->tensors[out_tensor];
-    const int span = dilation * (kernel - 1) + 1;
-    PIFPAF_CHECK_ARG(tin.h + 2 * pad >= span && tin.w + 2 * pad >= span, "conv window larger than the padded input");
-    const int ho = (tin.h + 2 * pad - span) / stride + 1, wo = (tin.w + 2 * pad - span) / stride + 1;
+    const int ho = conv_out(tin.h, kernel, stride, pad, dilation), wo = conv_out(tin.w, kernel, stride, pad, dilation);
+    PIFPAF_CHECK_ARG(ho >= 1 && wo >= 1, "conv window larger than the padded input");
     PIFPAF_CHECK_ARG(to.h == ho && to.w == wo, "conv output tensor shape mismatch");
     PIFPAF_CHECK_ARG(in_col_off % 8 == 0 && in_col_off + c_in <= tin.c, "conv input column window");
     PIFPAF_CHECK_ARG(out_col_off % 16 == 0 && out_col_off + pad8(n_out) <= to.c, "conv output column window");
@@ -2595,6 +2686,8 @@ int pifpaf_net_conv_dilated(pifpaf_net_t* net, int32_t in_tensor, int32_t in_col
         rc = set_plain_epilogue(net, op, relu, to, out_col_off, residual_tensor, residual_col_off);
         if (rc != PIFPAF_OK) return rc;
         plan_gemm_smem(op);
+        rc = op_geometry(net, op);
+        if (rc != PIFPAF_OK) return rc;
         op.touches = {in_tensor, out_tensor, residual_tensor};
         net->ops.push_back(op);
         return PIFPAF_OK;
@@ -2616,21 +2709,15 @@ int pifpaf_net_conv_dilated(pifpaf_net_t* net, int32_t in_tensor, int32_t in_col
     g.bias = gw.bias; g.mode = MODE_PLAIN; g.relu = relu;
     g.out = to.data; g.ldo = to.c; g.out_col_off = out_col_off;
     g.conv_k = kernel; g.conv_stride = stride; g.conv_pad = pad; g.conv_dil = dilation; g.conv_cblocks = cblocks;
-    g.Hi = tin.h; g.Wi = tin.w; g.Ho = ho; g.Wo = wo;
-    g.tiles_x = (wo + PW - 1) / PW; g.tiles_y = (ho + PH - 1) / PH;
     g.a = tin.data + in_col_off; g.lda = tin.c; g.wgt = gw.w; g.ldw = k_total;
     if (residual_tensor >= 0) {
         rc = set_residual(net, g, residual_tensor, residual_col_off, ho, wo);
         if (rc != PIFPAF_OK) return rc;
     }
-    op.a_tensor = in_tensor; op.rows_per_image = ho * wo; op.tiles_per_image = g.tiles_x * g.tiles_y;
+    op.a_tensor = in_tensor;
     plan_gemm_smem(op);
-    // dense shapes: every weight and input channel counted
-    op.flops_per_image = 2.0 * (double)ho * wo * n_out * c_in * taps;
-    op.bytes_per_image = (double)tin.h * tin.w * c_in * 2.0 + (double)ho * wo * n_out * 2.0 * (residual_tensor >= 0 ? 2.0 : 1.0);
     op.weight_bytes = (double)n_out * c_in * taps * 2.0;
-    rc = make_tmap_conv(&op.tmap_a, tin.data + in_col_off, (uint64_t)c_in, (uint64_t)tin.w, (uint64_t)tin.h,
-                        (uint64_t)net->max_batch, (uint64_t)tin.c, stride);
+    rc = op_geometry(net, op);
     if (rc != PIFPAF_OK) return rc;
     rc = make_tmap(&op.tmap_b, gw.w, (uint64_t)n_pad, (uint64_t)k_total, (uint64_t)k_total, (uint32_t)block_n);
     if (rc != PIFPAF_OK) return rc;
@@ -2658,10 +2745,9 @@ int pifpaf_net_dwconv_dilated(pifpaf_net_t* net, int32_t in_tensor, int32_t in_c
     PIFPAF_CHECK_ARG(dilation == 1 || stride == 1, "a dilated dwconv (dilation > 1) must have stride 1");
     const Tensor& tin = net->tensors[in_tensor];
     const Tensor& to = net->tensors[out_tensor];
-    const int span = dilation * (kernel - 1) + 1;
-    const int ho = (tin.h + 2 * pad - span) / stride + 1, wo = (tin.w + 2 * pad - span) / stride + 1;
+    const int ho = conv_out(tin.h, kernel, stride, pad, dilation), wo = conv_out(tin.w, kernel, stride, pad, dilation);
     const int C = pad8(channels);
-    PIFPAF_CHECK_ARG(to.h == ho && to.w == wo, "dwconv output tensor shape mismatch");
+    PIFPAF_CHECK_ARG(ho >= 1 && wo >= 1 && to.h == ho && to.w == wo, "dwconv output tensor shape mismatch");
     PIFPAF_CHECK_ARG(in_col_off % 8 == 0 && out_col_off % 8 == 0 && in_col_off + C <= tin.c && out_col_off + C <= to.c,
                      "dwconv column windows");
     PIFPAF_CUDA_TRY(cudaSetDevice(net->device));
@@ -2673,19 +2759,14 @@ int pifpaf_net_dwconv_dilated(pifpaf_net_t* net, int32_t in_tensor, int32_t in_c
     a.in = tin.data; a.ld_in = tin.c; a.in_col_off = in_col_off;
     a.out = to.data; a.ld_out = to.c; a.out_col_off = out_col_off;
     a.weight = d_w; a.bias = d_b;
-    a.Hin = tin.h; a.Win = tin.w; a.Hout = ho; a.Wout = wo; a.C8 = C / 8;
+    a.C8 = C / 8;
     a.kernel = kernel; a.stride = stride; a.pad = pad; a.relu = relu;
     op.dw_dil = dilation;
-    op.flops_per_image = 2.0 * ho * wo * channels * (double)kernel * kernel;
-    op.bytes_per_image = ((double)tin.h * tin.w + (double)ho * wo) * channels * 2.0;
+    op.a_tensor = in_tensor; op.c_real = channels;
     choose_dw_kernels(net, op);
-    if (op.dw_tma) {
-        rc = make_tmap_dw(&op.tmap_dw, tin.data + in_col_off, (uint64_t)C, (uint64_t)tin.w, (uint64_t)tin.h,
-                          (uint64_t)net->max_batch, (uint64_t)tin.c, op.dw_tma->box_w, op.dw_tma->box_h);
-        if (rc != PIFPAF_OK) return rc;
-    }
+    rc = op_geometry(net, op);
+    if (rc != PIFPAF_OK) return rc;
     op.touches = {in_tensor, out_tensor};
-    op.dw_out_bytes_per_image = (double)ho * wo * channels * 2.0;
     net->ops.push_back(op);
     return PIFPAF_OK;
 }
@@ -2699,7 +2780,7 @@ int pifpaf_net_maxpool(pifpaf_net_t* net, int32_t in_tensor, int32_t in_col_off,
     PIFPAF_CHECK_ARG(channels >= 1, "bad channel count");
     const Tensor& tin = net->tensors[in_tensor];
     const Tensor& to = net->tensors[out_tensor];
-    const int ho = (tin.h - 1) / stride + 1, wo = (tin.w - 1) / stride + 1;     // (h + 2 * 1 - 3) / s + 1
+    const int ho = conv_out(tin.h, 3, stride, 1, 1), wo = conv_out(tin.w, 3, stride, 1, 1);
     const int C = pad8(channels);
     PIFPAF_CHECK_ARG(to.h == ho && to.w == wo, "max pool output tensor shape mismatch");
     PIFPAF_CHECK_ARG(in_col_off % 8 == 0 && out_col_off % 8 == 0 && in_col_off + C <= tin.c && out_col_off + C <= to.c,
@@ -2708,10 +2789,11 @@ int pifpaf_net_maxpool(pifpaf_net_t* net, int32_t in_tensor, int32_t in_col_off,
     DwArgs& a = op.dw;
     a.in = tin.data; a.ld_in = tin.c; a.in_col_off = in_col_off;
     a.out = to.data; a.ld_out = to.c; a.out_col_off = out_col_off;
-    a.Hin = tin.h; a.Win = tin.w; a.Hout = ho; a.Wout = wo; a.C8 = C / 8;
+    a.C8 = C / 8;
     a.kernel = 3; a.stride = stride; a.pad = 1; a.relu = 0;
-    op.flops_per_image = 0;
-    op.bytes_per_image = ((double)tin.h * tin.w + (double)ho * wo) * channels * 2.0;
+    op.a_tensor = in_tensor; op.c_real = channels;
+    const int rc = op_geometry(net, op);
+    if (rc != PIFPAF_OK) return rc;
     op.touches = {in_tensor, out_tensor};
     net->ops.push_back(op);
     return PIFPAF_OK;
@@ -2759,9 +2841,7 @@ int pifpaf_net_dw_conv1x1_scatter(pifpaf_net_t* net, int32_t in_tensor, int32_t 
     g.num_k_blocks = (C + BK - 1) / BK;
     g.bias = gw.bias; g.mode = MODE_SCATTER; g.relu = relu;
     g.conv_k = kernel; g.conv_stride = stride; g.conv_pad = pad; g.conv_dil = 1; g.conv_cblocks = g.num_k_blocks;
-    g.Hi = tin.h; g.Wi = tin.w; g.Ho = tin.h; g.Wo = tin.w;
-    g.tiles_x = (g.Wo + PW - 1) / PW; g.tiles_y = (g.Ho + PH - 1) / PH;
-    op.a_tensor = in_tensor; op.rows_per_image = g.Ho * g.Wo; op.tiles_per_image = g.tiles_x * g.tiles_y;
+    op.a_tensor = in_tensor; op.in_col_off = in_col_off;
     // ring depths: as deep as the shared memory allows, windows first (their TMA has the longest latency)
     const int cand[][2] = {{3, 2}, {2, 2}, {2, 1}, {1, 1}};
     bool fits = false;
@@ -2772,13 +2852,9 @@ int pifpaf_net_dw_conv1x1_scatter(pifpaf_net_t* net, int32_t in_tensor, int32_t 
     }
     PIFPAF_CHECK_ARG(fits, "fused depthwise -> 1x1 op does not fit in shared memory");
     op.smem = fused_smem_bytes(f.ws, f.bs, block_n, n_pad, C);
-    op.n_real = gw.n_real;
-    op.flops_per_image = 2.0 * (double)op.rows_per_image * ((double)gw.nnz + 25.0 * channels);
-    op.bytes_per_image = (double)op.rows_per_image * (channels + gw.n_real) * 2.0;     // dw input once + 1x1 output once
+    op.n_real = gw.n_real; op.nnz = gw.nnz; op.c_real = channels;
     op.weight_bytes = (double)gw.nnz * 2.0 + 25.0 * channels * 4.0;
-    using T = DwTile<1, PH, PW, 4, 1>;
-    rc = make_tmap_dw(&op.tmap_dw, tin.data + in_col_off, (uint64_t)C, (uint64_t)tin.w, (uint64_t)tin.h,
-                      (uint64_t)net->max_batch, (uint64_t)tin.c, T::IW, T::IH);
+    rc = op_geometry(net, op);
     if (rc != PIFPAF_OK) return rc;
     rc = make_tmap(&op.tmap_b, gw.w, (uint64_t)n_pad, (uint64_t)C, (uint64_t)C, (uint32_t)block_n);
     if (rc != PIFPAF_OK) return rc;
@@ -2802,12 +2878,7 @@ int pifpaf_net_heads_upsampled(pifpaf_net_t* net, int32_t in_tensor, int32_t k_c
     PIFPAF_CHECK_ARG(upsample_stride >= 1 && upsample_stride <= 8, "upsample_stride must be in [1, 8]");
     PIFPAF_CHECK_ARG(in_tensor >= 0 && in_tensor < (int)net->tensors.size(), "bad tensor id");
     PIFPAF_CUDA_TRY(cudaSetDevice(net->device));
-    const Tensor& tin = net->tensors[in_tensor];
     const int up = upsample_stride, up2 = up * up;
-    // heads.py:336-343: low_cut = (up - 1) / 2, high_cut = ceil((up - 1) / 2)
-    const int low = (up - 1) / 2, high = up / 2;
-    const int out_h = tin.h * up - low - high, out_w = tin.w * up - low - high;
-    PIFPAF_CHECK_ARG(out_h >= 1 && out_w >= 1, "feature map too small for this upsample_stride");
     int n_total = 0;
     for (int i = 0; i < n_heads; i++) n_total += n_fields[i] * n_comp[i] * up2;
     Op op; op.kind = OP_GEMM;
@@ -2815,7 +2886,9 @@ int pifpaf_net_heads_upsampled(pifpaf_net_t* net, int32_t in_tensor, int32_t k_c
     if (rc != PIFPAF_OK) return rc;
     GemmArgs& g = op.g;
     g.mode = MODE_HEADS; g.relu = 0;
-    op.bytes_per_image += (double)out_h * out_w * (op.n_real / up2) * 4.0;
+    g.up = up; g.up_low = (up - 1) / 2;
+    rc = op_geometry(net, op);
+    if (rc != PIFPAF_OK) return rc;
     std::vector<HeadCol> cols((size_t)g.block_n * g.n_blocks, HeadCol{0, 0, 0, 0});
     int col = 0, op_off = 0;
     for (int i = 0; i < n_heads; i++) {
@@ -2826,7 +2899,7 @@ int pifpaf_net_heads_upsampled(pifpaf_net_t* net, int32_t in_tensor, int32_t k_c
                         cols[col++] = HeadCol{i, f * n_comp[i] + c, comp_ops[op_off + c], (dy << 8) | dx};
         op_off += n_comp[i];
         net->head_fields[i] = n_fields[i]; net->head_comp[i] = n_comp[i];
-        net->head_elems[i] = (size_t)net->max_batch * n_fields[i] * n_comp[i] * out_h * out_w;
+        net->head_elems[i] = (size_t)net->max_batch * n_fields[i] * n_comp[i] * g.out_h * g.out_w;
         rc = net_alloc(net, &net->head_out[0][i], net->head_elems[i], true);
         if (rc != PIFPAF_OK) return rc;
         g.head_base[i] = net->head_out[0][i];
@@ -2835,12 +2908,61 @@ int pifpaf_net_heads_upsampled(pifpaf_net_t* net, int32_t in_tensor, int32_t k_c
     HeadCol* d_cols = nullptr;
     rc = net_upload(net, &d_cols, cols); if (rc != PIFPAF_OK) return rc;
     g.head_cols = d_cols;
-    g.hw = tin.h * tin.w; g.w = tin.w;
-    g.up = up; g.up_low = low; g.out_h = out_h; g.out_w = out_w;
     plan_gemm_smem(op);
-    net->n_heads = n_heads; net->head_h = out_h; net->head_w = out_w;
+    net->n_heads = n_heads;
     op.touches = {in_tensor};
     net->ops.push_back(op);
+    return PIFPAF_OK;
+}
+
+int pifpaf_net_set_input_size(pifpaf_net_t* net, int32_t in_h, int32_t in_w, int32_t n_tensors,
+                              const int32_t* tensor_hw) {
+    PIFPAF_CHECK_ARG(net != nullptr && tensor_hw != nullptr, "null argument");
+    const int nt = (int)net->tensors.size();
+    PIFPAF_CHECK_ARG(n_tensors == nt, "the tensor table needs one (h, w) pair per tensor of the net");
+    PIFPAF_CHECK_ARG(in_h >= 1 && in_w >= 1 && (net->cap_in_h == 0 || (in_h <= net->cap_in_h && in_w <= net->cap_in_w)),
+                     "input size outside 1 .. the size the net was created for");
+    for (int t = 0; t < nt; t++) {
+        const Tensor& tt = net->tensors[t];
+        const int h = tensor_hw[2 * t], w = tensor_hw[2 * t + 1];
+        if (h < 1 || w < 1 || h > tt.cap_h || w > tt.cap_w) {
+            pifpaf::set_error("tensor %d would be %dx%d: outside 1x1 .. its capacity %dx%d", t, h, w, tt.cap_h, tt.cap_w);
+            return PIFPAF_E_BADARG;
+        }
+    }
+    // the table must be what every op makes of its input at this size
+    for (size_t i = 0; i < net->ops.size(); i++) {
+        const Op& op = net->ops[i];
+        const int hin = op.a_tensor >= 0 ? tensor_hw[2 * op.a_tensor] : in_h;
+        const int win = op.a_tensor >= 0 ? tensor_hw[2 * op.a_tensor + 1] : in_w;
+        int ho, wo;
+        op_out_hw(op, hin, win, &ho, &wo);
+        if (ho < 1 || wo < 1) {
+            pifpaf::set_error("op %zu would have an empty output on its %dx%d input", i, hin, win);
+            return PIFPAF_E_BADARG;
+        }
+        for (int t : op.touches)
+            if (t >= 0 && t != op.a_tensor && (tensor_hw[2 * t] != ho || tensor_hw[2 * t + 1] != wo)) {
+                pifpaf::set_error("tensor %d is %dx%d in the table, op %zu makes it %dx%d", t, tensor_hw[2 * t],
+                                  tensor_hw[2 * t + 1], i, ho, wo);
+                return PIFPAF_E_BADARG;
+            }
+    }
+    PIFPAF_CUDA_TRY(cudaSetDevice(net->device));
+    const std::vector<Tensor> old_tensors = net->tensors;
+    const std::vector<Op> old_ops = net->ops;
+    const int old_size[4] = {net->in_h, net->in_w, net->head_h, net->head_w};
+    for (int t = 0; t < nt; t++) { net->tensors[t].h = tensor_hw[2 * t]; net->tensors[t].w = tensor_hw[2 * t + 1]; }
+    if (net->cap_in_h > 0) { net->in_h = in_h; net->in_w = in_w; }
+    int rc = PIFPAF_OK;
+    for (size_t i = 0; i < net->ops.size() && rc == PIFPAF_OK; i++) rc = op_geometry(net, net->ops[i]);
+    if (rc == PIFPAF_OK) rc = plan_pw_dw(net);
+    if (rc != PIFPAF_OK) {
+        net->tensors = old_tensors; net->ops = old_ops;
+        net->in_h = old_size[0]; net->in_w = old_size[1]; net->head_h = old_size[2]; net->head_w = old_size[3];
+        return rc;
+    }
+    net->elided_batch = 0;      // the tensors hold the last forward at the previous size
     return PIFPAF_OK;
 }
 

@@ -651,6 +651,55 @@ def _dw_rows(wb, kernel, width, cols=None):
     return wp, bp
 
 
+def conv_out_hw(h, w, kernel, stride, pad, dilation=1):
+    """Output size of a conv window (torch.nn.Conv2d / MaxPool2d without ceil_mode) on an h x w input; a size < 1 means
+    the window does not fit in the padded input.  The one rule the lowering and `tensor_shapes_at` size tensors by."""
+    span = dilation * (kernel - 1) + 1
+    return (h + 2 * pad - span) // stride + 1, (w + 2 * pad - span) // stride + 1
+
+
+def tensor_shapes_at(ops, capacity_shapes, in_h, in_w):
+    """The tensors (h, w, c_phys) of a lowering (`build_ops` at its capacity: `capacity_shapes`, `ops`) at another input
+    size, derived op by op with the rule `build_ops` lowered them with: what `build_ops(plan, in_h, in_w)` would give
+    (for a heads-only plan in_h x in_w is the feature map).  Raises RuntimeError where an op's output would be empty or
+    a tensor larger than its capacity in h or w."""
+    shapes = [None] * len(capacity_shapes)
+
+    def put(t, hw, op):
+        if hw[0] < 1 or hw[1] < 1:
+            raise RuntimeError(f'input {in_h}x{in_w}: the {op} op would have an empty output')
+        if shapes[t] is not None and shapes[t] != hw:
+            raise RuntimeError(f'tensor {t} gets two sizes, {shapes[t]} and {hw}')
+        shapes[t] = hw
+
+    for o in ops:
+        kind = o['kind']
+        if kind == 'input_conv':
+            put(o['out'], conv_out_hw(in_h, in_w, o['kernel'], o['stride'], o['pad']), kind)
+            continue
+        if shapes[o['in']] is None:          # read before anything wrote it: the net's input (heads-only plans)
+            shapes[o['in']] = (in_h, in_w)
+        h, w = shapes[o['in']]
+        if kind in ('conv', 'dwconv'):
+            hw = conv_out_hw(h, w, o['kernel'], o['stride'], o['pad'], o.get('dilation', 1))
+        elif kind == 'maxpool':
+            hw = conv_out_hw(h, w, 3, o['stride'], 1)
+        else:                               # 1x1 convs, the fused depthwise 5x5 (pad 2) -> 1x1, the heads
+            hw = (h, w)
+        outs = [pc[2] for pc in o['pieces']] if 'pieces' in o else [o[k] for k in ('out', 'residual', 'shuffle_src')
+                                                                     if o.get(k, -1) >= 0]
+        for t in outs:
+            put(t, hw, kind)
+    out = []
+    for t, ((ch, cw, c), hw) in enumerate(zip(capacity_shapes, shapes)):
+        if hw is None:
+            hw = (in_h, in_w)
+        if hw[0] > ch or hw[1] > cw:
+            raise RuntimeError(f'input {in_h}x{in_w}: tensor {t} would be {hw[0]}x{hw[1]}, above its capacity {ch}x{cw}')
+        out.append((hw[0], hw[1], c))
+    return out
+
+
 class _OpList:
     """The tensors (tensors[i] = (h, w, c_phys)) and ops of one lowering.  Each op kind is written by one method here,
     whose dict fields are the C ABI arguments (include/pifpaf_b200.h); the lowerings only wire them.  Methods without a
@@ -666,14 +715,12 @@ class _OpList:
     def out_hw(self, t_in, e):
         """output size of the conv entry e (kernel, stride, pad, optional dilation) on tensor t_in"""
         h, w, _ = self.tensors[t_in]
-        span = e.get('dilation', 1) * (e['kernel'] - 1) + 1
-        return (h + 2 * e['pad'] - span) // e['stride'] + 1, (w + 2 * e['pad'] - span) // e['stride'] + 1
+        return conv_out_hw(h, w, e['kernel'], e['stride'], e['pad'], e.get('dilation', 1))
 
     def input_conv(self, inp, in_h, in_w, act):
         """the stem on the [3, in_h, in_w] image"""
         k, c = inp['w'].shape[-1], inp['w'].shape[0]
-        t = self.tensor((in_h + 2 * inp['pad'] - k) // inp['stride'] + 1,
-                        (in_w + 2 * inp['pad'] - k) // inp['stride'] + 1, pad16(c))
+        t = self.tensor(*conv_out_hw(in_h, in_w, k, inp['stride'], inp['pad']), pad16(c))
         self.ops.append({'kind': 'input_conv', 'in_h': in_h, 'in_w': in_w, 'kernel': k, 'stride': inp['stride'],
                          'pad': inp['pad'], 'c_out': c, 'w': _f32(inp['w']), 'b': _f32(inp['b']), 'relu': act,
                          'out': t})
@@ -734,7 +781,7 @@ class _OpList:
     def maxpool(self, t_in, channels, stride):
         """3x3 max pool, padding 1"""
         h, w, _ = self.tensors[t_in]
-        t = self.tensor((h - 1) // stride + 1, (w - 1) // stride + 1, pad16(channels))
+        t = self.tensor(*conv_out_hw(h, w, 3, stride, 1), pad16(channels))
         self.ops.append({'kind': 'maxpool', 'in': t_in, 'in_off': 0, 'channels': channels, 'stride': stride,
                          'out': t, 'out_off': 0})
         return t
@@ -923,7 +970,9 @@ def _lower_mobilenetv2(L, plan, in_h, in_w):
 
 
 class CompiledNet:
-    """A plan compiled to libpifpaf_b200 ops for a fixed input size and maximum batch."""
+    """A plan compiled to libpifpaf_b200 ops for a maximum input size and batch.  in_h, in_w is that capacity; the net
+    runs at any input size up to it (`set_input_size`), each tensor packed densely in the buffer allocated for the
+    capacity, and computes there what a net compiled at exactly that size computes."""
 
     def __init__(self, plan, in_h, in_w, max_batch, device=0, layout=None, fuse_dw=None):
         self.lib = _lib.lib()
@@ -931,6 +980,8 @@ class CompiledNet:
         self.max_batch = int(max_batch)
         self.in_h, self.in_w = int(in_h), int(in_w)
         self.tensor_shapes, ops, self.info = build_ops(plan, self.in_h, self.in_w, layout=layout, fuse_dw=fuse_dw)
+        self.capacity_shapes = list(self.tensor_shapes)
+        self._input_size = (self.in_h, self.in_w)
         self.op_desc = [{k: v for k, v in o.items() if not isinstance(v, np.ndarray)} for o in ops]
         self.handle = ctypes.c_void_p()
         _lib.check(self.lib.pifpaf_net_create(ctypes.byref(self.handle), self.device, self.max_batch))
@@ -945,6 +996,33 @@ class CompiledNet:
                                                        ctypes.byref(nc), ctypes.byref(hh), ctypes.byref(ww)))
             self.heads.append({'ptr': ptr.value, 'n_fields': nf.value, 'n_comp': nc.value,
                                'h': hh.value, 'w': ww.value, 'stride': h['stride']})
+
+    @property
+    def input_size(self):
+        """(h, w) the forwards take now: the capacity (in_h, in_w) until `set_input_size` changes it."""
+        return self._input_size
+
+    def set_input_size(self, h, w):
+        """Run the following forwards on [B, 3, h, w] images (for a heads-only plan: h x w feature maps).  The tensors
+        and head outputs take the sizes a net compiled at h x w has (`tensor_shapes`, heads[i]['h'], ['w']); taps and
+        head views cover that size.  A size above the capacity in any tensor, or one that empties a layer, raises
+        RuntimeError and leaves the previous size in force.  A forward still running keeps its own size; the head
+        outputs it writes are reused by the next forward as before."""
+        h, w = int(h), int(w)
+        if (h, w) == self._input_size:
+            return
+        if not (1 <= h <= self.in_h and 1 <= w <= self.in_w):
+            raise RuntimeError(f'input size {h}x{w}: outside 1x1 .. the capacity {self.in_h}x{self.in_w}')
+        shapes = tensor_shapes_at(self.op_desc, self.capacity_shapes, h, w)
+        table = np.ascontiguousarray([hw for s in shapes for hw in s[:2]], dtype=np.int32)
+        _lib.check(self.lib.pifpaf_net_set_input_size(self.handle, h, w, len(shapes), _ptr(table)))
+        self.tensor_shapes, self._input_size = shapes, (h, w)
+        self.flops_per_image = float(self.lib.pifpaf_net_flops_per_image(self.handle))
+        for i, hd in enumerate(self.heads):
+            hh, ww = ctypes.c_int32(), ctypes.c_int32()
+            _lib.check(self.lib.pifpaf_net_head_output(self.handle, i, None, None, None, ctypes.byref(hh),
+                                                       ctypes.byref(ww)))
+            hd['h'], hd['w'] = hh.value, ww.value
 
     def __del__(self):
         self.close()
@@ -1019,8 +1097,8 @@ class CompiledNet:
         (valid until the next forward)."""
         if not image_batch.is_cuda or image_batch.dtype != torch.float32:
             raise RuntimeError('image_batch must be a float32 CUDA tensor')
-        if image_batch.dim() != 4 or image_batch.shape[1] != 3 or tuple(image_batch.shape[2:]) != (self.in_h, self.in_w):
-            raise RuntimeError(f'expected [B,3,{self.in_h},{self.in_w}]')
+        if image_batch.dim() != 4 or image_batch.shape[1] != 3 or tuple(image_batch.shape[2:]) != self._input_size:
+            raise RuntimeError('expected [B,3,{},{}]'.format(*self._input_size))
         b = int(image_batch.shape[0])
         if b > self.max_batch:
             raise RuntimeError('batch exceeds max_batch')
@@ -1069,8 +1147,8 @@ class CompiledNet:
         equals forward() on the normalised float batch bit for bit."""
         if not image_batch.is_cuda or image_batch.dtype != torch.uint8:
             raise RuntimeError('image_batch must be a uint8 CUDA tensor')
-        if image_batch.dim() != 4 or image_batch.shape[3] != 3 or tuple(image_batch.shape[1:3]) != (self.in_h, self.in_w):
-            raise RuntimeError(f'expected [B,{self.in_h},{self.in_w},3]')
+        if image_batch.dim() != 4 or image_batch.shape[3] != 3 or tuple(image_batch.shape[1:3]) != self._input_size:
+            raise RuntimeError('expected [B,{},{},3]'.format(*self._input_size))
         b = int(image_batch.shape[0])
         if b > self.max_batch:
             raise RuntimeError('batch exceeds max_batch')

@@ -12,8 +12,10 @@ batch is decoded by one batched launch sequence; only the final annotations
 on its own stream (on SMs the forward's persistent grids leave free) under the
 forward of batch i+1; the head outputs are double buffered for that.
 """
+import math
 import time
 
+import numpy as np
 import torch
 
 from . import decoder as _decoder
@@ -29,6 +31,22 @@ def raw_image_chunks(images, max_batch, fill):
         raise RuntimeError(f'fill has {len(fill)} colours for {len(images)} images')
     for i in range(0, len(images), max_batch):
         yield images[i:i + max_batch], fill[i:i + max_batch] if isinstance(fill, list) else fill
+
+
+def tight_pad_groups(sizes, long_edge, max_batch, capacity, multiple=16):
+    """The batches of `Predictor.raw_images(tight_pad=True)`: images (w, h) go through RescaleAbsolute(long_edge) (none
+    when long_edge is None) and CenterPadTight(multiple) (transforms/pad.py:62-110), whose canvas depends on the aspect
+    ratio.  Returns [((canvas_h, canvas_w), [image indices])] in order of each canvas's first image, every list in input
+    order and at most max_batch long.  A canvas above capacity (h, w) raises RuntimeError."""
+    groups = {}
+    for i, (w, h) in enumerate(sizes):
+        tw, th = _preprocess.rescale_target(w, h, long_edge) if long_edge else (w, h)
+        canvas = (math.ceil((th - 1) / multiple) * multiple + 1, math.ceil((tw - 1) / multiple) * multiple + 1)
+        if canvas[0] > capacity[0] or canvas[1] > capacity[1]:
+            raise RuntimeError(f'image {i} ({w}x{h}) pads to a {canvas[1]}x{canvas[0]} canvas, above the net\'s '
+                               f'{capacity[1]}x{capacity[0]}')
+        groups.setdefault(canvas, []).append(i)
+    return [(canvas, idx[k:k + max_batch]) for canvas, idx in groups.items() for k in range(0, len(idx), max_batch)]
 
 
 class Predictor:
@@ -159,7 +177,7 @@ class Predictor:
         return result
 
     def raw_images(self, images, *, json_data=False, fill=None, score_weights=None, fast_rescaling=True,
-                   opencv_rescaling=False):
+                   opencv_rescaling=False, tight_pad=False, long_edge=None):
         """The reference's Predictor.numpy_images / images (predictor.py:155-196) for a list of RAW uint8 [h, w, 3]
         images with everything after the JPEG decode on the GPU: RescaleAbsolute(long edge = the compiled input size)
         + CenterPad (`preprocess.GpuPreprocess`, bit-identical to the reference's Pillow path), ToTensor + Normalize in
@@ -170,8 +188,18 @@ class Predictor:
         opencv_rescaling: True rescales like cv2.resize(INTER_LINEAR), which the reference's fast rescale uses when
         OpenCV is importable (`GpuPreprocess(opencv=True)`); with fast_rescaling=False scipy is used either way, as in
         the reference.
-        Returns per image (data [N, K, 3] (x, y, v) in original-image pixels, joint_scales [N, K], meta) or, with
-        json_data, (list of dicts, meta)."""
+        tight_pad: pad like the reference's Predictor at batch size 1 instead: RescaleAbsolute(long_edge) (no rescale
+        with long_edge None, the reference's default) + CenterPadTight(16), the pad colour (124, 116, 104) unless `fill`
+        says otherwise.  Images are grouped by canvas into batches of at most max_batch, each group runs at its canvas
+        size on this one net (`CompiledNet.set_input_size`) and is decoded at its field size; a canvas larger than the
+        net's input raises RuntimeError before anything is enqueued.
+        Returns per image, in input order, (data [N, K, 3] (x, y, v) in original-image pixels, joint_scales [N, K],
+        meta) or, with json_data, (list of dicts, meta)."""
+        if tight_pad:
+            return self._tight_pad_images(images, json_data, fill, score_weights, fast_rescaling, opencv_rescaling,
+                                          long_edge)
+        if long_edge is not None:
+            raise RuntimeError('long_edge applies to tight_pad=True; the square canvas is the net\'s input size')
         if self.net.in_h != self.net.in_w:
             raise RuntimeError('raw_images needs a net compiled for a square input (CenterPad(long_edge))')
         if getattr(self, '_gpu_preprocess', None) is None:
@@ -188,21 +216,57 @@ class Predictor:
                 self.batch_device(canvas)
                 result = self.decoder.fetch(stream=self.result_stream())
                 self.join()
-            for (ann, _), meta in zip(result, metas):
-                data, scales = _preprocess.inverse_transform_batch(ann.numpy(), meta)
-                if json_data:
-                    out.append((_preprocess.json_data_batch(data, scales, score_weights=score_weights), meta))
-                else:
-                    out.append((data, scales, meta))
+            out += [self._result(ann, meta, json_data, score_weights) for (ann, _), meta in zip(result, metas)]
+        return out
+
+    @staticmethod
+    def _result(ann, meta, json_data, score_weights):
+        data, scales = _preprocess.inverse_transform_batch(ann.numpy(), meta)
+        if json_data:
+            return _preprocess.json_data_batch(data, scales, score_weights=score_weights), meta
+        return data, scales, meta
+
+    def _tight_pad_images(self, images, json_data, fill, score_weights, fast_rescaling, opencv_rescaling, long_edge):
+        """raw_images(tight_pad=True): one GpuPreprocess(batched=False) call, forward and decode per canvas group; the
+        net's input size is restored afterwards"""
+        sizes = []
+        for im in images:
+            if im.dtype not in (np.uint8, torch.uint8) or len(im.shape) != 3 or im.shape[2] != 3:
+                raise RuntimeError('images must be uint8 [h, w, 3]')
+            sizes.append((int(im.shape[1]), int(im.shape[0])))
+        groups = tight_pad_groups(sizes, long_edge, self.net.max_batch, (self.net.in_h, self.net.in_w))
+        fills = _preprocess.pad_fills(fill, len(images), False)
+        key = ('tight', long_edge, bool(fast_rescaling), bool(fast_rescaling) and bool(opencv_rescaling))
+        if getattr(self, '_gpu_preprocess', None) is None:
+            self._gpu_preprocess = {}
+        if key not in self._gpu_preprocess:
+            self._gpu_preprocess[key] = _preprocess.GpuPreprocess(long_edge, batched=False, fast_rescaling=key[2],
+                                                                  opencv=key[3], device=self.device.index)
+        preprocess = self._gpu_preprocess[key]
+        out = [None] * len(images)
+        restore = self.net.input_size
+        try:
+            for canvas_hw, idx in groups:
+                self.net.set_input_size(*canvas_hw)
+                with torch.cuda.stream(self.stream):
+                    canvas, metas = preprocess([images[i] for i in idx], fill=[fills[i] for i in idx],
+                                               stream=self.stream)
+                    self.batch_device(canvas)
+                    result = self.decoder.fetch(stream=self.result_stream())
+                    self.join()
+                for i, (ann, _), meta in zip(idx, result, metas):
+                    out[i] = self._result(ann, meta, json_data, score_weights)
+        finally:
+            self.net.set_input_size(*restore)
         return out
 
     def jpeg_images(self, files_or_bytes, *, json_data=False, fill=None, score_weights=None, fast_rescaling=True,
-                    opencv_rescaling=False):
+                    opencv_rescaling=False, tight_pad=False, long_edge=None):
         """`raw_images` of the JPEG files (paths or bytes) decoded like the reference's Predictor.images
         (PIL.Image.open(f).convert('RGB'), datasets/image_list.py:18), but on the GPU (`preprocess.GpuJpegDecoder`;
         streams it does not decode are decoded by Pillow).  Chunked by max_batch; each chunk's decode is enqueued on
-        the predictor's stream ahead of its resize (fast_rescaling and opencv_rescaling as for raw_images).  Returns
-        what raw_images returns, per file."""
+        the predictor's stream ahead of its resize (fast_rescaling, opencv_rescaling, tight_pad and long_edge as for
+        raw_images).  Returns what raw_images returns, per file."""
         files = list(files_or_bytes)
         if isinstance(fill, list) and len(fill) != len(files):
             raise RuntimeError(f'fill has {len(fill)} colours for {len(files)} images')
@@ -212,7 +276,8 @@ class Predictor:
             dec = self._jpeg_decoder(datas)
             images, _ = dec(datas, stream=self.stream, host_pillow=True)
             out.extend(self.raw_images(images, json_data=json_data, fill=chunk_fill, score_weights=score_weights,
-                                       fast_rescaling=fast_rescaling, opencv_rescaling=opencv_rescaling))
+                                       fast_rescaling=fast_rescaling, opencv_rescaling=opencv_rescaling,
+                                       tight_pad=tight_pad, long_edge=long_edge))
         return out
 
     def _jpeg_decoder(self, datas):
