@@ -266,3 +266,145 @@ def test_op_ref_bounds_hold_for_the_bf16_emulation(name, layout, fuse):
         assert r <= 1.0, (i, kind, r)
         kinds.add(kind)
     print(name, sorted(kinds))
+
+
+def _emulated(name, layout=None, fuse=None, u8=False, H=49, W=65, B=2):
+    """build_ops of an emulation plan and its bf16 emulation (ops_emulator.run_ops) on seeded images; u8: the images
+    are raw uint8 ones normalised as the uint8 stem does (kernel_refs.normalise_u8)"""
+    import ops_emulator
+    kw = {} if layout is None else {'layout': layout, 'fuse_dw': fuse}
+    tensors, ops, _ = network.build_ops(_emulation_plan(name), H, W, **kw)
+    rng = np.random.default_rng(1)
+    if u8:
+        raw = rng.integers(0, 256, (B, H, W, 3), dtype=np.uint8)
+        images = np.ascontiguousarray(
+            kr.normalise_u8(raw, network.CompiledNet.IMAGE_MEAN, network.CompiledNet.IMAGE_STD).transpose(0, 3, 1, 2))
+    else:
+        images = rng.standard_normal((B, 3, H, W)).astype(np.float32)
+    heads, acts = ops_emulator.run_ops(tensors, ops, torch.from_numpy(images), bf16=True)
+    return tensors, ops, {t: a.numpy() for t, a in enumerate(acts)}, [h.numpy() for h in heads], images
+
+
+def _at(a, pos, heads=False):
+    """a full-size op_terms array at positions: [B, h, w, C] -> [P, C]; head outputs [B, F, comp, h, w] -> [P, F, comp]"""
+    return a[pos[:, 0], :, :, pos[:, 1], pos[:, 2]] if heads else a[pos[:, 0], pos[:, 1], pos[:, 2]]
+
+
+@pytest.mark.parametrize('name,layout,fuse,u8', [
+    ('dil2_conv5stage', 'bins', True, False), ('conv2_dil2', 'shuffle', False, False), ('cocodet', None, None, False),
+    ('pool2', None, None, True), ('dil4', None, None, False), ('mobilenetv2', None, None, True)])
+def test_sampled_op_terms_equal_the_full_reference(name, layout, fuse, u8):
+    """op_terms at sample_positions (every op kind, float and uint8-normalised stems) is the full reference, bound and
+    output restricted to those positions"""
+    tensors, ops, taps, heads, images = _emulated(name, layout, fuse, u8)
+    kinds = set()
+    for i, o in enumerate(ops):
+        pos = kr.op_positions(o, tensors, 2, seed=i, n_random=64)
+        kind, full = kr.op_terms(o, taps, heads, images, 2)
+        kind_s, sampled = kr.op_terms(o, taps, heads, images, 2, positions=pos)
+        assert kind_s == kind and len(sampled) == len(full)
+        for (g, r, bd), (gs, rs, bds) in zip(full, sampled):
+            assert np.array_equal(_at(g, pos, kind == 'heads'), gs), (i, kind)
+            np.testing.assert_allclose(rs, _at(r, pos, kind == 'heads'), rtol=1e-12, atol=1e-12, err_msg=f'{i} {kind}')
+            if bd is None:
+                assert bds is None
+            else:
+                np.testing.assert_allclose(bds, _at(bd, pos, kind == 'heads'), rtol=1e-12, atol=1e-15)
+        assert kr.op_ref(o, taps, heads, images, 2, positions=pos)[1] <= 1.0, (i, kind)
+        kinds.add(kind)
+    print(name, sorted(kinds))
+
+
+def test_sampled_op_kinds_cover_every_kind():
+    """the plans above reach every label op_terms gives: each sampled path was compared"""
+    kinds = set()
+    for name, layout, fuse in (('dil2_conv5stage', 'bins', True), ('conv2_dil2', 'shuffle', False),
+                               ('cocodet', None, None), ('pool2', None, None), ('dil4', None, None),
+                               ('mobilenetv2', None, None)):
+        kw = {} if layout is None else {'layout': layout, 'fuse_dw': fuse}
+        _, ops, _ = network.build_ops(_emulation_plan(name), 49, 65, **kw)
+        for o in ops:
+            kinds.add(o['kind'] + ('-pieces' if 'pieces' in o else '') + ('-shuffle' if o.get('shuffle_src', -1) >= 0 else '')
+                      + ('-res' if o.get('residual', -1) >= 0 else '') + ('-dil' if o.get('dilation', 1) > 1 else '')
+                      + ('-up' if o.get('upsample', 1) > 1 else ''))
+    want = {'input_conv', 'conv', 'conv-res', 'conv-dil', 'conv1x1', 'conv1x1-pieces', 'conv1x1-shuffle', 'dwconv',
+            'dwconv-dil', 'dw_conv1x1-pieces', 'maxpool', 'heads', 'heads-up'}
+    assert want <= kinds, want - kinds
+
+
+def _defect_case():
+    """the emulated mobilenetv2 and its first plain implicit-GEMM conv with an output of at least 16 x 32 pixels"""
+    tensors, ops, taps, heads, images = _emulated('mobilenetv2', H=65, W=129)
+    i = next(i for i, o in enumerate(ops) if o['kind'] == 'conv' and tensors[o['out']][0] >= 16
+             and tensors[o['out']][1] >= 32)
+    return tensors, ops, taps, heads, images, i
+
+
+@pytest.mark.parametrize('where', ['last pixel', 'tile corner', 'crossing row'])
+def test_sampled_reference_reports_one_wrong_value(where):
+    """a single wrong value in the emulated output of one op is reported (ratio > 1) by the sampled reference without
+    any random positions: at the last pixel of the last image, at a corner of an 8 x 16 tile of the last image, and at
+    the pixel row holding a (here synthetic) 32-bit offset crossing of the output"""
+    tensors, ops, taps, heads, images, i = _defect_case()
+    o = ops[i]
+    B = 2
+    Ho, Wo, c = tensors[o['out']]
+    limits = kr.BYTE_LIMITS
+    if where == 'last pixel':
+        b, y, x = B - 1, Ho - 1, Wo - 1
+    elif where == 'tile corner':
+        b, y, x = B - 1, 2 * kr.TILE[0] - 1, kr.TILE[1]        # bottom-left corner of the second tile row's 2nd tile
+    else:
+        m = (B * Ho * Wo) * 3 // 5 + 7                           # an interior pixel no other class selects
+        b, y, x = m // (Ho * Wo), m // Wo % Ho, m % Wo
+        limits = (m * 2 * c + c,)                                # a byte limit inside that pixel row
+    pos = kr.op_positions(o, tensors, B, seed=0, n_random=0, limits=limits)
+    assert kr.op_ref(o, taps, heads, images, B, positions=pos)[1] <= 1.0
+    if where == 'crossing row':
+        clean = kr.op_positions(o, tensors, B, seed=0, n_random=0)
+        assert not ((clean == (b, y, x)).all(1)).any(), 'the crossing row alone must select the pixel'
+    bad = dict(taps)
+    bad[o['out']] = taps[o['out']].copy()
+    v = bad[o['out']][b, y, x, o['n_out'] // 2]
+    bad[o['out']][b, y, x, o['n_out'] // 2] = v + 1.0 + 0.25 * abs(v)      # far outside the bound at any magnitude
+    kind, r = kr.op_ref(o, bad, heads, images, B, positions=pos)
+    assert r > 1.0, (where, kind, r)
+
+
+def test_sample_positions_hold_every_class():
+    """the benchmark's stage-2 entry: t_c (64 x 321 x 321 x 192 bf16 = 2 532 335 616 B) written by a 1x1 GEMM and read
+    by the stride-2 depthwise 5x5; both ops' positions hold the pixels around byte 2^31 (row 5 592 405, image 54)"""
+    import bench
+    cfg = bench.CONFIGS['C0']
+    tensors, ops, _ = network.build_ops(bench.make_plan(cfg), 641, 641)
+    B = 64
+    big = [t for t, (h, w, c) in enumerate(tensors) if B * h * w * c * 2 > 2 ** 31]
+    assert len(big) == 1 and tensors[big[0]] == (321, 321, 192)
+    assert kr.crossing_rows(B * 321 * 321, 192) == [5592405]
+    writer = next(o for o in ops if o.get('out') == big[0] and o['kind'] == 'conv1x1')
+    reader = next(o for o in ops if o.get('in') == big[0])
+    assert reader['kind'] == 'dwconv' and reader['stride'] == 2 and reader['kernel'] == 5
+    pw = kr.op_positions(writer, tensors, B, seed=1)
+    dw = kr.op_positions(reader, tensors, B, seed=2)
+
+    def has(pos, pts):
+        s = {tuple(p) for p in pos.tolist()}
+        return all(tuple(p) in s for p in pts)
+    assert has(pw, [(m // 321 ** 2, m // 321 % 321, m % 321) for m in range(5592403, 5592408)])
+    assert (54, 87, 264) == (5592405 // 321 ** 2, 5592405 // 321 % 321, 5592405 % 321)
+    # outputs oy 43..44 / ox 131..133 of the stride-2 window (pad 2) cover input pixel (87, 264)
+    assert has(dw, [(54, y, x) for y in (43, 44) for x in (131, 132, 133)])
+    for pos, (Ho, Wo) in ((pw, (321, 321)), (dw, (161, 161))):
+        M = B * Ho * Wo
+        assert (pos[:, 0] < B).all() and (pos[:, 1] < Ho).all() and (pos[:, 2] < Wo).all()
+        edge = [(b, r, x) for b in (0, B - 1) for r in (0, 1, Ho - 2, Ho - 1) for x in range(Wo)]
+        edge += [(b, y, c) for b in (0, B - 1) for c in (0, 1, Wo - 2, Wo - 1) for y in range(Ho)]
+        corners = [(B - 1, y, x) for y0 in range(0, Ho, 8) for x0 in range(0, Wo, 16)
+                   for y in (y0, min(y0 + 7, Ho - 1)) for x in (x0, min(x0 + 15, Wo - 1))]
+        n_t = (M + 127) // 128
+        rows = [min(t * 128 + r, M - 1) for t in (0, 1, 2, n_t - 3, n_t - 2, n_t - 1) for r in (0, 127)] + [M - 1]
+        assert has(pos, edge) and has(pos, corners)
+        assert has(pos, [(m // (Ho * Wo), m // Wo % Ho, m % Wo) for m in rows])
+        structured = len({*edge, *corners})
+        assert structured + 3500 < len(pos) < structured + 4200, len(pos)      # ~4096 random ones besides
+        print('positions', Ho, Wo, len(pos))
