@@ -407,9 +407,17 @@ int pifpaf_net_conv_dilated(pifpaf_net_t* net, int32_t in_tensor, int32_t in_col
 
 /* 3x3 max pool, padding 1, stride 1 or 2 (torchvision ResNet's MaxPool2d(3, 2, 1) kept by --resnet-pool0-stride,
  * basenetworks.py:85-93) on channels [in_col_off, in_col_off + channels) of in_tensor; taps outside the image are
- * ignored (torch pads with -inf).  forward_timed reports it as op kind 4. */
+ * ignored (torch pads with -inf).  forward_timed reports it as op kind 4.  pifpaf_net_maxpool is
+ * pifpaf_net_maxpool_ceil with ceil_mode 0. */
 int pifpaf_net_maxpool(pifpaf_net_t* net, int32_t in_tensor, int32_t in_col_off, int32_t channels, int32_t stride,
                        int32_t out_tensor, int32_t out_col_off);
+
+/* pifpaf_net_maxpool with torch's ceil_mode (SqueezeNet 1.1's MaxPool2d(3, 2, ceil_mode=True), whose padding the
+ * reference sets to 1, basenetworks.py:461-499): ceil_mode 1 sizes the output ceil((H + 2 - 3) / stride) + 1, minus 1
+ * when the last window would start at or beyond H + 1 (likewise wide); ceil_mode 0 is the floor rule.  Any other
+ * value is PIFPAF_E_ARG. */
+int pifpaf_net_maxpool_ceil(pifpaf_net_t* net, int32_t in_tensor, int32_t in_col_off, int32_t channels,
+                            int32_t stride, int32_t out_tensor, int32_t out_col_off, int32_t ceil_mode);
 
 /* Depthwise kxk conv (basenetworks.py:228-231; torchvision InvertedResidual), weight [channels][k][k], + bias
  * (folded BN), activation code `relu`.  k = 5 and k = 3 with stride 1 or 2 run the TMA-fed kernel; other shapes, and

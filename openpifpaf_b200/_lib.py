@@ -105,6 +105,7 @@ SYMBOLS = {
     'pifpaf_net_conv_dilated': (ctypes.c_int, [VP, c_i32, c_i32, c_i32, c_i32, c_i32, c_i32, c_i32, VP, VP, c_i32, c_i32,
                                                c_i32, c_i32, c_i32, c_i32]),
     'pifpaf_net_maxpool': (ctypes.c_int, [VP, c_i32, c_i32, c_i32, c_i32, c_i32, c_i32]),
+    'pifpaf_net_maxpool_ceil': (ctypes.c_int, [VP, c_i32, c_i32, c_i32, c_i32, c_i32, c_i32, c_i32]),
     'pifpaf_net_dwconv': (ctypes.c_int, [VP, c_i32, c_i32, c_i32, c_i32, c_i32, c_i32, VP, VP, c_i32, c_i32, c_i32]),
     'pifpaf_net_dwconv_dilated': (ctypes.c_int, [VP, c_i32, c_i32, c_i32, c_i32, c_i32, c_i32, VP, VP, c_i32, c_i32,
                                                  c_i32, c_i32]),

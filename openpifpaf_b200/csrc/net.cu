@@ -1135,8 +1135,11 @@ using DwS1K3 = DwTile<1, DW1_TH, DW1_TW, 4, 4, 3>;
 using DwS2K3 = DwTile<2, DW2_TH, DW2_TW, 4, 3, 3>;
 
 // 3x3 max pool, pad 1, stride a.stride (torchvision's MaxPool2d(3, 2, 1) in the ResNet input block,
-// basenetworks.py:85-93): one output pixel x 8 channels (one 16-byte vector) per thread.  Taps outside the image are
-// skipped, as torch's -inf padding does; the centre tap is always inside.  The weight / bias fields of DwArgs are unused.
+// basenetworks.py:85-93, and the ceil-mode pools of SqueezeNet 1.1, basenetworks.py:461-499): one output pixel x 8
+// channels (one 16-byte vector) per thread.  Taps outside the image are skipped, as torch's -inf padding does; every
+// window starts inside the image's last column (row) or before it -- in ceil mode too, whose last window may end two
+// taps past the image (conv_out drops a window that would not) -- so it has a tap inside.  The weight / bias fields
+// of DwArgs are unused.
 __global__ void __launch_bounds__(256) k_maxpool(DwArgs a) {
     pdl_launch_dependents();
     pdl_wait();
@@ -1909,6 +1912,7 @@ struct Op {
     const DwTmaVariant* dw_tma = nullptr;     // TMA route of a depthwise op (choose_dw_kernels; nullptr: none)
     void (*dw_simt5)(DwArgs) = nullptr;       // its SIMT route: k_dwconv5<S> (nullptr: k_dwconv)
     int dw_dil = 1;                           // depthwise tap spacing (> 1: DW_K5_S1_D2 or k_dwconv)
+    bool pool_ceil = false;                   // max pool: output size by the ceil_mode rule (conv_out)
     // fused depthwise -> GEMM (OP_FUSED): g + tmap_dw (windows) + tmap_b
     FusedArgs fu{};
     // input conv
@@ -2212,10 +2216,14 @@ void choose_dw_kernels(const pifpaf_net* net, Op& op) {
 }
 
 // output rows (or columns) of a window of `kernel` taps `dil` apart, moved by `stride`, over n input rows zero padded
-// by `pad` on both sides; 0 where the window does not fit (an empty layer)
-inline int conv_out(int n, int kernel, int stride, int pad, int dil) {
+// by `pad` on both sides; 0 where the window does not fit (an empty layer).  ceil_mode: PyTorch's pooling rule -- the
+// division rounds up, and a last window that would start at or beyond n + pad (in the right padding) is dropped
+inline int conv_out(int n, int kernel, int stride, int pad, int dil, bool ceil_mode = false) {
     const int span = dil * (kernel - 1) + 1;
-    return n + 2 * pad < span ? 0 : (n + 2 * pad - span) / stride + 1;
+    if (n + 2 * pad < span) return 0;
+    if (!ceil_mode) return (n + 2 * pad - span) / stride + 1;
+    const int out = (n + 2 * pad - span + stride - 1) / stride + 1;
+    return (out - 1) * stride >= n + pad ? out - 1 : out;
 }
 
 // the output size of an op on an hin x win input (the stem's input: the image).  1x1 GEMMs, the fused depthwise ->
@@ -2225,8 +2233,8 @@ void op_out_hw(const Op& op, int hin, int win, int* ho, int* wo) {
     if (op.kind == OP_INPUT_CONV) { k = op.ic.kernel; s = op.ic.stride; p = op.ic.pad; }
     else if (op.kind == OP_DW || op.kind == OP_MAXPOOL) { k = op.dw.kernel; s = op.dw.stride; p = op.dw.pad; d = op.dw_dil; }
     else if (op.g.conv_k > 0) { k = op.g.conv_k; s = op.g.conv_stride; p = op.g.conv_pad; d = op.g.conv_dil; }
-    *ho = conv_out(hin, k, s, p, d);
-    *wo = conv_out(win, k, s, p, d);
+    *ho = conv_out(hin, k, s, p, d, op.pool_ceil);
+    *wo = conv_out(win, k, s, p, d, op.pool_ceil);
 }
 
 // The size-dependent part of an op, from the current h x w of its input tensor (the stem: net->in_h x in_w): the
@@ -2773,14 +2781,20 @@ int pifpaf_net_dwconv_dilated(pifpaf_net_t* net, int32_t in_tensor, int32_t in_c
 
 int pifpaf_net_maxpool(pifpaf_net_t* net, int32_t in_tensor, int32_t in_col_off, int32_t channels, int32_t stride,
                        int32_t out_tensor, int32_t out_col_off) {
+    return pifpaf_net_maxpool_ceil(net, in_tensor, in_col_off, channels, stride, out_tensor, out_col_off, 0);
+}
+
+int pifpaf_net_maxpool_ceil(pifpaf_net_t* net, int32_t in_tensor, int32_t in_col_off, int32_t channels, int32_t stride,
+                            int32_t out_tensor, int32_t out_col_off, int32_t ceil_mode) {
     PIFPAF_CHECK_ARG(net != nullptr, "null argument");
     const int nt = (int)net->tensors.size();
     PIFPAF_CHECK_ARG(in_tensor >= 0 && in_tensor < nt && out_tensor >= 0 && out_tensor < nt, "bad tensor id");
     PIFPAF_CHECK_ARG(stride == 1 || stride == 2, "max pool stride must be 1 or 2");
+    PIFPAF_CHECK_ARG(ceil_mode == 0 || ceil_mode == 1, "max pool ceil_mode must be 0 or 1");
     PIFPAF_CHECK_ARG(channels >= 1, "bad channel count");
     const Tensor& tin = net->tensors[in_tensor];
     const Tensor& to = net->tensors[out_tensor];
-    const int ho = conv_out(tin.h, 3, stride, 1, 1), wo = conv_out(tin.w, 3, stride, 1, 1);
+    const int ho = conv_out(tin.h, 3, stride, 1, 1, ceil_mode), wo = conv_out(tin.w, 3, stride, 1, 1, ceil_mode);
     const int C = pad8(channels);
     PIFPAF_CHECK_ARG(to.h == ho && to.w == wo, "max pool output tensor shape mismatch");
     PIFPAF_CHECK_ARG(in_col_off % 8 == 0 && out_col_off % 8 == 0 && in_col_off + C <= tin.c && out_col_off + C <= to.c,
@@ -2791,6 +2805,7 @@ int pifpaf_net_maxpool(pifpaf_net_t* net, int32_t in_tensor, int32_t in_col_off,
     a.out = to.data; a.ld_out = to.c; a.out_col_off = out_col_off;
     a.C8 = C / 8;
     a.kernel = 3; a.stride = stride; a.pad = 1; a.relu = 0;
+    op.pool_ceil = ceil_mode != 0;
     op.a_tensor = in_tensor; op.c_real = channels;
     const int rc = op_geometry(net, op);
     if (rc != PIFPAF_OK) return rc;

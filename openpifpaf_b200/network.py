@@ -4,6 +4,8 @@ Reference (paths relative to the reference's src/openpifpaf/):
   Shell.forward                       network/nets.py:35-48
   ShuffleNetV2K / InvertedResidualK   network/basenetworks.py:186-355
   MobileNetV2 (torchvision features)  network/basenetworks.py:407-417
+  ShuffleNetV2 (torchvision x1 / x2)  network/basenetworks.py:36-68
+  SqueezeNet (torchvision 1.1)        network/basenetworks.py:461-499
   CompositeField4 (eval)              network/heads.py:330-378
 
 `plan_from_shell(shell)` walks a reference-style ``Shell`` (duck-typed: the
@@ -59,8 +61,12 @@ class UnsupportedModel(RuntimeError):
 
 
 def _fold(conv, bn):
-    """conv (bias-free) followed by eval BatchNorm -> (weight, bias) float32 numpy."""
+    """conv (bias-free) followed by eval BatchNorm -> (weight, bias) float32 numpy.  bn None: the conv alone, its bias
+    (zero without one) as the bias (SqueezeNet's convs have biases and no BatchNorm)."""
     w = conv.weight.detach().double()
+    if bn is None:
+        b = conv.bias.detach().double() if conv.bias is not None else torch.zeros(w.shape[0], dtype=torch.float64)
+        return w.float().cpu().numpy(), b.float().cpu().numpy()
     scale = bn.weight.detach().double() / torch.sqrt(bn.running_var.detach().double() + bn.eps)
     b = bn.bias.detach().double() - bn.running_mean.detach().double() * scale
     if conv.bias is not None:
@@ -236,8 +242,99 @@ def _plan_from_mobilenetv2(shell):
     return {'kind': 'mobilenetv2', 'input': stem, 'blocks': blocks, 'last': last, 'heads': _heads_plan(shell, base)}
 
 
+def _conv_bn_relu(m, what, kernel, stride, pad):
+    """a Sequential of Conv2d (kernel, stride, pad, groups 1) + BatchNorm2d + ReLU -> (conv, bn)"""
+    parts = list(m) if isinstance(m, torch.nn.Sequential) else []
+    if len(parts) != 3 or not isinstance(parts[0], torch.nn.Conv2d) or not isinstance(parts[1], torch.nn.BatchNorm2d) \
+            or not isinstance(parts[2], torch.nn.ReLU):
+        raise UnsupportedModel(f'ShuffleNetV2 {what}: expected Conv2d + BatchNorm2d + ReLU')
+    c = parts[0]
+    if (_pair(c.kernel_size), _pair(c.stride), _pair(c.padding), _pair(c.dilation), c.groups) != \
+            ((kernel, kernel), (stride, stride), (pad, pad), (1, 1), 1):
+        raise UnsupportedModel(f'ShuffleNetV2 {what}: unsupported conv {c}')
+    return parts[0], parts[1]
+
+
+def _plan_from_shufflenetv2(shell):
+    """basenetworks.py:36-68: torchvision's ShuffleNetV2 (x1 / x2) without its max pool -- conv1 (3x3 stride-2 conv +
+    BN + ReLU), stages 2-4 of torchvision InvertedResidual blocks (InvertedResidualK with 3x3 depthwise convs and the
+    same Sequential indices; a stride-1 block has an empty branch1) and conv5 (1x1 conv + BN + ReLU); stride 16.  The
+    plan is a ShuffleNetV2K plan, so it takes that lowering."""
+    base = shell.base_net
+    conv, bn = _conv_bn_relu(base.conv1, 'conv1', 3, 2, 1)
+    if conv.in_channels != 3:
+        raise UnsupportedModel('ShuffleNetV2 conv1: expected 3 input channels')
+    plan = {'kind': 'shufflenetv2k', 'input': _fold_stem(conv, bn), 'stages': [], 'heads': []}
+    for stage in (base.stage2, base.stage3, base.stage4):
+        plan['stages'].append([_shufflenetv2k_block(blk) for blk in stage])
+    plan['conv5'] = _fold(*_conv_bn_relu(base.conv5, 'conv5', 1, 1, 0))
+    plan['heads'] = _heads_plan(shell, base)
+    return plan
+
+
+def _is_fire(m):
+    return all(hasattr(m, a) for a in ('squeeze', 'expand1x1', 'expand3x3'))
+
+
+def _squeezenet_conv(conv, act, what, kernel):
+    """one conv of a Fire module (or the stem) with its activation: stride 1 (the stem: 2), padding (kernel - 1) // 2 as
+    the reference sets it, groups 1, a ReLU, and a width the column windows of the lowering can hold"""
+    stride = 2 if what == 'stem' else 1
+    if not isinstance(conv, torch.nn.Conv2d) or (_pair(conv.kernel_size), _pair(conv.stride), _pair(conv.padding),
+                                                 _pair(conv.dilation)) != \
+            ((kernel, kernel), (stride, stride), ((kernel - 1) // 2,) * 2, (1, 1)):
+        raise UnsupportedModel(f'SqueezeNet {what}: unsupported conv {conv}')
+    if conv.groups != 1:
+        raise UnsupportedModel(f'SqueezeNet {what}: grouped convolutions are not supported')
+    if not isinstance(act, torch.nn.ReLU):
+        raise UnsupportedModel(f'SqueezeNet {what}: expected a ReLU, got {type(act).__name__}')
+    # the expand pair writes one tensor through two column windows that start at multiples of 8 channels
+    if conv.out_channels % 8 or (conv.in_channels % 8 and what != 'stem'):
+        raise UnsupportedModel(f'SqueezeNet {what}: widths must be multiples of 8, got {conv}')
+    w, b = _fold(conv, None)
+    return {'w': w, 'b': b, 'kernel': kernel, 'stride': stride, 'pad': (kernel - 1) // 2}
+
+
+def _plan_from_squeezenet(shell):
+    """basenetworks.py:461-499: base_net.backbone = torchvision squeezenet1_1().features with the reference's padding
+    edits -- the 3x3 stride-2 stem (pad 1) + ReLU, three 3x3 stride-2 max pools (pad 1, ceil_mode) and eight Fire
+    modules (squeeze 1x1 + ReLU, then cat(expand1x1 + ReLU, expand3x3 (pad 1) + ReLU)); convs with biases, no
+    BatchNorm; stride 16.  plan['layers'] holds {'type': 'pool', 'stride', 'ceil_mode'} and {'type': 'fire',
+    'squeeze', 'expand1x1', 'expand3x3'} in order."""
+    base = shell.base_net
+    mods = list(base.backbone)
+    if len(mods) < 3 or not isinstance(mods[0], torch.nn.Conv2d):
+        raise UnsupportedModel('SqueezeNet backbone: expected a stem conv + ReLU, then max pools and Fire modules')
+    stem = _squeezenet_conv(mods[0], mods[1], 'stem', 3)
+    if mods[0].in_channels != 3:
+        raise UnsupportedModel('SqueezeNet stem: expected 3 input channels')
+    layers = []
+    for i, m in enumerate(mods[2:], start=2):
+        what = f'backbone[{i}]'
+        if isinstance(m, torch.nn.MaxPool2d):
+            if (_pair(m.kernel_size), _pair(m.padding), _pair(m.dilation)) != ((3, 3), (1, 1), (1, 1)) or \
+                    _pair(m.stride) not in ((1, 1), (2, 2)):
+                raise UnsupportedModel(f'SqueezeNet {what}: only a 3x3 max pool with padding 1 and stride 1 or 2 is '
+                                       'supported')
+            layers.append({'type': 'pool', 'stride': int(_pair(m.stride)[0]), 'ceil_mode': bool(m.ceil_mode)})
+        elif _is_fire(m):
+            acts = [getattr(m, a, None) for a in ('squeeze_activation', 'expand1x1_activation', 'expand3x3_activation')]
+            layers.append({'type': 'fire', 'squeeze': _squeezenet_conv(m.squeeze, acts[0], f'{what}.squeeze', 1),
+                           'expand1x1': _squeezenet_conv(m.expand1x1, acts[1], f'{what}.expand1x1', 1),
+                           'expand3x3': _squeezenet_conv(m.expand3x3, acts[2], f'{what}.expand3x3', 3)})
+            # the expand3x3 half is written from column e1: pifpaf_net_conv starts an output window on a 16-channel
+            # (32-byte) boundary
+            if m.expand1x1.out_channels % 16:
+                raise UnsupportedModel(f'SqueezeNet {what}.expand1x1: the expand3x3 half would start at column '
+                                       f'{m.expand1x1.out_channels}, not a multiple of 16')
+        else:
+            raise UnsupportedModel(f'SqueezeNet {what}: expected a MaxPool2d or a Fire module, got {type(m).__name__}')
+    return {'kind': 'squeezenet', 'input': stem, 'layers': layers, 'heads': _heads_plan(shell, base)}
+
+
 def plan_from_shell(shell):
-    """Extract a folded plan from a reference-style Shell (ShuffleNetV2K, Resnet or MobileNetV2 base net)."""
+    """Extract a folded plan from a reference-style Shell (ShuffleNetV2K, Resnet, MobileNetV2, torchvision ShuffleNetV2
+    or SqueezeNet base net)."""
     base = shell.base_net
     if shell.training:
         raise UnsupportedModel('the Shell must be in eval() mode (BatchNorm is folded)')
@@ -251,8 +348,13 @@ def plan_from_shell(shell):
             raise UnsupportedModel(f'unsupported module in the base network: {type(m).__name__} (only ReLU + BatchNorm)')
     if all(hasattr(base, a) for a in ('input_block', 'block2', 'block3', 'block4', 'block5')):
         return _plan_from_resnet(shell)
+    # SqueezeNet keeps its layers in base.backbone as MobileNetV2 does: its Fire modules tell them apart
+    if isinstance(getattr(base, 'backbone', None), torch.nn.Sequential) and any(_is_fire(m) for m in base.backbone):
+        return _plan_from_squeezenet(shell)
     if isinstance(getattr(base, 'backbone', None), torch.nn.Sequential):
         return _plan_from_mobilenetv2(shell)
+    if all(hasattr(base, a) for a in ('conv1', 'stage2', 'stage3', 'stage4', 'conv5')):
+        return _plan_from_shufflenetv2(shell)
     if not all(hasattr(base, a) for a in ('input_block', 'stage2', 'stage3', 'stage4', 'conv5')):
         raise UnsupportedModel(f'unsupported base network {type(base).__name__}: expected ShuffleNetV2K, Resnet or '
                                'MobileNetV2')
@@ -260,11 +362,13 @@ def plan_from_shell(shell):
 
 
 def _shufflenetv2k_block(blk):
-    """one InvertedResidualK (basenetworks.py:186-242), folded; 'dilation' only where it is not 1
+    """one InvertedResidualK (basenetworks.py:186-242) or torchvision InvertedResidual (the same Sequential indices; its
+    stride-1 blocks have an empty branch1 where InvertedResidualK has None), folded; 'dilation' only where it is not 1
     (--shufflenetv2k-stage4-dilation, which the reference pairs with stride 1)"""
     b2 = blk.branch2
     dw = b2[3]
-    entry = {'first': blk.branch1 is not None, 'stride': int(dw.stride[0]),
+    first = blk.branch1 is not None and len(blk.branch1) > 0
+    entry = {'first': first, 'stride': int(dw.stride[0]),
              'kernel': int(dw.kernel_size[0]), 'pad': int(dw.padding[0])}
     if dw.dilation[0] != 1:
         if entry['stride'] != 1:
@@ -273,7 +377,7 @@ def _shufflenetv2k_block(blk):
     entry['b2_pw1'] = _fold(b2[0], b2[1])
     entry['b2_dw'] = _fold(b2[3], b2[4])
     entry['b2_pw2'] = _fold(b2[5], b2[6])
-    if blk.branch1 is not None:
+    if first:
         entry['b1_dw'] = _fold(blk.branch1[0], blk.branch1[1])
         entry['b1_pw'] = _fold(blk.branch1[2], blk.branch1[3])
     return entry
@@ -651,11 +755,19 @@ def _dw_rows(wb, kernel, width, cols=None):
     return wp, bp
 
 
-def conv_out_hw(h, w, kernel, stride, pad, dilation=1):
-    """Output size of a conv window (torch.nn.Conv2d / MaxPool2d without ceil_mode) on an h x w input; a size < 1 means
-    the window does not fit in the padded input.  The one rule the lowering and `tensor_shapes_at` size tensors by."""
+def conv_out_hw(h, w, kernel, stride, pad, dilation=1, ceil_mode=False):
+    """Output size of a conv window (torch.nn.Conv2d / MaxPool2d) on an h x w input; a size < 1 means the window does
+    not fit in the padded input.  ceil_mode: MaxPool2d(ceil_mode=True) -- the division rounds up, and a last window
+    that would start at or beyond n + pad (in the right padding) is dropped.  The one rule the lowering and
+    `tensor_shapes_at` size tensors by."""
     span = dilation * (kernel - 1) + 1
-    return (h + 2 * pad - span) // stride + 1, (w + 2 * pad - span) // stride + 1
+
+    def size(n):
+        if not ceil_mode or n + 2 * pad < span:
+            return (n + 2 * pad - span) // stride + 1
+        out = (n + 2 * pad - span + stride - 1) // stride + 1
+        return out - 1 if (out - 1) * stride >= n + pad else out
+    return size(h), size(w)
 
 
 def tensor_shapes_at(ops, capacity_shapes, in_h, in_w):
@@ -683,7 +795,7 @@ def tensor_shapes_at(ops, capacity_shapes, in_h, in_w):
         if kind in ('conv', 'dwconv'):
             hw = conv_out_hw(h, w, o['kernel'], o['stride'], o['pad'], o.get('dilation', 1))
         elif kind == 'maxpool':
-            hw = conv_out_hw(h, w, 3, o['stride'], 1)
+            hw = conv_out_hw(h, w, 3, o['stride'], 1, ceil_mode=o.get('ceil_mode', False))
         else:                               # 1x1 convs, the fused depthwise 5x5 (pad 2) -> 1x1, the heads
             hw = (h, w)
         outs = [pc[2] for pc in o['pieces']] if 'pieces' in o else [o[k] for k in ('out', 'residual', 'shuffle_src')
@@ -726,13 +838,14 @@ class _OpList:
                          'out': t})
         return t
 
-    def conv(self, t_in, e, act, residual=-1):
-        """implicit-GEMM conv of entry e; residual: a tensor added to the output before the activation"""
+    def conv(self, t_in, e, act, residual=-1, out=None):
+        """implicit-GEMM conv of entry e; residual: a tensor added to the output before the activation; out: (tensor,
+        first column) of an existing tensor to write (default: a new tensor, from column 0)"""
         n = e['w'].shape[0]
-        t = self.tensor(*self.out_hw(t_in, e), pad16(n))
+        t, off = (self.tensor(*self.out_hw(t_in, e), pad16(n)), 0) if out is None else out
         self.ops.append({'kind': 'conv', 'in': t_in, 'in_off': 0, 'c_in': e['w'].shape[1], 'kernel': e['kernel'],
                          'stride': e['stride'], 'pad': e['pad'], 'dilation': e.get('dilation', 1), 'n_out': n,
-                         'w': _f32(e['w']), 'b': _f32(e['b']), 'relu': int(act), 'out': t, 'out_off': 0,
+                         'w': _f32(e['w']), 'b': _f32(e['b']), 'relu': int(act), 'out': t, 'out_off': int(off),
                          'residual': residual, 'residual_off': 0})
         return t
 
@@ -778,12 +891,14 @@ class _OpList:
                          'n_out': len(order), 'w': w, 'b': b, 'relu': int(act), 'out': pieces[0][2],
                          'pieces': [tuple(int(v) for v in pc) for pc in pieces]})
 
-    def maxpool(self, t_in, channels, stride):
-        """3x3 max pool, padding 1"""
+    def maxpool(self, t_in, channels, stride, ceil_mode=False):
+        """3x3 max pool, padding 1; 'ceil_mode' only where it is set"""
         h, w, _ = self.tensors[t_in]
-        t = self.tensor(*conv_out_hw(h, w, 3, stride, 1), pad16(channels))
-        self.ops.append({'kind': 'maxpool', 'in': t_in, 'in_off': 0, 'channels': channels, 'stride': stride,
-                         'out': t, 'out_off': 0})
+        t = self.tensor(*conv_out_hw(h, w, 3, stride, 1, ceil_mode=ceil_mode), pad16(channels))
+        op = {'kind': 'maxpool', 'in': t_in, 'in_off': 0, 'channels': channels, 'stride': stride, 'out': t, 'out_off': 0}
+        if ceil_mode:
+            op['ceil_mode'] = True
+        self.ops.append(op)
         return t
 
     def heads(self, heads, t_in, k_cols, cols=None):
@@ -815,6 +930,8 @@ def build_ops(plan, in_h, in_w, layout=None, fuse_dw=None):
         info = _lower_resnet(L, plan, in_h, in_w)
     elif kind == 'mobilenetv2':
         info = _lower_mobilenetv2(L, plan, in_h, in_w)
+    elif kind == 'squeezenet':
+        info = _lower_squeezenet(L, plan, in_h, in_w)
     elif kind == 'heads_only':
         # in_h x in_w is the FEATURE map here; the feature tensor is filled through CompiledNet.forward_features
         c_in = int(plan['c_in'])
@@ -969,6 +1086,29 @@ def _lower_mobilenetv2(L, plan, in_h, in_w):
     return {'block_outputs': block_outputs, 'feature': (cur, _Layout(c, split=False))}
 
 
+def _lower_squeezenet(L, plan, in_h, in_w):
+    """torchvision SqueezeNet 1.1 features (eval): the stem and every Fire conv are implicit-GEMM conv ops with ReLU, the
+    pools ceil-mode max pool ops.  A Fire's two expand convs read its squeeze output and write columns [0, e1) and
+    [e1, e1 + e3) of one tensor, so torch.cat never runs."""
+    cur = L.input_conv(plan['input'], in_h, in_w, ACT_RELU)
+    c = plan['input']['w'].shape[0]
+    block_outputs = []
+    for layer in plan['layers']:
+        if layer['type'] == 'pool':
+            cur = L.maxpool(cur, c, layer['stride'], ceil_mode=layer['ceil_mode'])
+            continue
+        sq = L.conv(cur, layer['squeeze'], ACT_RELU)
+        e1, e3 = layer['expand1x1'], layer['expand3x3']
+        n1 = e1['w'].shape[0]
+        c = n1 + e3['w'].shape[0]
+        cur = L.tensor(*L.out_hw(sq, e1), pad16(c))
+        L.conv(sq, e1, ACT_RELU, out=(cur, 0))
+        L.conv(sq, e3, ACT_RELU, out=(cur, n1))
+        block_outputs.append((cur, _Layout(c, split=False)))
+    L.heads(plan['heads'], cur, c)
+    return {'block_outputs': block_outputs, 'feature': (cur, _Layout(c, split=False))}
+
+
 class CompiledNet:
     """A plan compiled to libpifpaf_b200 ops for a maximum input size and batch.  in_h, in_w is that capacity; the net
     runs at any input size up to it (`set_input_size`), each tensor packed densely in the buffer allocated for the
@@ -1075,8 +1215,8 @@ class CompiledNet:
                                                      o['out'], o['out_off'], o['residual'], o['residual_off'],
                                                      o['dilation']))
             elif o['kind'] == 'maxpool':
-                _lib.check(L.pifpaf_net_maxpool(H, o['in'], o['in_off'], o['channels'], o['stride'], o['out'],
-                                                o['out_off']))
+                _lib.check(L.pifpaf_net_maxpool_ceil(H, o['in'], o['in_off'], o['channels'], o['stride'], o['out'],
+                                                     o['out_off'], int(o.get('ceil_mode', False))))
             elif o['kind'] == 'dwconv':
                 _lib.check(L.pifpaf_net_dwconv_dilated(H, o['in'], o['in_off'], o['channels'], o['kernel'],
                                                        o['stride'], o['pad'], _ptr(o['w']), _ptr(o['b']), o['relu'],
